@@ -891,6 +891,61 @@ static void sage_scatter_block(const Tensor& dA, int64_t d, int64_t mean_col, co
   check_cuda_err("sage_scatter_block");
 }
 
+// Exact full-neighbourhood aggregation of the global rows [r0, r1) (csrc/cuda/sage_infer.cu).  `src` (bf16, indexed by
+// global id) is the source of deeper layers; without it the rows come from `feat` (bf16 or MXFP8 rows, layer 1).
+static void sage_full_aggregate(GraphHandle* graph, RowTableHandle* feat, const c10::optional<Tensor>& src,
+                                int64_t src_col, int64_t self_col, int64_t d, int64_t r0, int64_t r1, bool combine,
+                                const c10::optional<Tensor>& bias, bool relu, Tensor out) {
+  c10::cuda::CUDAGuard guard(out.device());
+  TORCH_CHECK(graph != nullptr && graph->tbl.num_parts > 0, "sage_full_aggregate: graph has no shards");
+  TORCH_CHECK(d % 8 == 0 && d >= 8 && d <= 1024, "sage_full_aggregate: d must be a multiple of 8 in [8, 1024]");
+  TORCH_CHECK(0 <= r0 && r0 <= r1 && r1 <= graph->num_rows, "sage_full_aggregate: rows [r0, r1) outside the graph");
+  TORCH_CHECK(out.is_cuda() && out.scalar_type() == torch::kBFloat16 && out.dim() == 2 && out.stride(1) == 1 &&
+              out.stride(0) % 8 == 0 && reinterpret_cast<uintptr_t>(out.data_ptr()) % 16 == 0 &&
+              out.size(0) >= r1 - r0 && out.size(1) >= (combine ? d : 2 * d),
+              "sage_full_aggregate: out must be bf16 [>= r1 - r0, >= ", combine ? "d" : "2d",
+              "] with unit inner stride and 16-byte aligned rows");
+  SageFullAggArgs a{};
+  a.g = graph->tbl;
+  a.d = static_cast<int>(d);
+  a.r0 = r0;
+  a.r1 = r1;
+  a.combine = combine ? 1 : 0;
+  a.out = out.data_ptr();
+  a.out_ld = out.stride(0);
+  if (src.has_value() && src->defined()) {
+    TORCH_CHECK(src->is_cuda() && src->scalar_type() == torch::kBFloat16 && src->dim() == 2 && src->stride(1) == 1 &&
+                src->stride(0) % 8 == 0 && reinterpret_cast<uintptr_t>(src->data_ptr()) % 16 == 0,
+                "sage_full_aggregate: src must be a bf16 CUDA table with unit inner stride and 16-byte aligned rows");
+    TORCH_CHECK(src->size(0) >= graph->num_rows, "sage_full_aggregate: src needs one row per graph node");
+    TORCH_CHECK(src_col >= 0 && src_col % 8 == 0 && src_col + d <= src->size(1) && self_col >= 0 && self_col % 8 == 0 &&
+                self_col + d <= src->size(1), "sage_full_aggregate: column blocks outside src");
+    a.src = src->data_ptr();
+    a.n_src = src->size(0);
+    a.src_ld = src->stride(0);
+    a.src_col = static_cast<int>(src_col);
+    a.self_col = static_cast<int>(self_col);
+  } else {
+    TORCH_CHECK(!combine, "sage_full_aggregate: combine reads a dense src table");
+    TORCH_CHECK(feat != nullptr, "sage_full_aggregate: needs a feature table or a src table");
+    TORCH_CHECK(feat->dtype == torch::kBFloat16 || feat->dtype == torch::kUInt8,
+                "engine features must be bf16 rows or MXFP8 (uint8) rows");
+    TORCH_CHECK(feat->dtype == torch::kBFloat16 ? feat->width == d : (feat->width == d + 16 && d == 128),
+                "feature width mismatch (MXFP8 rows are d + 16 bytes, d = 128)");
+    a.feat = feat->tbl;
+    a.feat_fp8 = feat->dtype == torch::kUInt8 ? 1 : 0;
+  }
+  if (combine && bias.has_value() && bias->defined()) {
+    TORCH_CHECK(bias->is_cuda() && bias->scalar_type() == torch::kBFloat16 && bias->numel() == d &&
+                bias->is_contiguous() && reinterpret_cast<uintptr_t>(bias->data_ptr()) % 16 == 0,
+                "sage_full_aggregate: bias must be a 16-byte aligned bf16 [d] CUDA tensor");
+    a.bias = bias->data_ptr();
+  }
+  a.relu = relu ? 1 : 0;
+  launch_sage_full_aggregate(a, cur_stream());
+  check_cuda_err("sage_full_aggregate");
+}
+
 static void add_block_f32(const Tensor& dA, int64_t col, int64_t d, const Tensor& counters, int64_t n_hops, Tensor dH) {
   c10::cuda::CUDAGuard guard(dA.device());
   TORCH_CHECK(dA.scalar_type() == torch::kBFloat16 && dA.dim() == 2 && dA.stride(1) == 1 && dA.stride(0) % 8 == 0 &&
@@ -1533,6 +1588,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   // ---- GraphSAGE engine ----
   m.def("sage_aggregate", &sage_aggregate);
   m.def("sage_scatter_bwd", &sage_scatter_bwd);
+  m.def("sage_full_aggregate", &sage_full_aggregate, py::arg("graph"), py::arg("feat"), py::arg("src"),
+        py::arg("src_col"), py::arg("self_col"), py::arg("d"), py::arg("r0"), py::arg("r1"), py::arg("combine"),
+        py::arg("bias"), py::arg("relu"), py::arg("out"));
   m.def("sage_aggregate_block", &sage_aggregate_block);
   m.def("sage_scatter_block", &sage_scatter_block);
   m.def("add_block_f32", &add_block_f32);

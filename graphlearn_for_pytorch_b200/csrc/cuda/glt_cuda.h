@@ -189,6 +189,31 @@ struct SageAggArgs {
 };
 void launch_sage_aggregate(const SageAggArgs& a, cudaStream_t s);
 
+// ---- sage_infer.cu (exact layer-wise inference over the full CSR) ---------------
+// For every global row r in [r0, r1) the mean over ALL of r's CSR neighbours (multi-edges counted with their
+// multiplicity, degree 0 -> 0), accumulated in fp32 in a fixed order and rounded once:
+//   concat  (combine = 0): out[r - r0] = bf16([mean_u x_u | x_r])                       (out width >= 2d)
+//   combine (combine = 1): out[r - r0] = bf16(act(mean_u src[u, src_col:] + src[r, self_col:] + bias))
+// Sources: the dense bf16 table `src` (row u at src + u * src_ld, ids outside [0, n_src) read as zero rows), or,
+// when src == nullptr, the feature table `feat` (bf16 rows of d elements, or MXFP8 rows with feat_fp8 = 1, d = 128).
+struct SageFullAggArgs {
+  GraphTable g;
+  RowTable feat;
+  int feat_fp8;
+  const void* src;              // bf16 [n_src, src_ld] indexed by global id, or nullptr
+  int64_t n_src, src_ld;
+  int src_col;                  // first column of the neighbour block in src
+  int self_col;                 // first column of the self block in src
+  int d;                        // width of the aggregated block (multiple of 8, <= 1024)
+  int64_t r0, r1;
+  int combine;
+  const void* bias;             // combine: bf16 [d] or nullptr
+  int relu;                     // combine: ReLU after the bias
+  void* out;                    // bf16 [r1 - r0, out_ld]
+  int64_t out_ld;
+};
+void launch_sage_full_aggregate(const SageFullAggArgs& a, cudaStream_t s);
+
 struct SageScatterArgs {
   const void* dA;               // bf16 [cap_targets, 2d]
   int d;

@@ -1,0 +1,223 @@
+// Exact layer-wise GraphSAGE inference: the neighbour mean over a node's FULL CSR row (the `fanout >= degree` limit of
+// the sampler, which takes every neighbour of a row with d <= k), for a chunk [r0, r1) of global node ids.
+//
+// Rows are reduced in a fixed order with fp32 accumulators and rounded once, without floating-point atomics, so the
+// result is bitwise identical from call to call and for any chunking.  Degrees are power-law: a row above kHubDeg is
+// not walked by one lane group while the rest of the GPU idles -- the whole CTA splits it (group g takes neighbours
+// g, g + G, ...) and the G partial sums are added in group order in shared memory.  Whether a row takes that path
+// depends on its degree alone, so the summation order of every row is fixed.
+#include "device_utils.cuh"
+#include "launch_utils.h"
+
+namespace glt {
+
+namespace {
+
+constexpr int kHubDeg = 256;
+constexpr int kInferThreads = 256;
+
+// Source row of global node u: the dense bf16 table at column src_col, or the feature table (layer 1).
+__device__ __forceinline__ const uint8_t* full_src_row(const SageFullAggArgs& a, int64_t u) {
+  if (a.src) {
+    if (u < 0 || u >= a.n_src) return nullptr;
+    return reinterpret_cast<const uint8_t*>(a.src) + (u * a.src_ld + a.src_col) * 2;
+  }
+  return row_ptr(a.feat, u);
+}
+
+// LPR lanes per row; each lane owns VPL vectors of EPV elements (8 bf16 or 16 e4m3 = 16 bytes).
+template <int LPR, int VPL, bool FP8>
+struct FullAgg {
+  static constexpr int EPV = FP8 ? 16 : 8;
+  static constexpr int R = LPR < 8 ? LPR : 8;   // LPR and R are powers of two: jj + u < LPR
+
+  // acc += x_u for neighbours j = first, first + stride, ... < deg of the row (part, start), in increasing j order.
+  __device__ static void accumulate(const SageFullAggArgs& a, int part, int64_t start, int deg, int first, int stride,
+                                    int gl, unsigned gmask, float (&acc)[VPL][EPV]) {
+    const int n = first < deg ? (deg - first + stride - 1) / stride : 0;
+    const int nvec = a.d >> 3;
+    for (int i0 = 0; i0 < n; i0 += LPR) {
+      const uint8_t* mine = nullptr;
+      if (i0 + gl < n)
+        mine = full_src_row(a, load_col(a.g, part, start + first + static_cast<int64_t>(i0 + gl) * stride));
+      const int cnt = min(LPR, n - i0);
+      // R rows in flight per lane group, accumulated in neighbour order
+      for (int jj = 0; jj < cnt; jj += R) {
+        const uint8_t* p[R];
+        uint4 raw[R][VPL];
+        uint32_t sc[R];
+#pragma unroll
+        for (int u = 0; u < R; ++u) {
+          p[u] = reinterpret_cast<const uint8_t*>(
+              __shfl_sync(gmask, reinterpret_cast<unsigned long long>(mine), jj + u, LPR));
+          if (jj + u >= cnt) p[u] = nullptr;
+          sc[u] = 0u;
+#pragma unroll
+          for (int v = 0; v < VPL; ++v) raw[u][v] = make_uint4(0, 0, 0, 0);
+        }
+#pragma unroll
+        for (int u = 0; u < R; ++u) {
+          if (p[u] == nullptr) continue;
+          if (FP8) {
+            // MXFP8 rows (d == 128): d e4m3 bytes, then the d/32 UE8M0 block scales
+            raw[u][0] = ld_nc_v4(p[u] + gl * 16);
+            sc[u] = ld_nc_u32(p[u] + a.d);
+          } else {
+#pragma unroll
+            for (int v = 0; v < VPL; ++v)
+              if (v * LPR + gl < nvec) raw[u][v] = ld_nc_v4(p[u] + (v * LPR + gl) * 16);
+          }
+        }
+#pragma unroll
+        for (int u = 0; u < R; ++u) {
+          if (p[u] == nullptr) continue;
+          if (FP8) {
+            mxfp8x16_accum(raw[u][0], sc[u], gl, acc[0]);
+          } else {
+#pragma unroll
+            for (int v = 0; v < VPL; ++v) bf16x8_accum(raw[u][v], acc[v]);
+          }
+        }
+      }
+    }
+  }
+
+  // concat: out = bf16([mean | self]);  combine: out = act(mean + src[r, self_col:] + b)
+  __device__ static void epilogue(const SageFullAggArgs& a, int64_t r, int deg, int gl, const float (&acc)[VPL][EPV]) {
+    const float inv = deg > 0 ? 1.f / static_cast<float>(deg) : 0.f;
+    uint8_t* o = reinterpret_cast<uint8_t*>(a.out) + (r - a.r0) * a.out_ld * 2;
+    if (FP8) {
+      float self[16];
+#pragma unroll
+      for (int i = 0; i < 16; ++i) self[i] = 0.f;
+      const uint8_t* sp = row_ptr(a.feat, r);
+      if (sp) mxfp8x16_accum(ld_nc_v4(sp + gl * 16), ld_nc_u32(sp + a.d), gl, self);
+      reinterpret_cast<uint4*>(o)[gl * 2] = pack_bf16x8(acc[0], inv);
+      reinterpret_cast<uint4*>(o)[gl * 2 + 1] = pack_bf16x8(acc[0] + 8, inv);
+      reinterpret_cast<uint4*>(o + a.d * 2)[gl * 2] = pack_bf16x8(self, 1.f);
+      reinterpret_cast<uint4*>(o + a.d * 2)[gl * 2 + 1] = pack_bf16x8(self + 8, 1.f);
+      return;
+    }
+    const int nvec = a.d >> 3;
+    const uint8_t* sp;
+    if (a.src)
+      sp = reinterpret_cast<const uint8_t*>(a.src) + (r * a.src_ld + a.self_col) * 2;
+    else
+      sp = row_ptr(a.feat, r);
+#pragma unroll
+    for (int v = 0; v < VPL; ++v) {
+      const int c = v * LPR + gl;
+      if (c >= nvec) continue;
+      const uint4 sv = sp ? ld_nc_v4(sp + c * 16) : make_uint4(0, 0, 0, 0);
+      if (!a.combine) {
+        reinterpret_cast<uint4*>(o)[c] = pack_bf16x8(acc[v], inv);
+        reinterpret_cast<uint4*>(o + a.d * 2)[c] = sv;
+      } else {
+        float z[8], b[8];
+#pragma unroll
+        for (int i = 0; i < 8; ++i) z[i] = b[i] = 0.f;
+        bf16x8_accum(sv, z);
+        if (a.bias) bf16x8_accum(reinterpret_cast<const uint4*>(a.bias)[c], b);
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          z[i] += acc[v][i] * inv + b[i];
+          if (a.relu) z[i] = fmaxf(z[i], 0.f);
+        }
+        reinterpret_cast<uint4*>(o)[c] = pack_bf16x8(z, 1.f);
+      }
+    }
+  }
+};
+
+// One row per lane group (G = 256 / LPR rows per CTA); rows above kHubDeg are queued and reduced by the whole CTA.
+template <int LPR, int VPL, bool FP8>
+__global__ void __launch_bounds__(kInferThreads) k_sage_full_aggregate(SageFullAggArgs a) {
+  using K = FullAgg<LPR, VPL, FP8>;
+  constexpr int EPV = K::EPV;
+  constexpr int G = kInferThreads / LPR;
+  extern __shared__ float s_part[];    // [G][d] partial sums of a hub row
+  __shared__ int64_t s_hub[G];
+  __shared__ int s_nhub;
+  pdl_enter();
+  const int lane = threadIdx.x & 31;
+  const int gl = lane % LPR;
+  const int g = threadIdx.x / LPR;
+  const unsigned gmask = (LPR == 32) ? 0xffffffffu : (((1u << LPR) - 1u) << ((lane / LPR) * LPR));
+  if (threadIdx.x == 0) s_nhub = 0;
+  __syncthreads();
+
+  const int64_t r = a.r0 + static_cast<int64_t>(blockIdx.x) * G + g;
+  float acc[VPL][EPV];
+#pragma unroll
+  for (int v = 0; v < VPL; ++v)
+#pragma unroll
+    for (int i = 0; i < EPV; ++i) acc[v][i] = 0.f;
+  if (r < a.r1) {
+    const RowRef rr = load_row(a.g, r);
+    if (rr.deg > kHubDeg) {
+      if (gl == 0) s_hub[atomicAdd(&s_nhub, 1)] = r;
+    } else {
+      if (rr.deg > 0) K::accumulate(a, rr.part, rr.start, rr.deg, 0, 1, gl, gmask, acc);
+      K::epilogue(a, r, rr.deg, gl, acc);
+    }
+  }
+  __syncthreads();
+  const int nhub = s_nhub;
+  for (int h = 0; h < nhub; ++h) {
+    const int64_t hr = s_hub[h];
+    const RowRef rr = load_row(a.g, hr);
+#pragma unroll
+    for (int v = 0; v < VPL; ++v)
+#pragma unroll
+      for (int i = 0; i < EPV; ++i) acc[v][i] = 0.f;
+    K::accumulate(a, rr.part, rr.start, rr.deg, g, G, gl, gmask, acc);
+#pragma unroll
+    for (int v = 0; v < VPL; ++v) {
+      const int col = (v * LPR + gl) * EPV;
+      if (col < a.d)
+#pragma unroll
+        for (int i = 0; i < EPV; ++i) s_part[g * a.d + col + i] = acc[v][i];
+    }
+    __syncthreads();
+    if (g == 0) {
+#pragma unroll
+      for (int v = 0; v < VPL; ++v) {
+        const int col = (v * LPR + gl) * EPV;
+        if (col >= a.d) continue;
+#pragma unroll
+        for (int i = 0; i < EPV; ++i) {
+          float s = 0.f;
+#pragma unroll 1
+          for (int q = 0; q < G; ++q) s += s_part[q * a.d + col + i];
+          acc[v][i] = s;
+        }
+      }
+      K::epilogue(a, hr, rr.deg, gl, acc);
+    }
+    __syncthreads();
+  }
+}
+
+template <int LPR, int VPL, bool FP8>
+void launch_full(const SageFullAggArgs& a, cudaStream_t s) {
+  constexpr int G = kInferThreads / LPR;
+  const int64_t blocks = (a.r1 - a.r0 + G - 1) / G;
+  launch_k(k_sage_full_aggregate<LPR, VPL, FP8>, dim3(static_cast<unsigned>(blocks)), dim3(kInferThreads),
+           sizeof(float) * G * a.d, s, a);
+}
+
+}  // namespace
+
+void launch_sage_full_aggregate(const SageFullAggArgs& a, cudaStream_t s) {
+  if (a.r1 <= a.r0) return;
+  if (a.feat_fp8) { launch_full<8, 1, true>(a, s); return; }
+  const int nvec = a.d / 8;
+  if (nvec <= 4) launch_full<4, 1, false>(a, s);
+  else if (nvec <= 8) launch_full<8, 1, false>(a, s);
+  else if (nvec <= 16) launch_full<16, 1, false>(a, s);
+  else if (nvec <= 32) launch_full<32, 1, false>(a, s);
+  else if (nvec <= 64) launch_full<32, 2, false>(a, s);
+  else launch_full<32, 4, false>(a, s);
+}
+
+}  // namespace glt

@@ -949,3 +949,67 @@ class GraphSageEngine(object):
     self._sample()
     self._forward(train=False)
     return float(self.loss.item()), int(self.correct.item()), int(self.arena.counters[1].item())
+
+  def _project_first(self, l: int) -> bool:
+    """Layer l >= 2 projects before it aggregates when it narrows the width: the neighbour rows it gathers are then
+    dims_out wide instead of dims_in (DESIGN.md, "SURVEY §7.4 hard parts", row 2).  Layer 1 always aggregates first:
+    its rows come from the feature table in place."""
+    return l >= 2 and self.dims_out[l - 1] < self.dims_in[l - 1]
+
+  @torch.no_grad()
+  def inference(self, chunk_rows: Optional[int] = None) -> torch.Tensor:
+    """Exact layer-wise full-neighbourhood inference: bf16 logits [num_nodes, num_classes] of every node.
+
+    Every layer aggregates each node's complete CSR row (the `fanout >= degree` limit of training; what the
+    reference's examples evaluate with, `SAGE.inference` over `sizes=[-1]`).  Aggregate-first layers run
+    `sage_full_aggregate` (concat) over chunks of `chunk_rows` nodes into an A chunk, then the TcGemm forward of the
+    layer; project-first layers run one TcGemm over the whole table, P = H . [W_neigh ; W_self]^T, then
+    `sage_full_aggregate` (combine).  Uses the bf16 parameters of the training forward, applies no dropout, and runs
+    on the current stream, so it sees every step queued before it.  The activation tables live for the call only;
+    arenas, captured graphs, gradients and optimizer state are not touched.  `chunk_rows=None` sizes the chunk from
+    free device memory.  The result is bitwise identical for any chunk size.
+
+    Not collective: with several GPUs every rank maps all shards and reads peer rows in place."""
+    nat, dev, bf = self.nat, self.device, torch.bfloat16
+    N, L = self._num_nodes, self.L
+    with torch.cuda.device(dev):
+      wide = max(self.dims_out)
+      bufs = [torch.empty(N, wide, dtype=bf, device=dev) for _ in range(2 if L > 1 else 1)]
+      agg_dims = [self.dims_in[l - 1] for l in range(1, L + 1) if not self._project_first(l)]
+      a_row = 2 * max(agg_dims)
+      if chunk_rows is None:
+        free, _ = torch.cuda.mem_get_info(dev)
+        chunk_rows = max(4096, min(1 << 19, free // 4 // (a_row * 2)))
+      chunk_rows = max(1, min(int(chunk_rows), N))
+      A = torch.empty(chunk_rows, a_row, dtype=bf, device=dev)
+      rows_dev = torch.tensor([chunk_rows, N], dtype=torch.int32, device=dev)   # TcGemm row counts (device-side)
+      H = None
+      for l in range(1, L + 1):
+        out = bufs[(l - 1) % len(bufs)][:, :self.dims_out[l - 1]]
+        self._infer_layer(l, H, out, A, rows_dev, chunk_rows)
+        H = out
+      return H[:, :self.C].contiguous()
+
+  def _infer_layer(self, l: int, H: Optional[torch.Tensor], out: torch.Tensor, A: torch.Tensor,
+                   rows_dev: torch.Tensor, chunk_rows: int):
+    """out = layer l of the full-neighbourhood forward over every node; H = the layer's input table (None: features)."""
+    nat, N = self.nat, self._num_nodes
+    d, n = self.dims_in[l - 1], self.dims_out[l - 1]
+    relu = l < self.L
+    if self._project_first(l):
+      W = self.W(l)
+      P = torch.empty(N, 2 * n, dtype=torch.bfloat16, device=self.device)
+      g = nat.TcGemm(self.device.index)
+      g.add_forward(H, torch.cat([W[:, :d], W[:, d:]], 0), None, False, P, rows_dev, 1)
+      g.run()
+      for r0 in range(0, N, chunk_rows):
+        r1 = min(N, r0 + chunk_rows)
+        nat.sage_full_aggregate(self.gh, None, P, 0, n, n, r0, r1, True, self.b(l), relu, out[r0:r1])
+      return
+    for r0 in range(0, N, chunk_rows):
+      r1 = min(N, r0 + chunk_rows)
+      a = A[:r1 - r0, :2 * d]
+      nat.sage_full_aggregate(self.gh, self.feat if l == 1 else None, H, 0, 0, d, r0, r1, False, None, False, a)
+      g = nat.TcGemm(self.device.index)
+      g.add_forward(a, self.W(l), self.b(l), relu, out[r0:r1], rows_dev, 0)
+      g.run()

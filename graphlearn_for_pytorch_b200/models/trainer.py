@@ -23,6 +23,7 @@ class GraphSageTrainer(object):
                hidden: int = 256, num_classes: int = 47, lr: float = 3e-3, weight_decay: float = 0.0, seed: int = 0,
                device: Optional[torch.device] = None):
     self.device = torch.device(device) if device is not None else torch.device('cpu')
+    self.graph = graph
     self.features, self.labels = features, labels.to(self.device)
     self.fanouts = list(fanouts)
     self.sampler = NeighborSampler(graph, self.fanouts, device=self.device, seed=seed)
@@ -61,6 +62,32 @@ class GraphSageTrainer(object):
     x, ei, nn_, ne_, y, n = self._batch(seeds)
     logits = self.model(x, ei, nn_, ne_)[:n]
     return float(F.cross_entropy(logits, y)), int((logits.argmax(1) == y).sum()), int(n)
+
+  @torch.no_grad()
+  def inference(self, chunk_rows: int = 65536) -> torch.Tensor:
+    """Exact layer-wise full-neighbourhood inference: fp32 logits [num_nodes, num_classes] of every node, computed
+    layer by layer with the model's `SAGEConv`s over every node's complete CSR row, `chunk_rows` target nodes at a
+    time -- the same result as `GraphSageEngine.inference()` (which rounds to bf16 where the engine stores bf16)."""
+    self.model.eval()
+    topo = self.graph.topo
+    if topo is None:
+      raise ValueError('inference() needs the graph topology (a Graph built from a Topology)')
+    indptr, indices = topo.indptr.to(self.device), topo.indices.to(self.device)
+    n = indptr.numel() - 1
+    ids = torch.arange(n)
+    x = self.features[ids] if not isinstance(self.features, torch.Tensor) else self.features[:n]
+    x = x.to(self.device, dtype=torch.float32)
+    convs = self.model.convs
+    for i, conv in enumerate(convs):
+      out = torch.empty(n, conv.lin_l.out_features, device=self.device)
+      for r0 in range(0, n, chunk_rows):
+        r1 = min(n, r0 + chunk_rows)
+        e0, e1 = int(indptr[r0]), int(indptr[r1])
+        deg = indptr[r0 + 1:r1 + 1] - indptr[r0:r1]
+        dst = torch.repeat_interleave(torch.arange(r1 - r0, device=self.device), deg)
+        out[r0:r1] = conv((x, x[r0:r1]), torch.stack([indices[e0:e1].long(), dst]), r1 - r0)
+      x = torch.relu(out) if i < len(convs) - 1 else out
+    return x
 
   def flush(self):          # API compatibility with the pipelined engine
     return None
