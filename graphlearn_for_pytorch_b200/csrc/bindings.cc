@@ -998,7 +998,7 @@ static void sage_gather_bwd(const Tensor& dA, int64_t d, SamplerArena& ar, int64
 }
 
 static void relu_bwd_cast(const Tensor& dH, const Tensor& Z, const Tensor& counters, int64_t n_hops,
-                          Tensor dPre, const c10::optional<Tensor>& colsum, bool prezeroed, double gscale) {
+                          Tensor dPre, const c10::optional<Tensor>& colsum, bool prezeroed, double gscale, bool relu) {
   c10::cuda::CUDAGuard guard(dH.device());
   TORCH_CHECK(dPre.size(0) <= dH.size(0) && dPre.size(0) <= Z.size(0) && dPre.size(1) % 8 == 0);
   TORCH_CHECK(dH.scalar_type() == torch::kFloat32 && Z.scalar_type() == torch::kBFloat16 &&
@@ -1008,8 +1008,61 @@ static void relu_bwd_cast(const Tensor& dH, const Tensor& Z, const Tensor& count
   launch_relu_bwd_cast(dH.data_ptr<float>(), Z.data_ptr(), counters.data_ptr<int32_t>(), n_hops,
                        dPre.size(0), dPre.size(1), dPre.data_ptr(),
                        (colsum.has_value() && colsum->defined()) ? colsum->data_ptr<float>() : nullptr, cur_stream(),
-                       prezeroed, static_cast<float>(gscale));
+                       prezeroed, static_cast<float>(gscale), relu);
   check_cuda_err("relu_bwd_cast");
+}
+
+// Link-prediction seeds of one batch (cuda/link.cu): pos int64 [2, B] -> seeds int64 [2 (1 + k) B], n_pairs int32.
+// `step` is the arena's device step, read before the arena's sample() advances it.
+static void link_seeds(GraphHandle* graph, const Tensor& pos, int64_t num_nodes, int64_t neg_ratio, int64_t seed,
+                       const Tensor& step, Tensor seeds, Tensor n_pairs) {
+  c10::cuda::CUDAGuard guard(seeds.device());
+  TORCH_CHECK(graph != nullptr && graph->tbl.num_parts > 0, "link_seeds: graph has no shards");
+  TORCH_CHECK(pos.is_cuda() && pos.scalar_type() == torch::kInt64 && pos.is_contiguous() && pos.dim() == 2 &&
+              pos.size(0) == 2, "link_seeds: pos must be a contiguous int64 [2, B] CUDA tensor");
+  TORCH_CHECK(neg_ratio >= 1, "link_seeds: neg_ratio must be >= 1");
+  TORCH_CHECK(num_nodes >= 1 && num_nodes <= graph->num_rows && num_nodes < (1LL << 32),
+              "link_seeds: num_nodes must be in [1, graph rows] and < 2^32");
+  const int64_t B = pos.size(1), P = (1 + neg_ratio) * B;
+  TORCH_CHECK(P < (1LL << 30), "link_seeds: batch too large");
+  TORCH_CHECK(seeds.is_cuda() && seeds.scalar_type() == torch::kInt64 && seeds.is_contiguous() &&
+              seeds.numel() == 2 * P, "link_seeds: seeds must be a contiguous int64 [2 (1 + k) B] CUDA tensor");
+  TORCH_CHECK(step.is_cuda() && step.scalar_type() == torch::kInt32 && step.numel() >= 1, "link_seeds: int32 step");
+  TORCH_CHECK(n_pairs.is_cuda() && n_pairs.scalar_type() == torch::kInt32 && n_pairs.numel() >= 1,
+              "link_seeds: int32 n_pairs");
+  launch_link_seeds(graph->tbl, pos.data_ptr<int64_t>(), static_cast<int>(B), static_cast<int>(neg_ratio), num_nodes,
+                    static_cast<uint64_t>(seed), step.data_ptr<int32_t>(), seeds.data_ptr<int64_t>(),
+                    n_pairs.data_ptr<int32_t>(), cur_stream());
+  check_cuda_err("link_seeds");
+}
+
+// Fused edge loss of a link batch (cuda/link.cu) over the embeddings Z (bf16 [rows, ld], first C columns real).
+static void link_bce(const Tensor& Z, int64_t C, const Tensor& seed_local, int64_t P, int64_t B, const Tensor& n_pairs,
+                     Tensor loss, const c10::optional<Tensor>& correct, const c10::optional<Tensor>& dZ) {
+  c10::cuda::CUDAGuard guard(Z.device());
+  TORCH_CHECK(Z.is_cuda() && Z.scalar_type() == torch::kBFloat16 && Z.is_contiguous() && Z.dim() == 2,
+              "link_bce: Z must be a contiguous bf16 [rows, ld] CUDA tensor");
+  TORCH_CHECK(C % 8 == 0 && C >= 8 && C <= 512 && C <= Z.size(1) && Z.size(1) % 8 == 0,
+              "link_bce: C must be a multiple of 8 in [8, 512] and <= Z's width");
+  TORCH_CHECK(0 <= B && B <= P && seed_local.is_cuda() && seed_local.scalar_type() == torch::kInt32 &&
+              seed_local.numel() >= 2 * P, "link_bce: seed_local must be int32 [>= 2P]");
+  TORCH_CHECK(n_pairs.is_cuda() && n_pairs.scalar_type() == torch::kInt32 && n_pairs.numel() >= 1);
+  TORCH_CHECK(loss.is_cuda() && loss.scalar_type() == torch::kFloat32 && loss.numel() >= 1);
+  int32_t* corr = nullptr;
+  if (correct.has_value() && correct->defined()) {
+    TORCH_CHECK(correct->is_cuda() && correct->scalar_type() == torch::kInt32 && correct->numel() >= 1);
+    corr = correct->data_ptr<int32_t>();
+  }
+  float* dz = nullptr;
+  if (dZ.has_value() && dZ->defined()) {
+    TORCH_CHECK(dZ->is_cuda() && dZ->scalar_type() == torch::kFloat32 && dZ->is_contiguous() &&
+                dZ->sizes() == Z.sizes(), "link_bce: dZ must be a contiguous fp32 tensor of Z's shape");
+    dz = dZ->data_ptr<float>();
+  }
+  launch_link_bce(Z.data_ptr(), static_cast<int>(Z.size(1)), static_cast<int>(C), seed_local.data_ptr<int32_t>(),
+                  static_cast<int>(P), static_cast<int>(B), n_pairs.data_ptr<int32_t>(), loss.data_ptr<float>(), corr,
+                  dz, cur_stream());
+  check_cuda_err("link_bce");
 }
 
 static void dropout_bf16(Tensor Z, const Tensor& counters, int64_t n_hops, double p, int64_t seed, int64_t layer,
@@ -1595,7 +1648,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("sage_scatter_block", &sage_scatter_block);
   m.def("add_block_f32", &add_block_f32);
   m.def("relu_bwd_cast", &relu_bwd_cast, py::arg("dH"), py::arg("Z"), py::arg("counters"), py::arg("n_hops"),
-        py::arg("dPre"), py::arg("colsum"), py::arg("prezeroed") = false, py::arg("gscale") = 1.0);
+        py::arg("dPre"), py::arg("colsum"), py::arg("prezeroed") = false, py::arg("gscale") = 1.0,
+        py::arg("relu") = true);
+  m.def("link_seeds", &link_seeds, py::arg("graph"), py::arg("pos"), py::arg("num_nodes"), py::arg("neg_ratio"),
+        py::arg("seed"), py::arg("step"), py::arg("seeds"), py::arg("n_pairs"));
+  m.def("link_bce", &link_bce, py::arg("Z"), py::arg("C"), py::arg("seed_local"), py::arg("P"), py::arg("B"),
+        py::arg("n_pairs"), py::arg("loss"), py::arg("correct"), py::arg("dZ"));
   m.def("dropout_bf16", &dropout_bf16, py::arg("Z"), py::arg("counters"), py::arg("n_hops"), py::arg("p"),
         py::arg("seed"), py::arg("layer"), py::arg("step_dev") = py::none());
   m.def("zero_grads", &zero_grads);

@@ -88,6 +88,19 @@ __device__ __forceinline__ int64_t load_col(const GraphTable& g, int part, int64
   return __ldg(reinterpret_cast<const int64_t*>(g.parts[part].indices) + pos);
 }
 
+// Strict edge test: is c a neighbour of r?  Binary search of r's row (rows are column-sorted, Topology guarantees it).
+__device__ __forceinline__ bool edge_exists(const GraphTable& g, int64_t r, int64_t c) {
+  const RowRef row = load_row(g, r);
+  int64_t lo = 0, hi = row.deg;
+  while (lo < hi) {
+    const int64_t mid = (lo + hi) >> 1;
+    const int64_t x = load_col(g, row.part, row.start + mid);
+    if (x == c) return true;
+    if (x < c) lo = mid + 1; else hi = mid;
+  }
+  return false;
+}
+
 __device__ __forceinline__ unsigned lanemask_lt() {
   unsigned m;
   asm volatile("mov.u32 %0, %%lanemask_lt;" : "=r"(m));

@@ -279,11 +279,11 @@ struct SageGatherBwdArgs {
 // Replaces zero_rows + sage_scatter_bwd (fp32 atomics) + relu_bwd_cast.
 void launch_sage_gather_bwd(const SageGatherBwdArgs& a, cudaStream_t s);
 
-// dPre = (Z > 0) ? bf16(dH) : 0 for rows < cum[n_hops]; 0 beyond.
+// dPre = (Z > 0) ? bf16(dH) : 0 for rows < cum[n_hops]; 0 beyond.  relu = false: dPre = bf16(dH), Z is not read.
 // colsum (optional, fp32 [d]): fused bias gradient = column sums of dPre.
 void launch_relu_bwd_cast(const float* dH, const void* Z, const int32_t* cum, int n_hops, int cap,
                           int d, void* dPre, float* colsum, cudaStream_t s, bool prezeroed = false,
-                          float gscale = 1.f);
+                          float gscale = 1.f, bool relu = true);
 // In-place inverted dropout (keep prob 1-p, kept values scaled by 1/(1-p)) on rows < cum[n_hops] of bf16 Z[cap, d];
 // mask = Philox(seed, layer, *step_dev, element).  Backward: launch_relu_bwd_cast(..., gscale = 1/(1-p)) on the
 // post-dropout Z.
@@ -309,6 +309,19 @@ void launch_adam(float* p, const float* g, float* m, float* v, void* p_bf16, int
                  float b1, float b2, float eps, float wd, int32_t* step_dev, float gscale,
                  cudaStream_t s);
 void launch_bf16_to_f32(const void* src, float* dst, int64_t n, cudaStream_t s);
+
+// ---- link.cu (link-prediction step: in-graph negatives + fused edge loss) --------
+// pos: int64 [2, B] positive pairs (-1 = padding).  Writes seeds [2P], P = (1 + k) B: seeds[p] = source and
+// seeds[P + p] = destination of pair p; pairs [0, B) are pos, pair B + i k + j is the j-th negative of positive i,
+// uniform over [0, num_nodes)^2 and redrawn (up to 5 draws) while it is an edge of g, keyed by Philox
+// (seed, a stream no sampling kernel uses, *step_dev, p).  *n_pairs = (1 + k) x #valid positives.
+void launch_link_seeds(GraphTable g, const int64_t* pos, int B, int k, int64_t num_nodes, uint64_t seed,
+                       const int32_t* step_dev, int64_t* seeds, int32_t* n_pairs, cudaStream_t s);
+// Mean BCE-with-logits over the pairs p < P with seed_local[p], seed_local[P + p] >= 0: logit = dot of the first C
+// columns of those rows of Z (bf16 [rows, ld]), label = (p < B).  Adds into *loss / *correct (pre-zeroed) and, when
+// dZ (fp32 [rows, ld], pre-zeroed) is given, the logit gradients of both endpoints with fp32 red.add.
+void launch_link_bce(const void* Z, int ld, int C, const int32_t* seed_local, int P, int B, const int32_t* n_pairs,
+                     float* loss, int32_t* correct, float* dZ, cudaStream_t s);
 
 // ---- peer.cu (collectives over NVLink peer memory, CUDA-graph capturable) ------
 struct PeerPtrs {

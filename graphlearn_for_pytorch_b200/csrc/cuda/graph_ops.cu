@@ -10,18 +10,6 @@ namespace glt {
 
 namespace {
 
-__device__ __forceinline__ bool edge_exists(const GraphTable& g, int64_t r, int64_t c) {
-  const RowRef row = load_row(g, r);
-  int64_t lo = 0, hi = row.deg;
-  while (lo < hi) {  // rows are column-sorted (Topology guarantees it)
-    const int64_t mid = (lo + hi) >> 1;
-    const int64_t x = load_col(g, row.part, row.start + mid);
-    if (x == c) return true;
-    if (x < c) lo = mid + 1; else hi = mid;
-  }
-  return false;
-}
-
 // Fused draw + reject + compaction (warp ballot + one atomic per warp); the
 // reference needs a kernel plus Thrust copy_if/gather/reduce passes
 // (csrc/cuda/random_negative_sampler.cu:95-160).

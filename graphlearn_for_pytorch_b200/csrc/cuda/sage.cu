@@ -150,11 +150,12 @@ __global__ void __launch_bounds__(256) k_sage_scatter_bwd(SageScatterArgs a) {
 
 __global__ void __launch_bounds__(256) k_relu_bwd_cast(const float* dH, const __nv_bfloat16* Z, const int32_t* cum,
                                                        int n_hops, int cap, int d, __nv_bfloat16* dPre,
-                                                       float* colsum, float gscale) {
+                                                       float* colsum, float gscale, int relu) {
   pdl_enter();
   // gscale: 1/(1-p) when Z is the post-dropout activation (dropped elements are 0 there, so the ReLU test also
   // masks them).  colsum != nullptr: also accumulate the bias gradient (column sums of dPre).  Requires
-  // d | 2048 so that a thread keeps the same 8 columns across grid-stride iterations.
+  // d | 2048 so that a thread keeps the same 8 columns across grid-stride iterations.  relu == 0: no mask, Z is
+  // not read (a layer without activation).
   __shared__ float s_acc[256][8];
   const int T = min(cum[n_hops], cap);
   const int64_t n8 = static_cast<int64_t>(cap) * d / 8;
@@ -172,8 +173,12 @@ __global__ void __launch_bounds__(256) k_relu_bwd_cast(const float* dH, const __
       float g[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
       float z[8];
 #pragma unroll
-      for (int q = 0; q < 8; ++q) z[q] = 0.f;
-      bf16x8_accum(*reinterpret_cast<const uint4*>(Z + e), z);
+      for (int q = 0; q < 8; ++q) z[q] = 1.f;
+      if (relu) {
+#pragma unroll
+        for (int q = 0; q < 8; ++q) z[q] = 0.f;
+        bf16x8_accum(*reinterpret_cast<const uint4*>(Z + e), z);
+      }
 #pragma unroll
       for (int q = 0; q < 8; ++q) g[q] = z[q] > 0.f ? g[q] * gscale : 0.f;
       o = pack_bf16x8(g, 1.f);
@@ -478,12 +483,12 @@ void launch_dropout_bf16(void* Z, const int32_t* cum, int n_hops, int cap, int d
 }
 
 void launch_relu_bwd_cast(const float* dH, const void* Z, const int32_t* cum, int n_hops, int cap,
-                          int d, void* dPre, float* colsum, cudaStream_t s, bool prezeroed, float gscale) {
+                          int d, void* dPre, float* colsum, cudaStream_t s, bool prezeroed, float gscale, bool relu) {
   if (colsum && (2048 % d != 0)) colsum = nullptr;  // caller falls back to launch_colsum_bf16
   if (colsum && !prezeroed) cudaMemsetAsync(colsum, 0, sizeof(float) * d, s);
   launch_k(k_relu_bwd_cast, dim3(grid_for(static_cast<int64_t>(cap) * d / 8, 256 * 2, 132 * 4)), dim3(256), 0, s,
            dH, reinterpret_cast<const __nv_bfloat16*>(Z), cum, n_hops, cap, d,
-           reinterpret_cast<__nv_bfloat16*>(dPre), colsum, gscale);
+           reinterpret_cast<__nv_bfloat16*>(dPre), colsum, gscale, relu ? 1 : 0);
 }
 
 void launch_bias_relu(void* Z, const void* bias, const int32_t* cum, int n_hops, int cap, int d,

@@ -1,5 +1,6 @@
 from .sage import SAGEConv, GraphSAGE, GraphSageEngine
-from .trainer import GraphSageTrainer
+from .sage_link import GraphSageLinkEngine, link_auc
+from .trainer import GraphSageTrainer, GraphSageLinkTrainer
 from .rgnn import RGNN, RelSAGEConv, RelGCNConv, RelGATConv
 from .seal import drnl_node_labeling, DGCNN
 from .hgt import HGT, HGTConv
