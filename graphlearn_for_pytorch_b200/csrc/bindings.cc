@@ -789,6 +789,12 @@ static void fill_ell(const std::vector<Tensor>& ell, const std::vector<int64_t>&
   for (size_t i = 0; i < ell.size(); ++i) { out_ell[i] = ell[i].data_ptr<int32_t>(); out_k[i] = ks[i]; }
 }
 
+// The aggregation / scatter kernels cover at most 128 16-byte vectors per row (csrc/cuda/sage.cu, GLT_DISPATCH_WIDTH).
+// `msg` is one string: a TORCH_CHECK message assembled from several arguments crashes this extension when thrown.
+static void check_sage_width(int64_t d, const char* msg) {
+  TORCH_CHECK(d % 8 == 0 && d >= 8 && d <= 1024, msg);
+}
+
 static SageAggArgs make_agg(RowTableHandle* feat, const c10::optional<Tensor>& nodes,
                             const c10::optional<Tensor>& src_local, int64_t d, const Tensor& counters,
                             int64_t n_hops_targets, int64_t cap_targets, const std::vector<Tensor>& ell,
@@ -822,6 +828,7 @@ static void sage_aggregate(RowTableHandle* feat, const c10::optional<Tensor>& no
                            int64_t n_hops_targets, const std::vector<Tensor>& ell,
                            const std::vector<int64_t>& ks, const Tensor& deg, Tensor out) {
   c10::cuda::CUDAGuard guard(out.device());
+  check_sage_width(d, "sage_aggregate: d must be a multiple of 8 in [8, 1024]");
   TORCH_CHECK(out.scalar_type() == torch::kBFloat16 && out.is_contiguous() && out.size(1) == 2 * d);
   TORCH_CHECK(feat == nullptr || (src_local.has_value() && src_local->defined()) || feat->dtype == torch::kBFloat16,
               "the unfused aggregation kernel reads bf16 rows; MXFP8 tables go through sage_fused");
@@ -835,6 +842,7 @@ static void sage_scatter_bwd(const Tensor& dA, int64_t d, const Tensor& counters
                              const std::vector<Tensor>& ell, const std::vector<int64_t>& ks,
                              const Tensor& deg, Tensor dH) {
   c10::cuda::CUDAGuard guard(dA.device());
+  check_sage_width(d, "sage_scatter_bwd: d must be a multiple of 8 in [8, 1024]");
   TORCH_CHECK(dA.scalar_type() == torch::kBFloat16 && dA.is_contiguous() && dA.size(1) == 2 * d);
   TORCH_CHECK(dH.scalar_type() == torch::kFloat32 && dH.is_contiguous() && dH.size(1) == d);
   SageScatterArgs a{};
@@ -857,6 +865,7 @@ static void sage_aggregate_block(RowTableHandle* feat, const c10::optional<Tenso
                                  int64_t n_hops_targets, const std::vector<Tensor>& ell,
                                  const std::vector<int64_t>& ks, const Tensor& deg, Tensor out, int64_t mean_col) {
   c10::cuda::CUDAGuard guard(out.device());
+  check_sage_width(d, "sage_aggregate_block: d must be a multiple of 8 in [8, 1024]");
   TORCH_CHECK(out.scalar_type() == torch::kBFloat16 && out.dim() == 2 && out.stride(1) == 1 &&
               mean_col >= 0 && mean_col % 8 == 0 && mean_col + d <= out.size(1) && out.stride(0) % 8 == 0);
   SageAggArgs a = make_agg(feat, nodes, src_local, d, counters, n_hops_targets, out.size(0), ell, ks,
@@ -872,6 +881,7 @@ static void sage_scatter_block(const Tensor& dA, int64_t d, int64_t mean_col, co
                                int64_t n_hops_targets, const std::vector<Tensor>& ell,
                                const std::vector<int64_t>& ks, const Tensor& deg, Tensor dH) {
   c10::cuda::CUDAGuard guard(dA.device());
+  check_sage_width(d, "sage_scatter_block: d must be a multiple of 8 in [8, 1024]");
   TORCH_CHECK(dA.scalar_type() == torch::kBFloat16 && dA.dim() == 2 && dA.stride(1) == 1 && dA.stride(0) % 8 == 0 &&
               mean_col >= 0 && mean_col % 8 == 0 && mean_col + d <= dA.size(1));
   TORCH_CHECK(dH.scalar_type() == torch::kFloat32 && dH.is_contiguous() && dH.size(1) == d);
@@ -997,19 +1007,24 @@ static void sage_gather_bwd(const Tensor& dA, int64_t d, SamplerArena& ar, int64
   check_cuda_err("sage_gather_bwd");
 }
 
-static void relu_bwd_cast(const Tensor& dH, const Tensor& Z, const Tensor& counters, int64_t n_hops,
-                          Tensor dPre, const c10::optional<Tensor>& colsum, bool prezeroed, double gscale, bool relu) {
+// Returns the number of kernels launched (2 when the bias gradient takes a separate column-sum pass).
+static int64_t relu_bwd_cast(const Tensor& dH, const Tensor& Z, const Tensor& counters, int64_t n_hops,
+                             Tensor dPre, const c10::optional<Tensor>& colsum, bool prezeroed, double gscale, bool relu) {
   c10::cuda::CUDAGuard guard(dH.device());
   TORCH_CHECK(dPre.size(0) <= dH.size(0) && dPre.size(0) <= Z.size(0) && dPre.size(1) % 8 == 0);
   TORCH_CHECK(dH.scalar_type() == torch::kFloat32 && Z.scalar_type() == torch::kBFloat16 &&
               dPre.scalar_type() == torch::kBFloat16, "relu_bwd_cast: dH fp32, Z/dPre bf16");
   TORCH_CHECK(dH.is_contiguous() && Z.is_contiguous() && dPre.is_contiguous() && dH.size(1) == dPre.size(1) &&
               Z.size(1) == dPre.size(1), "relu_bwd_cast: contiguous [rows, d] operands of equal width");
-  launch_relu_bwd_cast(dH.data_ptr<float>(), Z.data_ptr(), counters.data_ptr<int32_t>(), n_hops,
-                       dPre.size(0), dPre.size(1), dPre.data_ptr(),
-                       (colsum.has_value() && colsum->defined()) ? colsum->data_ptr<float>() : nullptr, cur_stream(),
-                       prezeroed, static_cast<float>(gscale), relu);
+  const bool has_colsum = colsum.has_value() && colsum->defined();
+  TORCH_CHECK(!has_colsum || (colsum->scalar_type() == torch::kFloat32 && colsum->is_contiguous() &&
+                              colsum->numel() == dPre.size(1)), "relu_bwd_cast: colsum must be fp32 [d]");
+  const int n = launch_relu_bwd_cast(dH.data_ptr<float>(), Z.data_ptr(), counters.data_ptr<int32_t>(), n_hops,
+                                     dPre.size(0), dPre.size(1), dPre.data_ptr(),
+                                     has_colsum ? colsum->data_ptr<float>() : nullptr, cur_stream(),
+                                     prezeroed, static_cast<float>(gscale), relu);
   check_cuda_err("relu_bwd_cast");
+  return n;
 }
 
 // Link-prediction seeds of one batch (cuda/link.cu): pos int64 [2, B] -> seeds int64 [2 (1 + k) B], n_pairs int32.
@@ -1090,7 +1105,8 @@ static void bias_relu(Tensor Z, const Tensor& bias, const Tensor& counters, int6
   check_cuda_err("bias_relu");
 }
 
-static void softmax_nll(const Tensor& logits, int64_t C, const c10::optional<Tensor>& y,
+// Returns the number of kernels launched (2 when the bias gradient takes a separate column-sum pass).
+static int64_t softmax_nll(const Tensor& logits, int64_t C, const c10::optional<Tensor>& y,
                         const c10::optional<Tensor>& labels_all, const c10::optional<Tensor>& nodes,
                         const Tensor& counters, Tensor loss, Tensor dlogits,
                         const c10::optional<Tensor>& correct, const c10::optional<Tensor>& colsum, bool prezeroed) {
@@ -1099,15 +1115,20 @@ static void softmax_nll(const Tensor& logits, int64_t C, const c10::optional<Ten
   TORCH_CHECK(dlogits.sizes() == logits.sizes() && dlogits.is_contiguous());
   const bool direct = y.has_value() && y->defined();
   TORCH_CHECK(direct || (labels_all.has_value() && nodes.has_value()), "need y or (labels_all, nodes)");
-  launch_softmax_nll(logits.data_ptr(), logits.size(1), C, direct ? y->data_ptr<int64_t>() : nullptr,
-                     direct ? nullptr : labels_all->data_ptr<int64_t>(),
-                     direct ? nullptr : nodes->data_ptr<int64_t>(),
-                     counters.data_ptr<int32_t>(), logits.size(0), loss.data_ptr<float>(),
-                     dlogits.data_ptr(),
-                     (correct.has_value() && correct->defined()) ? correct->data_ptr<int32_t>() : nullptr,
-                     (colsum.has_value() && colsum->defined()) ? colsum->data_ptr<float>() : nullptr,
-                     cur_stream(), prezeroed);
+  TORCH_CHECK(logits.dim() == 2 && logits.size(1) % 8 == 0 && 1 <= C && C <= logits.size(1),
+              "softmax_nll: logits must be [rows, ld] with ld a multiple of 8 and 1 <= C <= ld");
+  const bool has_colsum = colsum.has_value() && colsum->defined();
+  TORCH_CHECK(!has_colsum || (colsum->scalar_type() == torch::kFloat32 && colsum->is_contiguous() &&
+                              colsum->numel() == logits.size(1)), "softmax_nll: colsum must be fp32 [ld]");
+  const int n = launch_softmax_nll(logits.data_ptr(), logits.size(1), C, direct ? y->data_ptr<int64_t>() : nullptr,
+                                   direct ? nullptr : labels_all->data_ptr<int64_t>(),
+                                   direct ? nullptr : nodes->data_ptr<int64_t>(),
+                                   counters.data_ptr<int32_t>(), logits.size(0), loss.data_ptr<float>(),
+                                   dlogits.data_ptr(),
+                                   (correct.has_value() && correct->defined()) ? correct->data_ptr<int32_t>() : nullptr,
+                                   has_colsum ? colsum->data_ptr<float>() : nullptr, cur_stream(), prezeroed);
   check_cuda_err("softmax_nll");
+  return n;
 }
 
 static void zero_grads(Tensor g, const c10::optional<Tensor>& loss, const c10::optional<Tensor>& correct) {

@@ -315,13 +315,28 @@ __global__ void k_adam(float* p, const float* g, float* m, float* v, __nv_bfloat
   }
 }
 
-// column sums of the valid rows of a bf16 [rows, d] matrix (bias gradients); replaces a
-// cap-sized torch reduce kernel that was the most expensive launch of the step.
+// column sums of the valid rows of a bf16 [rows, d] matrix (bias gradients), accumulated into `out` with atomics;
+// replaces a cap-sized torch reduce kernel that was the most expensive launch of the step.  Any d (multiple of 8):
+// rows wider than blockDim.x 8-column groups are summed one row per block iteration.
 __global__ void __launch_bounds__(256) k_colsum(const __nv_bfloat16* X, const int32_t* cum, int n_hops,
                                                 int cap, int d, float* out) {
+  pdl_enter();
   extern __shared__ float s_part[];  // [rows_per_block][d]
   const int T = min(cum[n_hops], cap);
   const int groups = d >> 3;               // 8-column groups per row
+  if (groups > static_cast<int>(blockDim.x)) {
+    for (int cg = threadIdx.x; cg < groups; cg += blockDim.x) {
+      float acc[8];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) acc[i] = 0.f;
+      for (int r = blockIdx.x; r < T; r += gridDim.x)
+        bf16x8_accum(*reinterpret_cast<const uint4*>(X + static_cast<int64_t>(r) * d + cg * 8), acc);
+#pragma unroll
+      for (int i = 0; i < 8; ++i)
+        if (acc[i] != 0.f) atomicAdd(out + cg * 8 + i, acc[i]);
+    }
+    return;
+  }
   const int rpb = blockDim.x / groups;     // rows handled per block iteration
   const int cg = threadIdx.x % groups, rl = threadIdx.x / groups;
   float acc[8];
@@ -482,13 +497,28 @@ void launch_dropout_bf16(void* Z, const int32_t* cum, int n_hops, int cap, int d
            reinterpret_cast<__nv_bfloat16*>(Z), cum, n_hops, cap, d, thresh, scale, seed, layer, step_dev);
 }
 
-void launch_relu_bwd_cast(const float* dH, const void* Z, const int32_t* cum, int n_hops, int cap,
-                          int d, void* dPre, float* colsum, cudaStream_t s, bool prezeroed, float gscale, bool relu) {
-  if (colsum && (2048 % d != 0)) colsum = nullptr;  // caller falls back to launch_colsum_bf16
+// Accumulates the column sums of the first min(cum[n_hops], cap) rows of X into `out` (not zeroed here).
+static void launch_colsum_accum(const void* X, const int32_t* cum, int n_hops, int cap, int d, float* out,
+                                cudaStream_t s) {
+  const int groups = d / 8;
+  const int rpb = 256 / groups > 0 ? 256 / groups : 1;
+  const size_t smem = groups <= 256 ? sizeof(float) * rpb * d : 0;
+  launch_k(k_colsum, dim3(grid_for(cap, rpb * 8, 132 * 2)), dim3(256), smem, s,
+           reinterpret_cast<const __nv_bfloat16*>(X), cum, n_hops, cap, d, out);
+}
+
+int launch_relu_bwd_cast(const float* dH, const void* Z, const int32_t* cum, int n_hops, int cap,
+                         int d, void* dPre, float* colsum, cudaStream_t s, bool prezeroed, float gscale, bool relu) {
+  // the fused column sum needs d | 2048 (a thread keeps its 8 columns across grid-stride iterations); other widths
+  // sum the bf16 dPre in a second pass
+  const bool fused = colsum && 2048 % d == 0;
   if (colsum && !prezeroed) cudaMemsetAsync(colsum, 0, sizeof(float) * d, s);
   launch_k(k_relu_bwd_cast, dim3(grid_for(static_cast<int64_t>(cap) * d / 8, 256 * 2, 132 * 4)), dim3(256), 0, s,
            dH, reinterpret_cast<const __nv_bfloat16*>(Z), cum, n_hops, cap, d,
-           reinterpret_cast<__nv_bfloat16*>(dPre), colsum, gscale, relu ? 1 : 0);
+           reinterpret_cast<__nv_bfloat16*>(dPre), fused ? colsum : nullptr, gscale, relu ? 1 : 0);
+  if (colsum == nullptr || fused) return 1;
+  launch_colsum_accum(dPre, cum, n_hops, cap, d, colsum, s);
+  return 2;
 }
 
 void launch_bias_relu(void* Z, const void* bias, const int32_t* cum, int n_hops, int cap, int d,
@@ -498,17 +528,23 @@ void launch_bias_relu(void* Z, const void* bias, const int32_t* cum, int n_hops,
       cap, d, relu);
 }
 
-void launch_softmax_nll(const void* logits, int ld, int C, const int64_t* y, const int64_t* labels_all,
-                        const int64_t* nodes, const int32_t* cum, int cap, float* loss, void* dlogits,
-                        int32_t* correct, float* colsum, cudaStream_t s, bool prezeroed) {
-  if (ld > 256) colsum = nullptr;
+int launch_softmax_nll(const void* logits, int ld, int C, const int64_t* y, const int64_t* labels_all,
+                       const int64_t* nodes, const int32_t* cum, int cap, float* loss, void* dlogits,
+                       int32_t* correct, float* colsum, cudaStream_t s, bool prezeroed) {
+  // the loss kernel sums the bias gradient in registers for ld <= 256; wider rows sum the bf16 dlogits in a second
+  // pass over the n0 = cum[1] seed rows
+  const bool fused = colsum && ld <= 256;
   if (!prezeroed) {   // memset nodes would break the programmatic-launch chain: the engine zeroes these in k_zero_grads
     if (colsum) cudaMemsetAsync(colsum, 0, sizeof(float) * ld, s);
     cudaMemsetAsync(loss, 0, sizeof(float), s);
     if (correct) cudaMemsetAsync(correct, 0, sizeof(int32_t), s);
   }
   launch_k(k_softmax_nll, dim3(grid_for(cap, 8)), dim3(256), 0, s, reinterpret_cast<const __nv_bfloat16*>(logits), ld,
-           C, y, labels_all, nodes, cum, cap, loss, reinterpret_cast<__nv_bfloat16*>(dlogits), correct, colsum);
+           C, y, labels_all, nodes, cum, cap, loss, reinterpret_cast<__nv_bfloat16*>(dlogits), correct,
+           fused ? colsum : nullptr);
+  if (colsum == nullptr || fused) return 1;
+  launch_colsum_accum(dlogits, cum, 1, cap, ld, colsum, s);
+  return 2;
 }
 
 void launch_adam(float* p, const float* g, float* m, float* v, void* p_bf16, int64_t n, float lr,
@@ -521,10 +557,7 @@ void launch_adam(float* p, const float* g, float* m, float* v, void* p_bf16, int
 void launch_colsum_bf16(const void* X, const int32_t* cum, int n_hops, int cap, int d, float* out,
                         cudaStream_t s) {
   cudaMemsetAsync(out, 0, sizeof(float) * d, s);
-  const int groups = d / 8;
-  const int rpb = 256 / groups > 0 ? 256 / groups : 1;
-  k_colsum<<<grid_for(cap, rpb * 8, 132 * 2), 256, sizeof(float) * rpb * d, s>>>(
-      reinterpret_cast<const __nv_bfloat16*>(X), cum, n_hops, cap, d, out);
+  launch_colsum_accum(X, cum, n_hops, cap, d, out, s);
 }
 
 void launch_add_block_f32(const void* dA, int dA_ld, int col, int d, const int32_t* cum, int n_hops, int cap,

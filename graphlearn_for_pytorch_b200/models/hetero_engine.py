@@ -42,8 +42,12 @@ class HeteroSageEngine(object):
     feature_tables: {node type: native RowTableHandle of bf16 rows indexed by global id} (`UnifiedTensor._table()`,
       `PartitionedFeature.table`).
     labels: int64 [num_nodes[seed_type]].
-    in_dim: feature width (int or {type: int}; multiples of 8).
+    in_dim: feature width (int or {type: int}), a multiple of 8 up to 1024.  The layer-1 operand of each destination
+      type (its incoming relations' source widths plus its own) must be a multiple of 64 wide.
     num_nodes: {type: node count}.
+    hidden: a multiple of 64 up to 1024.
+
+  Widths outside these limits raise ValueError at construction.
     fanouts: [k per hop] (all relations) or {etype: [k per hop]}.
   """
 
@@ -85,7 +89,14 @@ class HeteroSageEngine(object):
     assert 1 <= self.L <= 4 and all(len(f) == self.L for f in self.fan)
     NT, NR = len(self.ntypes), len(self.edge_types)
     self.dim_in = {t: int(in_dim[t] if isinstance(in_dim, dict) else in_dim) for t in self.ntypes}
-    assert all(d % 8 == 0 for d in self.dim_in.values()) and self.hidden % 64 == 0
+    # the aggregation / scatter kernels cover rows of up to 1024 columns; the wgmma GEMMs need 64-column multiples
+    for t, d in self.dim_in.items():
+      if d % 8 != 0 or not 8 <= d <= 1024:
+        raise ValueError(f'in_dim of node type {t!r} must be a multiple of 8 in [8, 1024] (got {d})')
+    if self.hidden % 64 != 0 or not 64 <= self.hidden <= 1024:
+      raise ValueError(f'hidden must be a multiple of 64 in [64, 1024] (got {self.hidden})')
+    if self.C < 1:
+      raise ValueError(f'num_classes must be >= 1 (got {self.C})')
     self.feat = feature_tables
     self.labels = labels.to(dev)
     # types that can appear at hop h (static reachability over the schema)
@@ -148,6 +159,9 @@ class HeteroSageEngine(object):
           c += self._width_in(l, self.nt[r])
         col[t] = (offs, c)                       # mean-block offsets, self-block offset
         K = c + self._width_in(l, t)
+        if K % 64 != 0:                          # weight-gradient GEMM: N = K
+          raise ValueError(f'layer {l} operand of node type {self.ntypes[t]!r} is {K} columns wide (the widths of its '
+                           f'incoming relations\' source types plus its own); it must be a multiple of 64')
         A[t] = torch.zeros(cap, K, dtype=bf, device=dev)
         Z[t] = torch.zeros(cap, n_out, dtype=bf, device=dev)
         dP[t] = torch.zeros(cap, n_out, dtype=bf, device=dev)
@@ -274,9 +288,8 @@ class HeteroSageEngine(object):
       self._k()
     nat.zero_grads(self.g32, self.loss, self.correct)
     boff, n = self._b_off[(self.L, st)]
-    nat.softmax_nll(self.Z[self.L][st], self.C, None, self.labels, ar.nodes_of(st), self._ctr[st], self.loss,
-                    self.dPre[self.L][st], self.correct, self.g32[boff:boff + n], True)
-    self._k(2)
+    self._k(1 + nat.softmax_nll(self.Z[self.L][st], self.C, None, self.labels, ar.nodes_of(st), self._ctr[st],
+                                self.loss, self.dPre[self.L][st], self.correct, self.g32[boff:boff + n], True))
 
   def _backward(self):
     nat, ar = self.nat, self.arena
@@ -302,9 +315,8 @@ class HeteroSageEngine(object):
         self._k()
       for s in self.targets[l - 1]:
         boff, n = self._b_off[(l - 1, s)]
-        nat.relu_bwd_cast(self.dH[l - 1][s], self.Z[l - 1][s], self._ctr[s], nh + 1, self.dPre[l - 1][s],
-                          self.g32[boff:boff + n], True)
-        self._k()
+        self._k(nat.relu_bwd_cast(self.dH[l - 1][s], self.Z[l - 1][s], self._ctr[s], nh + 1, self.dPre[l - 1][s],
+                                  self.g32[boff:boff + n], True))
 
   def _optimizer(self):
     if self.peer_group is not None:

@@ -91,9 +91,12 @@ class GraphSageEngine(object):
     feature_table: native RowTableHandle of bf16 rows indexed by global node id
       (`UnifiedTensor._table()` / `PartitionedFeature.table`); width = in_dim.
     labels: int64 [num_nodes] on the device.
-    in_dim: feature width (multiple of 64 for the fused kernel).
+    in_dim: feature width, a multiple of 8 up to 1024 (64 or 128 for the fused layer-1 kernel, a multiple of 32
+      for the wgmma weight-gradient GEMM).
     num_nodes: number of graph nodes (arena sizing).
-    fanouts / batch_size / hidden / num_classes: model + sampling config.
+    fanouts / batch_size / hidden / num_classes: model + sampling config.  `hidden` is a multiple of 8 up to 1024
+      (a multiple of 64 unless every hidden layer runs the fused kernel); see `_check_widths`.  Widths that no
+      kernel supports raise ValueError here.
     group: torch.distributed group for the gradient all-reduce (None = single process).
     use_fused: True = use the wgmma gather+GEMM kernel where the shape allows; 'auto' = time the
       fused and the unfused (aggregate kernel + cuBLAS) layer on real batches during warm-up and
@@ -144,7 +147,7 @@ class GraphSageEngine(object):
     if use_gather_bwd is None:
       import os as _os
       use_gather_bwd = _os.environ.get('GLT_B200_GATHER_BWD', '1') == '1'
-    self.use_gather_bwd = bool(use_gather_bwd) and int(hidden) <= 1024
+    self.use_gather_bwd = bool(use_gather_bwd)
     # every dense contraction outside the fused layer-1 kernel runs on the TMA-fed wgmma GEMM kernel
     # (csrc/cuda/tc_gemm.cu); GLT_B200_TC_GEMM=0 falls back to cuBLAS for A/B measurements
     import os as _os2
@@ -163,8 +166,8 @@ class GraphSageEngine(object):
     assert 1 <= self.L <= 4
     self.bs = int(batch_size)
     self.in_dim, self.hidden, self.C = int(in_dim), int(hidden), int(num_classes)
-    assert self.in_dim % 8 == 0 and self.hidden % 8 == 0
     self.n_out_pad = _round_up(self.C, 64)
+    self._check_widths(use_fused)
     self.lr, self.wd = lr, weight_decay
     self.seed = int(seed)
     self.group = group
@@ -215,6 +218,35 @@ class GraphSageEngine(object):
     self._graph_fb = None
     self._graph_opt = None
     self._graph_full = None
+
+  def _check_widths(self, use_fused):
+    """Rejects, at construction, widths that a kernel of the step cannot run (instead of failing at the first step or
+    silently computing on truncated rows).  `in_dim` and `hidden` are multiples of 8 up to 1024, the widest row of
+    the aggregation / scatter kernels.  With the wgmma GEMMs (the default), every layer's A operand [mean | self]
+    is a multiple of 64 wide (weight gradients), so `in_dim` and `hidden` are multiples of 32; and `hidden` is a
+    multiple of 64 when a hidden layer runs the unfused forward GEMM, i.e. unless each hidden layer fits the fused
+    layer kernel (input width 64 or 128, `hidden` <= 256)."""
+    for name, d in (('in_dim', self.in_dim), ('hidden', self.hidden)):
+      if d % 8 != 0 or not 8 <= d <= 1024:
+        raise ValueError(f'{name} must be a multiple of 8 in [8, 1024] (got {d})')
+    if self.C < 1:
+      raise ValueError(f'num_classes must be >= 1 (got {self.C})')
+    if not self.use_tc_gemm:
+      return
+    for name, d in (('in_dim', self.in_dim), ('hidden', self.hidden)):
+      if name == 'hidden' and self.L == 1:
+        continue
+      if d % 32 != 0:
+        raise ValueError(f'{name} = {d}: the weight-gradient GEMM needs the layer input [mean | self] '
+                         f'(2 x {d} = {2 * d} columns) to be a multiple of 64 wide')
+    if self.hidden % 64 != 0:
+      dims_in = [self.in_dim] + [self.hidden] * (self.L - 1)
+      for l in range(1, self.L):          # hidden layers (the last layer's output is padded to 64 columns)
+        fused = use_fused != 'auto' and bool(use_fused) and \
+            bool(self.nat.sage_fused_supported(dims_in[l - 1], self.hidden))
+        if not fused:
+          raise ValueError(f'hidden = {self.hidden}: layer {l} runs the unfused forward GEMM, whose output width must '
+                           f'be a multiple of 64')
 
   def _build_buffers(self, cap_override):
     """(Re)creates everything whose size depends on the arena capacities: sampler arenas, activation /
@@ -520,9 +552,8 @@ class GraphSageEngine(object):
     if train:                      # evaluation must not take part in the cross-rank gradient protocol
       self._begin_grads()
     # the bias gradient of the last layer (column sums of dlogits) is produced by the loss kernel
-    nat.softmax_nll(self.Z[self.L], self.C, None, self.labels, ar.nodes, ar.counters, self.loss,
-                    self.dPre[self.L], self.correct, self.g32[boff:boff + n], train)
-    self._k(1)
+    self._k(nat.softmax_nll(self.Z[self.L], self.C, None, self.labels, ar.nodes, ar.counters, self.loss,
+                            self.dPre[self.L], self.correct, self.g32[boff:boff + n], train))
 
   def _begin_grads(self):
     """Runs before the first kernel that writes into the flat gradient buffer (the loss kernel produces the
@@ -591,9 +622,8 @@ class GraphSageEngine(object):
         if l == self.L:
           main.wait_event(ev_zero)
         nat.sage_scatter_bwd(self.dA[l], self.dims_in[l - 1], ar.counters, nh, ell, ks, ar.deg, self.dH[l - 1])
-        nat.relu_bwd_cast(self.dH[l - 1], self.Z[l - 1], ar.counters, nh + 1, self.dPre[l - 1],
-                          self.g32[pboff:pboff + pn], True, 1.0 / (1.0 - self.dropout))
-        self._k(2)
+        self._k(1 + nat.relu_bwd_cast(self.dH[l - 1], self.Z[l - 1], ar.counters, nh + 1, self.dPre[l - 1],
+                                      self.g32[pboff:pboff + pn], True, 1.0 / (1.0 - self.dropout)))
         continue
       if self.use_tc_gemm:
         self._plan('wgrad' if overlap else 'bwd', l).run()
@@ -619,9 +649,8 @@ class GraphSageEngine(object):
         nat.zero_rows(self.dH[l - 1], ar.counters, nh + 1)
         self._k(1)
         nat.sage_scatter_bwd(self.dA[l], self.dims_in[l - 1], ar.counters, nh, ell, ks, ar.deg, self.dH[l - 1])
-        nat.relu_bwd_cast(self.dH[l - 1], self.Z[l - 1], ar.counters, nh + 1, self.dPre[l - 1],
-                          self.g32[pboff:pboff + pn], True, 1.0 / (1.0 - self.dropout))
-        self._k(2)
+        self._k(1 + nat.relu_bwd_cast(self.dH[l - 1], self.Z[l - 1], ar.counters, nh + 1, self.dPre[l - 1],
+                                      self.g32[pboff:pboff + pn], True, 1.0 / (1.0 - self.dropout)))
 
   _f32_mode = None
 

@@ -113,14 +113,8 @@ class GraphSageLinkEngine(GraphSageEngine):
     if not train:
       return
     boff, n = self._b_off[L - 1]
-    gb = self.g32[boff:boff + n]
-    fused_colsum = 2048 % n == 0            # relu_bwd_cast sums columns for widths dividing 2048
-    nat.relu_bwd_cast(self._dZ32, self.Z[L], ar.counters, 1, self.dPre[L], gb if fused_colsum else None, True, 1.0,
-                      relu=False)
-    self._k(1)
-    if not fused_colsum:
-      nat.colsum_bf16(self.dPre[L], ar.counters, 1, gb)
-      self._k(1)
+    self._k(nat.relu_bwd_cast(self._dZ32, self.Z[L], ar.counters, 1, self.dPre[L], self.g32[boff:boff + n], True, 1.0,
+                              relu=False))
 
   @torch.no_grad()
   def evaluate_batch(self, pairs: torch.Tensor):

@@ -32,3 +32,31 @@ def canonical_edges(out):
   """Set of (global src, global dst) pairs of a SamplerOutput."""
   node = out.node.cpu()
   return set(zip(node[out.row.cpu()].tolist(), node[out.col.cpu()].tolist()))
+
+
+# --------------------------------------------------------------------------- error bounds of GPU kernels
+def bf16_ulp(x: torch.Tensor) -> torch.Tensor:
+  """Spacing of bf16 numbers at |x| (float64): 2^(e - 7) for |x| in [2^e, 2^(e+1)); the smallest normal spacing at 0."""
+  x = x.double().abs()
+  _, e = torch.frexp(x)                     # x = m * 2^e, m in [0.5, 1)
+  return torch.where(x > 0, torch.ldexp(torch.ones_like(x), e - 8), torch.full_like(x, 2.0 ** -133))
+
+
+def gemm_bound(ref: torch.Tensor, absprod: torch.Tensor, k: int, bf16_out: bool = True) -> torch.Tensor:
+  """Largest error of a bf16 GEMM with fp32 accumulation over a contraction of length k: k * 2^-22 * (|A| . |W|^T)
+  (fp32 summation with margin for truncating adders), plus one bf16 ulp of the result for a bf16 output.  `ref` and
+  `absprod` are float64; for a split-K fp32 output (`bf16_out=False`) only the summation term applies."""
+  b = float(k) * 2.0 ** -22 * absprod.double()
+  return b + bf16_ulp(ref) if bf16_out else b
+
+
+def bound_ratio(got: torch.Tensor, ref: torch.Tensor, bound: torch.Tensor) -> float:
+  """max |got - ref| / bound over all elements (<= 1 when every element lies within its bound; 0-bound elements
+  must match exactly)."""
+  err = (got.double() - ref.double()).abs()
+  if err.numel() == 0:
+    return 0.0
+  exact = bound <= 0
+  if bool((err[exact] > 0).any()):
+    return float('inf')
+  return float((err[~exact] / bound[~exact]).max()) if bool((~exact).any()) else 0.0

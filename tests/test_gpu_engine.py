@@ -267,22 +267,33 @@ def test_transposed_adjacency_matches_ell(native):
   assert int(off[ar.tr_off.numel() - 1]) == sum(len(v) for e in exp for v in e.values())
 
 
+def _widths(in_dim, hidden, num_classes):
+  # the original three cases keep their ids ([hidden-gather])
+  legacy = in_dim == 128 and num_classes == 47
+  return pytest.param(in_dim, hidden, num_classes, id=str(hidden) if legacy else f'{in_dim}-{hidden}-{num_classes}')
+
+
 @experimental
 @pytest.mark.parametrize('gather', [True, False])
-@pytest.mark.parametrize('hidden', [256, 512, 64])
-def test_backward_matches_pytorch_gather_and_scatter(native, hidden, gather):
+@pytest.mark.parametrize('in_dim,hidden,num_classes', [
+    _widths(128, 256, 47), _widths(128, 512, 47), _widths(128, 64, 47),
+    # together every lane-group shape of the aggregation / scatter kernels (LPR 4 .. VPL 4), hidden widths that do
+    # not divide 2048 (bias gradient in a second pass) and a classifier wider than 256 columns
+    _widths(32, 1024, 8), _widths(256, 192, 47), _widths(1024, 768, 300)])
+def test_backward_matches_pytorch_gather_and_scatter(native, in_dim, hidden, num_classes, gather):
   """Weight / bias gradients of every layer against fp32 autograd on the same sampled batch, for the atomics-free
-  gather backward and the fp32-atomic scatter backward, at three hidden widths (lane-group shapes of the kernels)."""
+  gather backward and the fp32-atomic scatter backward, at feature widths 32 to 1024, hidden widths 64 to 1024 and 8
+  to 300 classes."""
   ei, topo = rmat_csr(6000, 120000, seed=3)
   g = glt.data.Graph(topo, 'CUDA', 0)
   torch.manual_seed(0)
-  feats = torch.randn(6000, 128, device=DEV).to(torch.bfloat16)
-  labels = torch.randint(0, 47, (6000,), device=DEV)
+  feats = torch.randn(6000, in_dim, device=DEV).to(torch.bfloat16)
+  labels = torch.randint(0, num_classes, (6000,), device=DEV)
   ut = glt.data.UnifiedTensor(0, torch.bfloat16)
   ut.append_shared_tensor(feats)
-  eng = GraphSageEngine(g, ut._table(), labels, in_dim=128, num_nodes=6000, fanouts=[5, 4, 3], batch_size=256,
-                        hidden=hidden, num_classes=47, device=DEV, use_fused=(hidden <= 256), use_cuda_graph=False,
-                        seed=5, use_gather_bwd=gather)
+  eng = GraphSageEngine(g, ut._table(), labels, in_dim=in_dim, num_nodes=6000, fanouts=[5, 4, 3], batch_size=256,
+                        hidden=hidden, num_classes=num_classes, device=DEV, use_fused=(hidden <= 256),
+                        use_cuda_graph=False, seed=5, use_gather_bwd=gather)
   assert eng.use_gather_bwd == gather
   eng.seeds_dev.copy_(torch.randperm(6000, device=DEV)[:256])
   eng._sample(); eng._forward(); eng._backward()
@@ -300,6 +311,48 @@ def test_backward_matches_pytorch_gather_and_scatter(native, hidden, gather):
   # bf16 operands, fp32 accumulation: the error grows with the contraction length of the hidden layers
   tol = 5e-2 if hidden <= 256 else 1e-1
   assert all(e < tol for e in errs.values()), errs
+
+
+@pytest.mark.parametrize('kw,ok', [
+    (dict(), True),
+    (dict(in_dim=32, hidden=1024, num_classes=8), True),
+    (dict(in_dim=1024, hidden=768, num_classes=2983), True),
+    (dict(hidden=96, fanouts=[7, 6]), True),                 # the only hidden layer is the fused layer 1
+    (dict(in_dim=200), False),                               # layer-1 weight gradient: A is 400 columns wide
+    (dict(in_dim=2048), False),                              # wider than the aggregation kernels' rows
+    (dict(hidden=1536, use_gather_bwd=False), False),
+    (dict(hidden=96), False),                                # layer 2 is unfused: forward GEMM with N = 96
+    (dict(hidden=96, fanouts=[7, 6], use_fused=False), False),
+    (dict(hidden=100), False),
+])
+def test_engine_constructor_rejects_unsupported_widths(native, kw, ok):
+  """Widths no kernel of the step can run raise ValueError at construction instead of failing at the first step or
+  training on truncated rows."""
+  args = dict(in_dim=128, hidden=256, num_classes=47, fanouts=[5, 4, 3])
+  args.update(kw)
+  ei, topo = rmat_csr(2000, 20000, seed=3)
+  g = glt.data.Graph(topo, 'CUDA', 0)
+  feats = torch.zeros(2000, args['in_dim'], dtype=torch.bfloat16, device=DEV)
+  ut = glt.data.UnifiedTensor(0, torch.bfloat16)
+  ut.append_shared_tensor(feats)
+  labels = torch.zeros(2000, dtype=torch.int64, device=DEV)
+  make = lambda: GraphSageEngine(g, ut._table(), labels, num_nodes=2000, batch_size=64, device=DEV,
+                                 use_cuda_graph=False, **args)
+  if ok:
+    make()
+  else:
+    with pytest.raises(ValueError, match=r'in_dim|hidden'):
+      make()
+
+
+def test_link_engine_rejects_wide_features(native):
+  from graphlearn_for_pytorch_b200.models import GraphSageLinkEngine
+  ei, topo = rmat_csr(2000, 20000, seed=3)
+  g = glt.data.Graph(topo, 'CUDA', 0)
+  ut = glt.data.UnifiedTensor(0, torch.bfloat16)
+  ut.append_shared_tensor(torch.zeros(2000, 2048, dtype=torch.bfloat16, device=DEV))
+  with pytest.raises(ValueError, match='in_dim'):
+    GraphSageLinkEngine(g, ut._table(), 2048, 2000, fanouts=[5, 4], batch_size=64, device=DEV)
 
 
 @experimental

@@ -1,5 +1,7 @@
 """HeteroSageEngine (device-resident R-SAGE step) against a plain fp32 PyTorch recomputation on the SAME sampled
-batch: forward loss, weight gradients of every (layer, type), and training progress under CUDA-graph replay."""
+batch: forward loss, weight and bias gradients of every (layer, type), and training progress under CUDA-graph
+replay.  The numerics are checked at 64-wide features / hidden 64 / 19 classes, at IGBH-like per-type feature widths
+(up to 1024) with a hidden width that does not divide 2048, and with the 2983-class IGBH label set."""
 import os
 import sys
 
@@ -14,9 +16,15 @@ sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(
 
 
 def _build(papers=4000, feat_dim=64, hidden=64, fan=(4, 3, 2), bs=256, use_graph=False, classes=19):
+  """feat_dim: one width for every node type, or {type: width}."""
   from common import synthetic_igbh
   from graphlearn_for_pytorch_b200.models import HeteroSageEngine
-  edges, feats, labels, sizes = synthetic_igbh(papers, papers // 2, 50, 30, feat_dim=feat_dim, num_classes=classes, seed=2)
+  edges, feats, labels, sizes = synthetic_igbh(papers, papers // 2, 50, 30, feat_dim=64, num_classes=classes, seed=2)
+  if isinstance(feat_dim, dict):
+    g = torch.Generator().manual_seed(3)
+    feats = {t: torch.randn(sizes[t], feat_dim[t], generator=g) for t in sizes}
+  elif feat_dim != 64:
+    feats = {t: torch.randn(sizes[t], feat_dim, generator=torch.Generator().manual_seed(3)) for t in sizes}
   graphs, tables, keep = {}, {}, []
   for et, ei in edges.items():
     topo = glt.data.Topology(ei.to(DEV), layout='CSC', num_nodes=sizes[et[2]])
@@ -41,7 +49,7 @@ def _reference(eng, fb, labels):
   L, nt, kt = eng.L, eng.nt, eng.kt
   bf = lambda x: x.to(torch.bfloat16).float()
   W = {k: eng.p16[off:off + n * kk].view(n, kk).float().requires_grad_(True) for k, (off, n, kk) in eng._w_off.items()}
-  B = {k: eng.p16[off:off + n].float() for k, (off, n) in eng._b_off.items()}
+  B = {k: eng.p16[off:off + n].float().requires_grad_(True) for k, (off, n) in eng._b_off.items()}
   x = {t: fb[eng.ntypes[t]][nodes[t]].float() for t in range(len(eng.ntypes))}
   for l in range(1, L + 1):
     nh = L - l + 1
@@ -67,29 +75,61 @@ def _reference(eng, fb, labels):
   y = labels[nodes[st][:n0]]
   loss = torch.nn.functional.cross_entropy(logits, y)
   loss.backward()
-  return float(loss), {k: w.grad for k, w in W.items()}, (nn, ne)
+  return float(loss), {k: w.grad for k, w in W.items()}, {k: b.grad for k, b in B.items()}, (nn, ne)
 
 
-def test_hetero_engine_forward_backward_match_fp32():
-  eng, fb, labels, sizes = _build()
-  seeds = torch.randperm(sizes['paper'], device=DEV)[:eng.bs]
-  eng._seeds.copy_(seeds)
+def _gradient_errors(feat_dim=64, hidden=64, classes=19, batch_seed=0):
+  """Runs one engine step on a seeded batch and returns {name: max |engine - fp32 reference| / max |reference|} for the
+  loss and every weight and bias gradient."""
+  eng, fb, labels, sizes = _build(feat_dim=feat_dim, hidden=hidden, classes=classes)
+  seeds = torch.randperm(sizes['paper'], generator=torch.Generator().manual_seed(batch_seed))[:eng.bs]
+  eng._seeds.copy_(seeds.to(DEV))
   eng._sample()
   eng._forward()
   eng._backward()
   torch.cuda.synchronize()
   assert eng.overflow_count() == 0
-  ref_loss, ref_grads, (nn, ne) = _reference(eng, fb, labels)
-  assert abs(float(eng.loss.item()) - ref_loss) < 3e-2 * max(1.0, abs(ref_loss)), (float(eng.loss.item()), ref_loss)
+  ref_loss, ref_grads, ref_bgrads, (nn, ne) = _reference(eng, fb, labels)
   assert sum(sum(v) for v in ne) > 1000                     # the batch really has relations of every kind
+  errs = {'loss': abs(float(eng.loss.item()) - ref_loss) / max(1.0, abs(ref_loss))}
   for k, (off, n, kk) in eng._w_off.items():
-    g = eng.g32[off:off + n * kk].view(n, kk)
     r = ref_grads[k]
-    if r is None:
-      continue
-    scale = max(float(r.abs().max()), 1e-6)
-    err = float((g - r).abs().max()) / scale
-    assert err < 6e-2, (k, err, scale)
+    if r is not None:
+      errs[f'W{k}'] = float((eng.g32[off:off + n * kk].view(n, kk) - r).abs().max()) / max(float(r.abs().max()), 1e-6)
+  for k, (off, n) in eng._b_off.items():
+    r = ref_bgrads[k]
+    if r is not None:
+      errs[f'b{k}'] = float((eng.g32[off:off + n] - r).abs().max()) / max(float(r.abs().max()), 1e-6)
+  return errs
+
+
+def _assert_gradients_match(errs):
+  assert errs.pop('loss') < 3e-2, errs
+  bad = {k: e for k, e in errs.items() if not e < 6e-2}
+  assert not bad, bad
+
+
+def test_hetero_engine_forward_backward_match_fp32():
+  _assert_gradients_match(_gradient_errors())
+
+
+@pytest.mark.parametrize('feat_dim,hidden,classes', [
+    ({'paper': 1024, 'author': 256, 'institute': 64, 'fos': 128}, 192, 19),   # hidden width not dividing 2048
+    (64, 64, 2983),                                                          # IGBH's 2983-class label set
+], ids=['igbh_widths-192-19', '64-64-2983'])
+def test_hetero_engine_gradients_match_fp32_at_wide_layers(feat_dim, hidden, classes):
+  _assert_gradients_match(_gradient_errors(feat_dim, hidden, classes))
+
+
+@pytest.mark.parametrize('feat_dim,hidden', [
+    ({'paper': 64, 'author': 64, 'institute': 64, 'fos': 40}, 64),   # fos operand 64 + 40 = 104 columns
+    (2048, 64),
+    (64, 96),
+    (64, 2048),
+])
+def test_hetero_engine_rejects_unsupported_widths(feat_dim, hidden):
+  with pytest.raises(ValueError, match='in_dim|hidden|multiple of 64'):
+    _build(papers=1000, feat_dim=feat_dim, hidden=hidden)
 
 
 def test_hetero_engine_trains_under_cuda_graph():
