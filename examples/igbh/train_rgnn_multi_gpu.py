@@ -7,11 +7,12 @@ writes resumable checkpoints (`--ckpt_steps`, `--ckpt_path`).  Two trainer back-
 
   --trainer loader   hetero `NeighborLoader` (native grouped sampling arena on the GPU) + eager `models.RGNN`
                      (rgat / rsage / rgcn) + DistributedDataParallel -- the reference's structure
-  --trainer engine   `models.HeteroSageEngine`: the whole R-SAGE step (sampling, aggregation, wgmma GEMMs,
-                     backward, Adam with the gradient all-reduce fused in over NVLink peer memory) is one CUDA graph
-                     per rank; relations and features are range-partitioned over the GPUs (no replica per rank)
+  --trainer engine   `models.HeteroGatEngine` (--model rgat, `--num_heads` heads) or `models.HeteroSageEngine`
+                     (--model rsage): the whole step (sampling, aggregation, wgmma GEMMs, backward, Adam with the
+                     gradient all-reduce fused in over NVLink peer memory) is one CUDA graph per rank; relations and
+                     features are range-partitioned over the GPUs (no replica per rank).  rgcn has no engine.
 
-  python examples/igbh/train_rgnn_multi_gpu.py --path /data/igbh --dataset_size tiny --model rsage --trainer engine
+  python examples/igbh/train_rgnn_multi_gpu.py --path /data/igbh --dataset_size tiny --model rgat --trainer engine
 
 Without a GPU the loader back-end runs on gloo + CPU so the script stays testable anywhere.
 """
@@ -125,7 +126,7 @@ def run_loader(rank, world, ds, igbh_meta, a, port):
 
 def run_engine(rank, world, igbh, a, port):
   """Device-resident back-end: relations and features range-partitioned over the GPUs, one CUDA graph per step."""
-  from graphlearn_for_pytorch_b200.models import HeteroSageEngine
+  from graphlearn_for_pytorch_b200.models import HeteroGatEngine, HeteroSageEngine
   from graphlearn_for_pytorch_b200.parallel import PartitionedFeature, partition_hetero_graph
   os.environ['MASTER_ADDR'], os.environ['MASTER_PORT'] = '127.0.0.1', str(port)
   torch.cuda.set_device(rank)
@@ -150,9 +151,12 @@ def run_engine(rank, world, igbh, a, port):
       stores[nt], tables[nt] = ut, ut._table()
   in_dim = {nt: (f.shape[1] + 7) // 8 * 8 for nt, f in feat_dict.items()}
   fan = [int(v) for v in a.fan_out.split(',')]
-  eng = HeteroSageEngine(graphs, tables, label.to(device), in_dim, num_nodes, 'paper', fanouts=fan,
-                         batch_size=a.train_batch_size, hidden=a.hidden_channels, num_classes=num_classes, edge_dir='in',
-                         lr=a.learning_rate, seed=a.random_seed, device=device)
+  common = dict(fanouts=fan, batch_size=a.train_batch_size, hidden=a.hidden_channels, num_classes=num_classes,
+                edge_dir='in', lr=a.learning_rate, seed=a.random_seed, device=device)
+  if a.model == 'rgat':
+    eng = HeteroGatEngine(graphs, tables, label.to(device), in_dim, num_nodes, 'paper', heads=a.num_heads, **common)
+  else:
+    eng = HeteroSageEngine(graphs, tables, label.to(device), in_dim, num_nodes, 'paper', **common)
   eng.warmup_and_capture(n_eager=1)
   mine = train_idx.split((train_idx.numel() + world - 1) // world)[rank]
   steps = mine.numel() // a.train_batch_size
@@ -220,6 +224,9 @@ if __name__ == '__main__':
   igbh = IGBHeteroDataset(a.path, a.dataset_size, layout=a.layout, use_fp16=a.use_fp16)
   assert igbh.train_idx is not None, 'run split_seeds.py first'
   port = free_port()
+  if a.trainer == 'engine' and a.model == 'rgcn':
+    ap.error('--trainer engine trains --model rgat (HeteroGatEngine) or rsage (HeteroSageEngine); '
+             'rgcn runs with --trainer loader')
   if a.trainer == 'engine':
     assert cuda, 'the engine back-end needs a GPU'
     assert a.layout == 'COO', 'the engine builds its own CSC shards from the COO edge lists'

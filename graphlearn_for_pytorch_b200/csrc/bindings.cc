@@ -1027,6 +1027,238 @@ static int64_t relu_bwd_cast(const Tensor& dH, const Tensor& Z, const Tensor& co
   return n;
 }
 
+// ---- relational GAT (cuda/gat.cu) -------------------------------------------------------------------------------
+// H = heads * C must be a multiple of 64 in [64, 1024] with C a multiple of 8 (one 16-byte vector never straddles two
+// heads).  Messages are single strings (see check_sage_width).
+static void check_gat_width(int64_t H, int64_t heads) {
+  TORCH_CHECK(H % 64 == 0 && H >= 64 && H <= 1024 && heads >= 1 && H % heads == 0 && (H / heads) % 8 == 0,
+              "gat: H must be a multiple of 64 in [64, 1024] and heads must divide H into head widths C with C % 8 == 0");
+}
+
+static bool has(const c10::optional<Tensor>& t) { return t.has_value() && t->defined(); }
+
+static void check_rows(const Tensor& t, c10::ScalarType dt, int64_t w, const char* msg) {
+  TORCH_CHECK(t.is_cuda() && t.scalar_type() == dt && t.dim() == 2 && t.size(1) == w && t.is_contiguous() &&
+              reinterpret_cast<uintptr_t>(t.data_ptr()) % 16 == 0, msg);
+}
+
+static void gat_fill_hops(const std::vector<Tensor>& ell, const std::vector<int64_t>& ks, const std::vector<Tensor>& bufs,
+                          int64_t heads, float** out) {
+  TORCH_CHECK(bufs.size() == ell.size(), "gat: one alpha buffer per hop");
+  for (size_t h = 0; h < 4; ++h) out[h] = nullptr;
+  for (size_t h = 0; h < bufs.size(); ++h) {
+    TORCH_CHECK(bufs[h].is_cuda() && bufs[h].scalar_type() == torch::kFloat32 && bufs[h].is_contiguous() &&
+                bufs[h].numel() >= ell[h].numel() * heads, "gat: alpha buffers must be fp32 [ELL slots of the hop, heads]");
+    out[h] = bufs[h].data_ptr<float>();
+  }
+}
+
+// scores of the source rows (P0, rows < counters0[idx0]) and, optionally, of the target rows (P1)
+static void gat_scores(const Tensor& P0, const Tensor& att0, Tensor out0, const Tensor& counters0, int64_t idx0,
+                       const c10::optional<Tensor>& P1, const c10::optional<Tensor>& att1,
+                       const c10::optional<Tensor>& out1, const c10::optional<Tensor>& counters1, int64_t idx1,
+                       const c10::optional<Tensor>& zero, int64_t heads) {
+  c10::cuda::CUDAGuard guard(P0.device());
+  const int64_t H = P0.size(1);
+  check_gat_width(H, heads);
+  GatScoreArgs a{};
+  a.H = H; a.heads = heads;
+  check_rows(P0, torch::kBFloat16, H, "gat_scores: P must be contiguous bf16 [rows, H]");
+  check_rows(out0, torch::kFloat32, heads, "gat_scores: out must be contiguous fp32 [rows, heads]");
+  TORCH_CHECK(att0.scalar_type() == torch::kBFloat16 && att0.numel() == H && att0.is_contiguous() &&
+              reinterpret_cast<uintptr_t>(att0.data_ptr()) % 16 == 0, "gat_scores: att must be 16-byte aligned bf16 [H]");
+  TORCH_CHECK(out0.size(0) >= P0.size(0), "gat_scores: out has fewer rows than P");
+  a.P[0] = P0.data_ptr(); a.att[0] = att0.data_ptr(); a.out[0] = out0.data_ptr<float>();
+  a.cum[0] = counters0.data_ptr<int32_t>(); a.idx[0] = idx0; a.cap[0] = P0.size(0);
+  if (has(P1)) {
+    TORCH_CHECK(has(att1) && has(out1) && has(counters1), "gat_scores: the second set needs P, att, out and counters");
+    check_rows(*P1, torch::kBFloat16, H, "gat_scores: P must be contiguous bf16 [rows, H]");
+    check_rows(*out1, torch::kFloat32, heads, "gat_scores: out must be contiguous fp32 [rows, heads]");
+    TORCH_CHECK(att1->scalar_type() == torch::kBFloat16 && att1->numel() == H && att1->is_contiguous() &&
+                reinterpret_cast<uintptr_t>(att1->data_ptr()) % 16 == 0, "gat_scores: att must be 16-byte aligned bf16 [H]");
+    TORCH_CHECK(out1->size(0) >= P1->size(0), "gat_scores: out has fewer rows than P");
+    a.P[1] = P1->data_ptr(); a.att[1] = att1->data_ptr(); a.out[1] = out1->data_ptr<float>();
+    a.cum[1] = counters1->data_ptr<int32_t>(); a.idx[1] = idx1; a.cap[1] = P1->size(0);
+  } else {
+    a.cum[1] = a.cum[0];
+  }
+  if (has(zero)) {
+    check_rows(*zero, torch::kFloat32, heads, "gat_scores: zero must be contiguous fp32 [rows, heads]");
+    TORCH_CHECK(zero->size(0) >= P0.size(0), "gat_scores: zero has fewer rows than P");
+    a.zero = zero->data_ptr<float>();
+  }
+  launch_gat_scores(a, cur_stream());
+  check_cuda_err("gat_scores");
+}
+
+// Returns nothing; writes alpha, and acc (first/last false) or Z (last).
+static void gat_aggregate(const Tensor& P, const Tensor& as, const Tensor& ad, int64_t heads, const Tensor& counters,
+                          int64_t n_hops_targets, const std::vector<Tensor>& ell, const std::vector<int64_t>& ks,
+                          const Tensor& deg, const std::vector<Tensor>& alpha, const c10::optional<Tensor>& acc,
+                          bool first, bool last, const c10::optional<Tensor>& bias, bool act, double p, int64_t seed,
+                          int64_t layer, const c10::optional<Tensor>& step_dev, const c10::optional<Tensor>& Z) {
+  c10::cuda::CUDAGuard guard(P.device());
+  const int64_t H = P.size(1);
+  check_gat_width(H, heads);
+  check_rows(P, torch::kBFloat16, H, "gat_aggregate: P must be contiguous bf16 [rows, H]");
+  check_rows(as, torch::kFloat32, heads, "gat_aggregate: as must be contiguous fp32 [rows, heads]");
+  check_rows(ad, torch::kFloat32, heads, "gat_aggregate: ad must be contiguous fp32 [rows, heads]");
+  TORCH_CHECK(as.size(0) >= P.size(0), "gat_aggregate: as has fewer rows than P");
+  TORCH_CHECK(p >= 0.0 && p < 1.0, "gat_aggregate: dropout p must be in [0, 1)");
+  GatAggArgs a{};
+  a.P = P.data_ptr(); a.as = as.data_ptr<float>(); a.ad = ad.data_ptr<float>();
+  a.H = H; a.heads = heads;
+  a.cum = counters.data_ptr<int32_t>();
+  a.n_hops_targets = n_hops_targets;
+  int64_t cap = ad.size(0);
+  fill_ell(ell, ks, a.ell, a.k);
+  a.deg = deg.data_ptr<int32_t>();
+  gat_fill_hops(ell, ks, alpha, heads, a.alpha);
+  a.first = first ? 1 : 0; a.last = last ? 1 : 0;
+  if (!(first && last)) {
+    TORCH_CHECK(has(acc), "gat_aggregate: a relation sum over several launches needs acc");
+    check_rows(*acc, torch::kFloat32, H, "gat_aggregate: acc must be contiguous fp32 [rows, H]");
+    cap = std::min<int64_t>(cap, acc->size(0));
+    a.acc = acc->data_ptr<float>();
+  }
+  if (last) {
+    TORCH_CHECK(has(Z), "gat_aggregate: the last relation writes Z");
+    check_rows(*Z, torch::kBFloat16, H, "gat_aggregate: Z must be contiguous bf16 [rows, H]");
+    cap = std::min<int64_t>(cap, Z->size(0));
+    a.z = Z->data_ptr();
+    if (has(bias)) {
+      TORCH_CHECK(bias->is_cuda() && bias->scalar_type() == torch::kBFloat16 && bias->is_contiguous() &&
+                  bias->numel() % H == 0 && reinterpret_cast<uintptr_t>(bias->data_ptr()) % 16 == 0,
+                  "gat_aggregate: bias must be 16-byte aligned bf16 [n_bias * H]");
+      a.bias = bias->data_ptr();
+      a.n_bias = bias->numel() / H;
+    }
+    a.act = act ? 1 : 0;
+    a.thresh16 = static_cast<uint32_t>(std::min(std::max(p, 0.0), 1.0) * 65536.0);
+    a.dscale = static_cast<float>(1.0 / (1.0 - p));
+    a.seed = static_cast<uint64_t>(seed);
+    a.layer = layer;
+    if (has(step_dev)) {
+      TORCH_CHECK(step_dev->scalar_type() == torch::kInt32 && step_dev->is_cuda(), "gat_aggregate: int32 step_dev");
+      a.step_dev = step_dev->data_ptr<int32_t>();
+    }
+  }
+  a.cap_targets = cap;
+  launch_gat_aggregate(a, cur_stream());
+  check_cuda_err("gat_aggregate");
+}
+
+static void gat_backward(const Tensor& G, const Tensor& P, int64_t heads, const Tensor& counters, int64_t n_hops_targets,
+                         const std::vector<Tensor>& ell, const std::vector<int64_t>& ks, const Tensor& deg,
+                         const std::vector<Tensor>& alpha, const std::vector<Tensor>& dal, Tensor dP, Tensor da_src,
+                         Tensor da_dst) {
+  c10::cuda::CUDAGuard guard(G.device());
+  const int64_t H = P.size(1);
+  check_gat_width(H, heads);
+  check_rows(G, torch::kBFloat16, H, "gat_backward: G must be contiguous bf16 [rows, H]");
+  check_rows(P, torch::kBFloat16, H, "gat_backward: P must be contiguous bf16 [rows, H]");
+  check_rows(dP, torch::kFloat32, H, "gat_backward: dP must be contiguous fp32 [rows, H]");
+  check_rows(da_src, torch::kFloat32, heads, "gat_backward: da_src must be contiguous fp32 [rows, heads]");
+  check_rows(da_dst, torch::kFloat32, heads, "gat_backward: da_dst must be contiguous fp32 [rows, heads]");
+  TORCH_CHECK(dP.size(0) >= P.size(0) && da_src.size(0) >= P.size(0), "gat_backward: dP / da_src have fewer rows than P");
+  GatBwdArgs a{};
+  a.G = G.data_ptr(); a.P = P.data_ptr(); a.H = H; a.heads = heads;
+  a.cum = counters.data_ptr<int32_t>();
+  a.n_hops_targets = n_hops_targets;
+  a.cap_targets = std::min<int64_t>(G.size(0), da_dst.size(0));
+  fill_ell(ell, ks, a.ell, a.k);
+  a.deg = deg.data_ptr<int32_t>();
+  float* al[4];
+  gat_fill_hops(ell, ks, alpha, heads, al);
+  for (int h = 0; h < 4; ++h) a.alpha[h] = al[h];
+  gat_fill_hops(ell, ks, dal, heads, a.dal);
+  a.dP = dP.data_ptr<float>(); a.da_src = da_src.data_ptr<float>(); a.da_dst = da_dst.data_ptr<float>();
+  launch_gat_backward(a, cur_stream());
+  check_cuda_err("gat_backward");
+}
+
+// Source segment: P_src / dP_src / da_src / att_src -> dPb_src (+ g_att_src).  Destination: a separate projection
+// P_dst -> dPb_dst, or (P_dst None) folded into the source rows, which then start with the target rows.
+static void gat_score_bwd(const Tensor& P_src, const Tensor& dP_src, const Tensor& da_src, const Tensor& att_src,
+                          Tensor g_att_src, Tensor dPb_src, const Tensor& ctr_src, int64_t idx_src, const Tensor& da_dst,
+                          const Tensor& att_dst, Tensor g_att_dst, const Tensor& ctr_dst, int64_t idx_dst,
+                          const c10::optional<Tensor>& P_dst, const c10::optional<Tensor>& dPb_dst, int64_t heads) {
+  c10::cuda::CUDAGuard guard(P_src.device());
+  const int64_t H = P_src.size(1);
+  check_gat_width(H, heads);
+  check_rows(P_src, torch::kBFloat16, H, "gat_score_bwd: P must be contiguous bf16 [rows, H]");
+  check_rows(dP_src, torch::kFloat32, H, "gat_score_bwd: dP must be contiguous fp32 [rows, H]");
+  check_rows(dPb_src, torch::kBFloat16, H, "gat_score_bwd: dPb must be contiguous bf16 [rows, H]");
+  check_rows(da_src, torch::kFloat32, heads, "gat_score_bwd: da must be contiguous fp32 [rows, heads]");
+  check_rows(da_dst, torch::kFloat32, heads, "gat_score_bwd: da must be contiguous fp32 [rows, heads]");
+  TORCH_CHECK(dP_src.size(0) >= P_src.size(0) && dPb_src.size(0) >= P_src.size(0) && da_src.size(0) >= P_src.size(0),
+              "gat_score_bwd: source buffers have fewer rows than P");
+  for (const Tensor* t : {&att_src, &att_dst})
+    TORCH_CHECK(t->scalar_type() == torch::kBFloat16 && t->numel() == H && t->is_contiguous() &&
+                reinterpret_cast<uintptr_t>(t->data_ptr()) % 16 == 0, "gat_score_bwd: att must be 16-byte aligned bf16 [H]");
+  for (const Tensor* t : {&g_att_src, &g_att_dst})
+    TORCH_CHECK(t->scalar_type() == torch::kFloat32 && t->numel() == H && t->is_contiguous(),
+                "gat_score_bwd: attention gradients must be fp32 [H]");
+  GatScoreBwdArgs a{};
+  a.H = H; a.heads = heads;
+  auto& s = a.seg[0];
+  s.P = P_src.data_ptr(); s.dP = dP_src.data_ptr<float>(); s.da0 = da_src.data_ptr<float>();
+  s.att0 = att_src.data_ptr(); s.gatt0 = g_att_src.data_ptr<float>(); s.dPb = dPb_src.data_ptr();
+  s.cum = ctr_src.data_ptr<int32_t>(); s.idx = idx_src; s.cap = P_src.size(0);
+  if (has(P_dst)) {
+    TORCH_CHECK(has(dPb_dst), "gat_score_bwd: a separate destination projection needs dPb_dst");
+    check_rows(*P_dst, torch::kBFloat16, H, "gat_score_bwd: P must be contiguous bf16 [rows, H]");
+    check_rows(*dPb_dst, torch::kBFloat16, H, "gat_score_bwd: dPb must be contiguous bf16 [rows, H]");
+    TORCH_CHECK(dPb_dst->size(0) >= P_dst->size(0) && da_dst.size(0) >= P_dst->size(0),
+                "gat_score_bwd: destination buffers have fewer rows than P");
+    auto& d = a.seg[1];
+    d.P = P_dst->data_ptr(); d.da0 = da_dst.data_ptr<float>(); d.att0 = att_dst.data_ptr();
+    d.gatt0 = g_att_dst.data_ptr<float>(); d.dPb = dPb_dst->data_ptr();
+    d.cum = ctr_dst.data_ptr<int32_t>(); d.idx = idx_dst; d.cap = P_dst->size(0);
+  } else {
+    s.da1 = da_dst.data_ptr<float>(); s.att1 = att_dst.data_ptr(); s.gatt1 = g_att_dst.data_ptr<float>();
+    s.cum1 = ctr_dst.data_ptr<int32_t>(); s.idx1 = idx_dst;
+  }
+  launch_gat_score_bwd(a, cur_stream());
+  check_cuda_err("gat_score_bwd");
+}
+
+static void gat_act_bwd(const c10::optional<Tensor>& dH, const c10::optional<Tensor>& Z, Tensor dPre,
+                        const Tensor& counters, int64_t n_hops, double p, int64_t seed, int64_t layer,
+                        const c10::optional<Tensor>& step_dev, const c10::optional<Tensor>& bias_g) {
+  c10::cuda::CUDAGuard guard(dPre.device());
+  const int64_t d = dPre.size(1);
+  TORCH_CHECK(d % 64 == 0 && d >= 64 && d <= 1024, "gat_act_bwd: width must be a multiple of 64 in [64, 1024]");
+  check_rows(dPre, torch::kBFloat16, d, "gat_act_bwd: dPre must be contiguous bf16 [rows, d]");
+  TORCH_CHECK(p >= 0.0 && p < 1.0, "gat_act_bwd: dropout p must be in [0, 1)");
+  GatActBwdArgs a{};
+  a.dPre = dPre.data_ptr(); a.cum = counters.data_ptr<int32_t>(); a.n_hops = n_hops; a.cap = dPre.size(0); a.d = d;
+  if (has(dH)) {
+    TORCH_CHECK(has(Z), "gat_act_bwd: the activation backward needs Z");
+    check_rows(*dH, torch::kFloat32, d, "gat_act_bwd: dH must be contiguous fp32 [rows, d]");
+    check_rows(*Z, torch::kBFloat16, d, "gat_act_bwd: Z must be contiguous bf16 [rows, d]");
+    TORCH_CHECK(dH->size(0) >= dPre.size(0) && Z->size(0) >= dPre.size(0), "gat_act_bwd: dH / Z have fewer rows than dPre");
+    a.dH = dH->data_ptr<float>(); a.Z = Z->data_ptr();
+  }
+  a.slope = 0.01f;
+  a.thresh16 = static_cast<uint32_t>(p * 65536.0);
+  a.dscale = static_cast<float>(1.0 / (1.0 - p));
+  a.seed = static_cast<uint64_t>(seed);
+  a.layer = layer;
+  if (has(step_dev)) {
+    TORCH_CHECK(step_dev->scalar_type() == torch::kInt32 && step_dev->is_cuda(), "gat_act_bwd: int32 step_dev");
+    a.step_dev = step_dev->data_ptr<int32_t>();
+  }
+  if (has(bias_g)) {
+    TORCH_CHECK(bias_g->is_cuda() && bias_g->scalar_type() == torch::kFloat32 && bias_g->is_contiguous() &&
+                bias_g->numel() % d == 0 && bias_g->numel() > 0, "gat_act_bwd: bias_g must be fp32 [n_bias * d]");
+    a.bias_g = bias_g->data_ptr<float>();
+    a.n_bias = bias_g->numel() / d;
+  }
+  launch_gat_act_bwd(a, cur_stream());
+  check_cuda_err("gat_act_bwd");
+}
+
 // Link-prediction seeds of one batch (cuda/link.cu): pos int64 [2, B] -> seeds int64 [2 (1 + k) B], n_pairs int32.
 // `step` is the arena's device step, read before the arena's sample() advances it.
 static void link_seeds(GraphHandle* graph, const Tensor& pos, int64_t num_nodes, int64_t neg_ratio, int64_t seed,
@@ -1681,6 +1913,24 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("set_pdl", [](bool on) { return set_pdl(on ? 1 : 0) != 0; });
   m.def("sage_gather_bwd", &sage_gather_bwd, py::arg("dA"), py::arg("d"), py::arg("arena"), py::arg("n_hops_targets"),
         py::arg("Z"), py::arg("dPre"), py::arg("colsum"), py::arg("prezeroed") = false, py::arg("gscale") = 1.0);
+  m.def("gat_scores", &gat_scores, py::arg("P0"), py::arg("att0"), py::arg("out0"), py::arg("counters0"),
+        py::arg("idx0"), py::arg("P1") = py::none(), py::arg("att1") = py::none(), py::arg("out1") = py::none(),
+        py::arg("counters1") = py::none(), py::arg("idx1") = 0, py::arg("zero") = py::none(), py::arg("heads") = 1);
+  m.def("gat_aggregate", &gat_aggregate, py::arg("P"), py::arg("as_"), py::arg("ad"), py::arg("heads"),
+        py::arg("counters"), py::arg("n_hops_targets"), py::arg("ell"), py::arg("ks"), py::arg("deg"), py::arg("alpha"),
+        py::arg("acc") = py::none(), py::arg("first") = true, py::arg("last") = true, py::arg("bias") = py::none(),
+        py::arg("act") = false, py::arg("p") = 0.0, py::arg("seed") = 0, py::arg("layer") = 0,
+        py::arg("step_dev") = py::none(), py::arg("Z") = py::none());
+  m.def("gat_backward", &gat_backward, py::arg("G"), py::arg("P"), py::arg("heads"), py::arg("counters"),
+        py::arg("n_hops_targets"), py::arg("ell"), py::arg("ks"), py::arg("deg"), py::arg("alpha"), py::arg("dal"),
+        py::arg("dP"), py::arg("da_src"), py::arg("da_dst"));
+  m.def("gat_score_bwd", &gat_score_bwd, py::arg("P_src"), py::arg("dP_src"), py::arg("da_src"), py::arg("att_src"),
+        py::arg("g_att_src"), py::arg("dPb_src"), py::arg("ctr_src"), py::arg("idx_src"), py::arg("da_dst"),
+        py::arg("att_dst"), py::arg("g_att_dst"), py::arg("ctr_dst"), py::arg("idx_dst"), py::arg("P_dst") = py::none(),
+        py::arg("dPb_dst") = py::none(), py::arg("heads") = 1);
+  m.def("gat_act_bwd", &gat_act_bwd, py::arg("dH"), py::arg("Z"), py::arg("dPre"), py::arg("counters"),
+        py::arg("n_hops"), py::arg("p") = 0.0, py::arg("seed") = 0, py::arg("layer") = 0,
+        py::arg("step_dev") = py::none(), py::arg("bias_g") = py::none());
   m.def("bias_relu", &bias_relu);
   m.def("softmax_nll", &softmax_nll, py::arg("logits"), py::arg("C"), py::arg("y"), py::arg("labels_all"),
         py::arg("nodes"), py::arg("counters"), py::arg("loss"), py::arg("dlogits"), py::arg("correct"),

@@ -326,6 +326,111 @@ void launch_link_seeds(GraphTable g, const int64_t* pos, int B, int k, int64_t n
 void launch_link_bce(const void* Z, int ld, int C, const int32_t* seed_local, int P, int B, const int32_t* n_pairs,
                      float* loss, int32_t* correct, float* dZ, cudaStream_t s);
 
+// ---- gat.cu (relational GAT engine kernels; H = heads * C, H a multiple of 64 in [64, 1024], C % 8 == 0) -----------
+// Per-node attention scores of two row sets: out[set][row * heads + h] = <att[set][h], P[set][row, h*C : (h+1)*C]>
+// for row < min(cum[set][idx[set]], cap[set]).  P[1] == nullptr skips the second set.  zero (optional, fp32
+// [cap[0], heads]) is cleared on the valid rows of set 0.
+struct GatScoreArgs {
+  const void* P[2];             // bf16 [cap, H]
+  const void* att[2];           // bf16 [H]
+  float* out[2];                // fp32 [cap, heads]
+  const int32_t* cum[2];
+  int idx[2], cap[2];
+  float* zero;
+  int H, heads;
+};
+void launch_gat_scores(const GatScoreArgs& a, cudaStream_t s);
+
+// Attention aggregation of one relation over its per-hop ELL blocks (targets t < min(cum[n_hops_targets],
+// cap_targets)).  alpha[h]: fp32 [rows of hop h, k[h], heads] softmax weights, sign bit = (score <= 0).  Output:
+// first/last select write / accumulate into acc (fp32 [cap, H]) / finish: Z = bf16(act(acc + out + sum_b bias[b])),
+// act = inverted dropout(leaky_relu(., 0.01)) with the Philox key of launch_dropout_bf16 (thresh16 = 0: no dropout).
+struct GatAggArgs {
+  const void* P;                // bf16 [n_src, H] source projections
+  const float* as;              // fp32 [n_src, heads]
+  const float* ad;              // fp32 [cap_targets, heads]
+  int H, heads;
+  const int32_t* cum;
+  int n_hops_targets, cap_targets;
+  const int32_t* ell[4];
+  int k[4];
+  const int32_t* deg;
+  float* alpha[4];
+  float* acc;
+  int first, last;
+  const void* bias;             // bf16 [n_bias, H]
+  int n_bias;
+  int act;
+  uint32_t thresh16;
+  float dscale;
+  uint64_t seed;
+  int layer;
+  const int32_t* step_dev;
+  void* z;                      // bf16 [cap_targets, H]
+};
+void launch_gat_aggregate(const GatAggArgs& a, cudaStream_t s);
+
+// Backward of the attention aggregation given G (bf16 [cap_targets, H]): dP += alpha G (fp32 red.add into source
+// rows), da_src[s, h] += dscore (atomics), da_dst[t, h] = sum_j dscore; dal (alpha's layout) is scratch.
+struct GatBwdArgs {
+  const void* G;
+  const void* P;
+  int H, heads;
+  const int32_t* cum;
+  int n_hops_targets, cap_targets;
+  const int32_t* ell[4];
+  int k[4];
+  const int32_t* deg;
+  const float* alpha[4];
+  float* dal[4];
+  float* dP;                    // fp32 [n_src, H]
+  float* da_src;                // fp32 [n_src, heads]
+  float* da_dst;                // fp32 [cap_targets, heads]
+};
+void launch_gat_backward(const GatBwdArgs& a, cudaStream_t s);
+
+// Projection gradients of one relation (see gat.cu): seg[0] = source rows (dP != nullptr: adds and re-zeroes the
+// fp32 rows of k_gat_backward), seg[1] = separate destination rows (P == nullptr: none).  Term 0 is always present;
+// term 1 (da1 != nullptr) folds the destination scores into the source rows when both ends share the projection.
+struct GatScoreBwdArgs {
+  struct Seg {
+    const void* P;              // bf16 [cap, H] projection
+    float* dP;                  // fp32 [cap, H] or nullptr
+    const float* da0;           // fp32 [cap, heads]
+    const void* att0;           // bf16 [H]
+    float* gatt0;               // fp32 [H] gradient of att0 (accumulated)
+    const float* da1;
+    const void* att1;
+    float* gatt1;
+    const int32_t* cum1;        // rows carrying term 1: min(cum1[idx1], rows)
+    int idx1;
+    void* dPb;                  // bf16 [cap, H] output
+    const int32_t* cum;
+    int idx, cap;
+  } seg[2];
+  int H, heads;
+};
+void launch_gat_score_bwd(const GatScoreBwdArgs& a, cudaStream_t s);
+
+// Activation backward of a GAT layer output Z (bf16 [cap, d]) and the column sums of its gradient into n_bias bias
+// gradient slots (bias_g fp32 [n_bias, d], accumulated).  dH == nullptr: dPre is an input (no activation).
+struct GatActBwdArgs {
+  const float* dH;
+  const void* Z;
+  void* dPre;
+  const int32_t* cum;
+  int n_hops, cap, d;
+  float slope;
+  uint32_t thresh16;
+  float dscale;
+  uint64_t seed;
+  int layer;
+  const int32_t* step_dev;
+  float* bias_g;
+  int n_bias;
+};
+void launch_gat_act_bwd(const GatActBwdArgs& a, cudaStream_t s);
+
 // ---- peer.cu (collectives over NVLink peer memory, CUDA-graph capturable) ------
 struct PeerPtrs {
   int world, rank;

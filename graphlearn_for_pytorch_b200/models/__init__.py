@@ -5,3 +5,4 @@ from .rgnn import RGNN, RelSAGEConv, RelGCNConv, RelGATConv
 from .seal import drnl_node_labeling, DGCNN
 from .hgt import HGT, HGTConv
 from .hetero_engine import HeteroSageEngine
+from .hetero_gat_engine import HeteroGatEngine

@@ -188,7 +188,12 @@ class HeteroSageEngine(object):
       if l == self.L and self.n_out_pad > self.C:
         w[self.C:] = 0
       self.p32[off:off + n * k].copy_(w.flatten())
-    pad = (-sizes) % 4
+    self._init_optimizer_state()
+
+  def _init_optimizer_state(self):
+    """bf16 shadow, gradient and Adam buffers of the flat fp32 parameters `p32` (and the peer group when world > 1)."""
+    dev = self.device
+    pad = (-self.p32.numel()) % 4
     self.p16 = self.p32.to(torch.bfloat16)
     self.g32 = torch.zeros_like(self.p32)
     if self.world > 1:
