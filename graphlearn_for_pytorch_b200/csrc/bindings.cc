@@ -1259,6 +1259,219 @@ static void gat_act_bwd(const c10::optional<Tensor>& dH, const c10::optional<Ten
   check_cuda_err("gat_act_bwd");
 }
 
+// ---- HGT (cuda/hgt.cu) ------------------------------------------------------------------------------------------
+// Per relation into the destination type: kv = the source rows [K | Q | V] (bf16 [rows, 3H]), prior (fp32 [heads]),
+// the per-hop ELL blocks and fan-outs, deg, and the per-hop alpha buffers.
+template <typename RelT>
+static void hgt_fill_rels(RelT* rel, int64_t H, int64_t heads, const std::vector<Tensor>& kv,
+                          const std::vector<Tensor>& prior, const std::vector<std::vector<Tensor>>& ell,
+                          const std::vector<std::vector<int64_t>>& ks, const std::vector<Tensor>& deg,
+                          const std::vector<std::vector<Tensor>>& alpha, int64_t n_hops) {
+  const size_t R = kv.size();
+  TORCH_CHECK(R >= 1 && R <= static_cast<size_t>(kHgtMaxRel), "hgt: a destination type takes 1 to 8 relations");
+  TORCH_CHECK(prior.size() == R && ell.size() == R && ks.size() == R && deg.size() == R && alpha.size() == R,
+              "hgt: kv, prior, ell, ks, deg and alpha need one entry per relation");
+  for (size_t r = 0; r < R; ++r) {
+    check_rows(kv[r], torch::kBFloat16, 3 * H, "hgt: source rows must be contiguous bf16 [rows, 3H] = [K | Q | V]");
+    TORCH_CHECK(prior[r].is_cuda() && prior[r].scalar_type() == torch::kFloat32 && prior[r].numel() == heads &&
+                prior[r].is_contiguous(), "hgt: prior must be fp32 [heads]");
+    TORCH_CHECK(deg[r].is_cuda() && deg[r].scalar_type() == torch::kInt32, "hgt: deg must be int32");
+    TORCH_CHECK(static_cast<int64_t>(ell[r].size()) == n_hops, "hgt: one ELL block per target hop");
+    rel[r].kv = kv[r].data_ptr();
+    rel[r].prior = prior[r].data_ptr<float>();
+    rel[r].deg = deg[r].data_ptr<int32_t>();
+    fill_ell(ell[r], ks[r], rel[r].ell, rel[r].k);
+    float* al[4];
+    gat_fill_hops(ell[r], ks[r], alpha[r], heads, al);
+    for (int h = 0; h < 4; ++h) rel[r].alpha[h] = al[h];
+  }
+}
+
+static void check_hgt_width(int64_t H, int64_t heads) {
+  TORCH_CHECK(H % 64 == 0 && H >= 64 && H <= 1024 && heads >= 1 && H % heads == 0 && (H / heads) % 8 == 0,
+              "hgt: H must be a multiple of 64 in [64, 1024] and heads must divide H into head widths D with D % 8 == 0");
+}
+
+static void hgt_attention(const Tensor& qq, Tensor u, int64_t heads, const Tensor& counters, int64_t n_hops_targets,
+                          const std::vector<Tensor>& kv, const std::vector<Tensor>& prior,
+                          const std::vector<std::vector<Tensor>>& ell, const std::vector<std::vector<int64_t>>& ks,
+                          const std::vector<Tensor>& deg, const std::vector<std::vector<Tensor>>& alpha) {
+  c10::cuda::CUDAGuard guard(qq.device());
+  const int64_t R = static_cast<int64_t>(kv.size());
+  TORCH_CHECK(R >= 1 && R <= kHgtMaxRel, "hgt: a destination type takes 1 to 8 relations");
+  TORCH_CHECK(qq.dim() == 2 && qq.size(1) % R == 0, "hgt_attention: qq must be [rows, n_rel * H]");
+  const int64_t H = qq.size(1) / R;
+  check_hgt_width(H, heads);
+  check_rows(qq, torch::kBFloat16, R * H, "hgt_attention: qq must be contiguous bf16 [rows, n_rel * H]");
+  check_rows(u, torch::kBFloat16, R * H, "hgt_attention: u must be contiguous bf16 [rows, n_rel * H]");
+  HgtAttnArgs a{};
+  a.qq = qq.data_ptr(); a.u = u.data_ptr();
+  a.H = H; a.heads = heads; a.n_rel = R; a.kv_ld = 3 * H; a.v_off = 2 * H;
+  a.scale = static_cast<float>(1.0 / std::sqrt(static_cast<double>(H / heads)));
+  a.cum = counters.data_ptr<int32_t>();
+  a.n_hops_targets = n_hops_targets;
+  a.cap_targets = std::min<int64_t>(qq.size(0), u.size(0));
+  hgt_fill_rels(a.rel, H, heads, kv, prior, ell, ks, deg, alpha, n_hops_targets);
+  launch_hgt_attention(a, cur_stream());
+  check_cuda_err("hgt_attention");
+}
+
+static void hgt_attention_bwd(const Tensor& du, const Tensor& qq, Tensor dqq, int64_t heads, const Tensor& counters,
+                              int64_t n_hops_targets, const std::vector<Tensor>& kv, const std::vector<Tensor>& prior,
+                              const std::vector<std::vector<Tensor>>& ell,
+                              const std::vector<std::vector<int64_t>>& ks, const std::vector<Tensor>& deg,
+                              const std::vector<std::vector<Tensor>>& alpha, const std::vector<std::vector<Tensor>>& dal,
+                              const std::vector<Tensor>& dkv, const std::vector<Tensor>& dprior) {
+  c10::cuda::CUDAGuard guard(qq.device());
+  const int64_t R = static_cast<int64_t>(kv.size());
+  TORCH_CHECK(R >= 1 && R <= kHgtMaxRel, "hgt: a destination type takes 1 to 8 relations");
+  TORCH_CHECK(qq.dim() == 2 && qq.size(1) % R == 0, "hgt_attention_bwd: qq must be [rows, n_rel * H]");
+  const int64_t H = qq.size(1) / R;
+  check_hgt_width(H, heads);
+  check_rows(qq, torch::kBFloat16, R * H, "hgt_attention_bwd: qq must be contiguous bf16 [rows, n_rel * H]");
+  check_rows(du, torch::kBFloat16, R * H, "hgt_attention_bwd: du must be contiguous bf16 [rows, n_rel * H]");
+  check_rows(dqq, torch::kBFloat16, R * H, "hgt_attention_bwd: dqq must be contiguous bf16 [rows, n_rel * H]");
+  TORCH_CHECK(dal.size() == static_cast<size_t>(R) && dkv.size() == static_cast<size_t>(R) &&
+              dprior.size() == static_cast<size_t>(R), "hgt_attention_bwd: dal, dkv and dprior need one entry per relation");
+  HgtAttnBwdArgs a{};
+  a.du = du.data_ptr(); a.qq = qq.data_ptr(); a.dqq = dqq.data_ptr();
+  a.H = H; a.heads = heads; a.n_rel = R; a.kv_ld = 3 * H; a.v_off = 2 * H;
+  a.scale = static_cast<float>(1.0 / std::sqrt(static_cast<double>(H / heads)));
+  a.cum = counters.data_ptr<int32_t>();
+  a.n_hops_targets = n_hops_targets;
+  a.cap_targets = std::min<int64_t>(std::min<int64_t>(qq.size(0), du.size(0)), dqq.size(0));
+  hgt_fill_rels(a.rel, H, heads, kv, prior, ell, ks, deg, alpha, n_hops_targets);
+  for (int64_t r = 0; r < R; ++r) {
+    TORCH_CHECK(dal[r].size() == ell[r].size(), "hgt_attention_bwd: one dal buffer per hop");
+    for (size_t h = 0; h < 4; ++h) a.rel[r].dal[h] = nullptr;
+    for (size_t h = 0; h < dal[r].size(); ++h) {
+      TORCH_CHECK(dal[r][h].is_cuda() && dal[r][h].scalar_type() == torch::kFloat32 && dal[r][h].is_contiguous() &&
+                  dal[r][h].numel() >= 2 * ell[r][h].numel() * heads &&
+                  reinterpret_cast<uintptr_t>(dal[r][h].data_ptr()) % 8 == 0,
+                  "hgt_attention_bwd: dal buffers must be fp32 [ELL slots of the hop, heads, 2]");
+      a.rel[r].dal[h] = dal[r][h].data_ptr<float>();
+    }
+    check_rows(dkv[r], torch::kFloat32, 2 * H, "hgt_attention_bwd: dkv must be contiguous fp32 [rows, 2H]");
+    TORCH_CHECK(dkv[r].size(0) >= kv[r].size(0), "hgt_attention_bwd: dkv has fewer rows than the source rows");
+    TORCH_CHECK(dprior[r].is_cuda() && dprior[r].scalar_type() == torch::kFloat32 && dprior[r].numel() == heads,
+                "hgt_attention_bwd: dprior must be fp32 [heads]");
+    a.rel[r].dkv = dkv[r].data_ptr<float>();
+    a.rel[r].dprior = dprior[r].data_ptr<float>();
+  }
+  launch_hgt_attention_bwd(a, cur_stream());
+  check_cuda_err("hgt_attention_bwd");
+}
+
+static void hgt_gelu(const Tensor& X, Tensor Y, const Tensor& counters, int64_t n_hops, const c10::optional<Tensor>& dY) {
+  c10::cuda::CUDAGuard guard(X.device());
+  const int64_t d = X.size(1);
+  TORCH_CHECK(d % 8 == 0, "hgt_gelu: width must be a multiple of 8");
+  check_rows(X, torch::kBFloat16, d, "hgt_gelu: X must be contiguous bf16 [rows, d]");
+  check_rows(Y, torch::kBFloat16, d, "hgt_gelu: Y must be contiguous bf16 [rows, d]");
+  int64_t cap = std::min<int64_t>(X.size(0), Y.size(0));
+  if (has(dY)) {
+    check_rows(*dY, torch::kBFloat16, d, "hgt_gelu: dY must be contiguous bf16 [rows, d]");
+    cap = std::min<int64_t>(cap, dY->size(0));
+  }
+  launch_hgt_gelu(X.data_ptr(), Y.data_ptr(), counters.data_ptr<int32_t>(), n_hops, cap, d,
+                  has(dY) ? dY->data_ptr() : nullptr, cur_stream());
+  check_cuda_err("hgt_gelu");
+}
+
+static void hgt_gate(const Tensor& A, const Tensor& X, Tensor out, const Tensor& skip, const Tensor& counters,
+                     int64_t n_hops, const c10::optional<Tensor>& dZ, const c10::optional<Tensor>& dX,
+                     const c10::optional<Tensor>& skip_g) {
+  c10::cuda::CUDAGuard guard(A.device());
+  const int64_t d = A.size(1);
+  TORCH_CHECK(d % 8 == 0, "hgt_gate: width must be a multiple of 8");
+  check_rows(A, torch::kBFloat16, d, "hgt_gate: A must be contiguous bf16 [rows, d]");
+  check_rows(X, torch::kBFloat16, d, "hgt_gate: X must be contiguous bf16 [rows, d]");
+  check_rows(out, torch::kBFloat16, d, "hgt_gate: out must be contiguous bf16 [rows, d]");
+  TORCH_CHECK(skip.is_cuda() && skip.scalar_type() == torch::kFloat32 && skip.numel() == 1, "hgt_gate: skip must be fp32 [1]");
+  HgtGateArgs a{};
+  a.A = A.data_ptr(); a.X = X.data_ptr(); a.out = out.data_ptr(); a.skip = skip.data_ptr<float>();
+  a.cum = counters.data_ptr<int32_t>(); a.n_hops = n_hops; a.d = d;
+  int64_t cap = std::min<int64_t>(std::min<int64_t>(A.size(0), X.size(0)), out.size(0));
+  if (has(dZ)) {
+    TORCH_CHECK(dZ->is_cuda() && dZ->is_contiguous() && dZ->dim() == 2 && dZ->size(1) == d &&
+                (dZ->scalar_type() == torch::kFloat32 || dZ->scalar_type() == torch::kBFloat16),
+                "hgt_gate: dZ must be contiguous fp32 or bf16 [rows, d]");
+    cap = std::min<int64_t>(cap, dZ->size(0));
+    if (dZ->scalar_type() == torch::kFloat32) a.dZ32 = dZ->data_ptr<float>(); else a.dZ16 = dZ->data_ptr();
+    if (has(dX)) {
+      check_rows(*dX, torch::kFloat32, d, "hgt_gate: dX must be contiguous fp32 [rows, d]");
+      cap = std::min<int64_t>(cap, dX->size(0));
+      a.dX = dX->data_ptr<float>();
+    }
+    if (has(skip_g)) {
+      TORCH_CHECK(skip_g->is_cuda() && skip_g->scalar_type() == torch::kFloat32 && skip_g->numel() == 1,
+                  "hgt_gate: skip_g must be fp32 [1]");
+      a.skip_g = skip_g->data_ptr<float>();
+    }
+  }
+  a.cap = cap;
+  launch_hgt_gate(a, cur_stream());
+  check_cuda_err("hgt_gate");
+}
+
+// Block-diagonal images of a (layer, type)'s relation transforms (att, msg bf16 [n_rel, heads, D, D]); with the
+// gradient arguments, the inverse map of the dense fp32 GEMM weight gradients into att_g / msg_g instead.
+static void hgt_blocks(const Tensor& att, const Tensor& msg, Tensor att_img, Tensor msg_img,
+                       const c10::optional<Tensor>& att_dense, const c10::optional<Tensor>& msg_dense,
+                       const c10::optional<Tensor>& att_g, const c10::optional<Tensor>& msg_g) {
+  c10::cuda::CUDAGuard guard(att.device());
+  TORCH_CHECK(att.dim() == 4 && att.size(2) == att.size(3) && msg.sizes() == att.sizes() && att.is_contiguous() &&
+              msg.is_contiguous() && att.scalar_type() == torch::kBFloat16 && msg.scalar_type() == torch::kBFloat16,
+              "hgt_blocks: att and msg must be contiguous bf16 [n_rel, heads, D, D]");
+  const int64_t R = att.size(0), heads = att.size(1), D = att.size(2), H = heads * D;
+  TORCH_CHECK(R >= 1 && R <= kHgtMaxRel, "hgt: a destination type takes 1 to 8 relations");
+  check_hgt_width(H, heads);
+  check_rows(att_img, torch::kBFloat16, H, "hgt_blocks: att_img must be contiguous bf16 [n_rel * H, H]");
+  check_rows(msg_img, torch::kBFloat16, R * H, "hgt_blocks: msg_img must be contiguous bf16 [H, n_rel * H]");
+  TORCH_CHECK(att_img.size(0) == R * H && msg_img.size(0) == H, "hgt_blocks: image shapes");
+  HgtBlockArgs a{};
+  a.att = att.data_ptr(); a.msg = msg.data_ptr(); a.att_img = att_img.data_ptr(); a.msg_img = msg_img.data_ptr();
+  a.n_rel = R; a.heads = heads; a.D = D;
+  if (has(att_g)) {
+    TORCH_CHECK(has(msg_g) && has(att_dense) && has(msg_dense), "hgt_blocks: the gradient map needs all four buffers");
+    for (const Tensor* t : {&*att_g, &*msg_g})
+      TORCH_CHECK(t->is_cuda() && t->scalar_type() == torch::kFloat32 && t->is_contiguous() && t->numel() == R * H * D,
+                  "hgt_blocks: att_g / msg_g must be fp32 [n_rel, heads, D, D]");
+    for (const Tensor* t : {&*att_dense, &*msg_dense})
+      TORCH_CHECK(t->is_cuda() && t->scalar_type() == torch::kFloat32 && t->is_contiguous() && t->numel() == R * H * H,
+                  "hgt_blocks: the dense gradients must be fp32 [n_rel * H, H] / [H, n_rel * H]");
+    a.att_dense = att_dense->data_ptr<float>(); a.msg_dense = msg_dense->data_ptr<float>();
+    a.att_g = att_g->data_ptr<float>(); a.msg_g = msg_g->data_ptr<float>();
+  }
+  launch_hgt_blocks(a, cur_stream());
+  check_cuda_err("hgt_blocks");
+}
+
+static void hgt_kqv_cast(Tensor dkv, const c10::optional<Tensor>& dq, Tensor out, const c10::optional<Tensor>& bias_g,
+                         const Tensor& counters, int64_t idx, int64_t idx_q) {
+  c10::cuda::CUDAGuard guard(dkv.device());
+  TORCH_CHECK(out.dim() == 2 && out.size(1) % 3 == 0, "hgt_kqv_cast: out must be [rows, 3H]");
+  const int64_t H = out.size(1) / 3;
+  TORCH_CHECK(H % 64 == 0 && H >= 64 && H <= 1024, "hgt_kqv_cast: H must be a multiple of 64 in [64, 1024]");
+  check_rows(out, torch::kBFloat16, 3 * H, "hgt_kqv_cast: out must be contiguous bf16 [rows, 3H]");
+  check_rows(dkv, torch::kFloat32, 2 * H, "hgt_kqv_cast: dkv must be contiguous fp32 [rows, 2H]");
+  HgtKqvCastArgs a{};
+  a.dkv = dkv.data_ptr<float>(); a.out = out.data_ptr(); a.cum = counters.data_ptr<int32_t>();
+  a.idx = idx; a.idx_q = idx_q; a.H = H;
+  a.cap = std::min<int64_t>(out.size(0), dkv.size(0));
+  if (has(dq)) {
+    check_rows(*dq, torch::kBFloat16, H, "hgt_kqv_cast: dq must be contiguous bf16 [rows, H]");
+    a.dq = dq->data_ptr();
+  }
+  if (has(bias_g)) {
+    TORCH_CHECK(bias_g->is_cuda() && bias_g->scalar_type() == torch::kFloat32 && bias_g->numel() == 3 * H &&
+                bias_g->is_contiguous(), "hgt_kqv_cast: bias_g must be fp32 [3H]");
+    a.bias_g = bias_g->data_ptr<float>();
+  }
+  launch_hgt_kqv_cast(a, cur_stream());
+  check_cuda_err("hgt_kqv_cast");
+}
+
 // Link-prediction seeds of one batch (cuda/link.cu): pos int64 [2, B] -> seeds int64 [2 (1 + k) B], n_pairs int32.
 // `step` is the arena's device step, read before the arena's sample() advances it.
 static void link_seeds(GraphHandle* graph, const Tensor& pos, int64_t num_nodes, int64_t neg_ratio, int64_t seed,
@@ -1931,6 +2144,21 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("gat_act_bwd", &gat_act_bwd, py::arg("dH"), py::arg("Z"), py::arg("dPre"), py::arg("counters"),
         py::arg("n_hops"), py::arg("p") = 0.0, py::arg("seed") = 0, py::arg("layer") = 0,
         py::arg("step_dev") = py::none(), py::arg("bias_g") = py::none());
+  m.def("hgt_attention", &hgt_attention, py::arg("qq"), py::arg("u"), py::arg("heads"), py::arg("counters"),
+        py::arg("n_hops_targets"), py::arg("kv"), py::arg("prior"), py::arg("ell"), py::arg("ks"), py::arg("deg"),
+        py::arg("alpha"));
+  m.def("hgt_attention_bwd", &hgt_attention_bwd, py::arg("du"), py::arg("qq"), py::arg("dqq"), py::arg("heads"),
+        py::arg("counters"), py::arg("n_hops_targets"), py::arg("kv"), py::arg("prior"), py::arg("ell"), py::arg("ks"),
+        py::arg("deg"), py::arg("alpha"), py::arg("dal"), py::arg("dkv"), py::arg("dprior"));
+  m.def("hgt_gelu", &hgt_gelu, py::arg("X"), py::arg("Y"), py::arg("counters"), py::arg("n_hops"),
+        py::arg("dY") = py::none());
+  m.def("hgt_gate", &hgt_gate, py::arg("A"), py::arg("X"), py::arg("out"), py::arg("skip"), py::arg("counters"),
+        py::arg("n_hops"), py::arg("dZ") = py::none(), py::arg("dX") = py::none(), py::arg("skip_g") = py::none());
+  m.def("hgt_blocks", &hgt_blocks, py::arg("att"), py::arg("msg"), py::arg("att_img"), py::arg("msg_img"),
+        py::arg("att_dense") = py::none(), py::arg("msg_dense") = py::none(), py::arg("att_g") = py::none(),
+        py::arg("msg_g") = py::none());
+  m.def("hgt_kqv_cast", &hgt_kqv_cast, py::arg("dkv"), py::arg("dq"), py::arg("out"), py::arg("bias_g"),
+        py::arg("counters"), py::arg("idx"), py::arg("idx_q"));
   m.def("bias_relu", &bias_relu);
   m.def("softmax_nll", &softmax_nll, py::arg("logits"), py::arg("C"), py::arg("y"), py::arg("labels_all"),
         py::arg("nodes"), py::arg("counters"), py::arg("loss"), py::arg("dlogits"), py::arg("correct"),

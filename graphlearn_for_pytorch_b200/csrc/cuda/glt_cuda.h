@@ -431,6 +431,101 @@ struct GatActBwdArgs {
 };
 void launch_gat_act_bwd(const GatActBwdArgs& a, cudaStream_t s);
 
+// ---- hgt.cu (HGT engine kernels; H = heads * D, H a multiple of 64 in [64, 1024], D % 8 == 0) ----------------------
+// Cross-relation attention of one (layer, destination type) over its n_rel <= kHgtMaxRel incoming relations, targets
+// t < min(cum[n_hops_targets], cap_targets).  Source rows are bf16 [n_src, kv_ld] with K at column 0 and V at column
+// v_off.  s = <qq_r[t, h], k_j,h> prior_r[h] scale; alpha (fp32 [rows of hop h, k[h], heads] per relation) is the
+// softmax over the slots of every relation; u_r[t] = sum_j alpha v_j (bf16 [cap_targets, n_rel * H]).
+constexpr int kHgtMaxRel = 8;
+struct HgtAttnArgs {
+  const void* qq;               // bf16 [cap_targets, n_rel * H]
+  void* u;                      // bf16 [cap_targets, n_rel * H]
+  int H, heads, n_rel, kv_ld, v_off;
+  float scale;                  // 1 / sqrt(D)
+  const int32_t* cum;
+  int n_hops_targets, cap_targets;
+  struct Rel {
+    const void* kv;
+    const float* prior;         // fp32 [heads]
+    const int32_t* deg;
+    const int32_t* ell[4];
+    int k[4];
+    float* alpha[4];
+  } rel[kHgtMaxRel];
+};
+void launch_hgt_attention(const HgtAttnArgs& a, cudaStream_t s);
+
+// Backward of launch_hgt_attention given dU (bf16 [cap_targets, n_rel * H]): dqq (bf16, rows [T, round_up(T, 128))
+// zeroed), dK / dV added with red.add into fp32 rows dkv [n_src, 2H] = [dK | dV], dprior [heads] accumulated (one
+// atomic per (relation, head) per CTA); dal (two floats per alpha entry) is scratch.
+struct HgtAttnBwdArgs {
+  const void* du;
+  const void* qq;
+  void* dqq;
+  int H, heads, n_rel, kv_ld, v_off;
+  float scale;
+  const int32_t* cum;
+  int n_hops_targets, cap_targets;
+  struct Rel {
+    const void* kv;
+    const float* prior;
+    const int32_t* deg;
+    const int32_t* ell[4];
+    int k[4];
+    const float* alpha[4];
+    float* dal[4];
+    float* dkv;
+    float* dprior;
+  } rel[kHgtMaxRel];
+};
+void launch_hgt_attention_bwd(const HgtAttnBwdArgs& a, cudaStream_t s);
+
+// dY == nullptr: Y = gelu(X) (exact erf) on rows < T.  dY given: Y = bf16(dY gelu'(X)), rows [T, round_up(T, 128)) = 0.
+void launch_hgt_gelu(const void* X, void* Y, const int32_t* cum, int n_hops, int cap, int d, const void* dY,
+                     cudaStream_t s);
+
+// Gated skip connection (see hgt.cu): forward out = sigmoid(skip) A + (1 - sigmoid(skip)) X; backward (dZ32 or dZ16)
+// out = dA, dX += (1 - sigmoid(skip)) dZ, skip_g += sum dZ (A - X) sigmoid'(skip).
+struct HgtGateArgs {
+  const void* A;                // bf16 [cap, d]
+  const void* X;                // bf16 [cap, d]
+  void* out;                    // bf16 [cap, d]
+  const float* skip;            // fp32 scalar
+  const float* dZ32;
+  const void* dZ16;
+  float* dX;                    // fp32 [cap, d] or nullptr
+  float* skip_g;
+  const int32_t* cum;
+  int n_hops, cap, d;
+};
+void launch_hgt_gate(const HgtGateArgs& a, cudaStream_t s);
+
+// Block-diagonal relation images (att_g == nullptr) or the inverse map of their dense fp32 gradients (see hgt.cu).
+struct HgtBlockArgs {
+  const void* att;              // bf16 [n_rel, heads, D, D]
+  const void* msg;
+  void* att_img;                // bf16 [n_rel * H, H]
+  void* msg_img;                // bf16 [H, n_rel * H]
+  float* att_dense;             // fp32 [n_rel * H, H]
+  float* msg_dense;             // fp32 [H, n_rel * H]
+  float* att_g;                 // fp32 [n_rel, heads, D, D]
+  float* msg_g;
+  int n_rel, heads, D;
+};
+void launch_hgt_blocks(const HgtBlockArgs& a, cudaStream_t s);
+
+// bf16 [cap, 3H] = [dK | dQ | dV] from fp32 dkv [cap, 2H] (rows < min(cum[idx], cap), re-zeroed) and bf16 dq [., H]
+// (rows < cum[idx_q]; nullptr: none); bias_g [3H] accumulates the column sums.
+struct HgtKqvCastArgs {
+  float* dkv;
+  const void* dq;
+  void* out;
+  float* bias_g;
+  const int32_t* cum;
+  int idx, idx_q, cap, H;
+};
+void launch_hgt_kqv_cast(const HgtKqvCastArgs& a, cudaStream_t s);
+
 // ---- peer.cu (collectives over NVLink peer memory, CUDA-graph capturable) ------
 struct PeerPtrs {
   int world, rank;

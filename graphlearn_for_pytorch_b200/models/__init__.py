@@ -6,3 +6,4 @@ from .seal import drnl_node_labeling, DGCNN
 from .hgt import HGT, HGTConv
 from .hetero_engine import HeteroSageEngine
 from .hetero_gat_engine import HeteroGatEngine
+from .hetero_hgt_engine import HeteroHgtEngine
