@@ -1670,14 +1670,23 @@ static void sage_fused(RowTableHandle* feat, const c10::optional<Tensor>& nodes,
 // ---------------------------------------------------------------------------
 // TcGemm: a cached launch of the TMA-fed wgmma GEMM kernel (csrc/cuda/tc_gemm.cu) over fixed engine buffers.
 // Tensor maps are encoded once; the batch-dependent extent is read from the sampler's device counters, so
-// run() is a single static launch (CUDA-graph capturable).  Up to two problems share a launch.
+// run() is a single static launch (CUDA-graph capturable).  Up to two problems share a launch.  The plan owns the
+// kernel's 8-byte work ticket, which the kernel leaves zeroed: launches of one plan must therefore be ordered (never
+// two in flight at once; every engine runs a plan on one stream).  GLT_B200_GEMM_TICKETS=0 keeps the static
+// item striding instead, for A/B measurements.
 // ---------------------------------------------------------------------------
 struct TcGemm {
   TcGemmLaunch L;
   int device;
   std::vector<Tensor> keep;   // keeps every operand alive
+  Tensor tickets;
   explicit TcGemm(int dev) : device(dev) {
     std::memset(&L, 0, sizeof(L));
+    const char* env = std::getenv("GLT_B200_GEMM_TICKETS");
+    if (!env || std::atoi(env) != 0) {
+      tickets = torch::zeros({2}, torch::dtype(torch::kInt32).device(torch::kCUDA, dev));
+      L.args.tickets = tickets.data_ptr<int32_t>();
+    }
   }
   static int pick_bn(int64_t n) { return n % 256 == 0 ? 256 : (n % 128 == 0 ? 128 : 64); }
   void check_bf16(const Tensor& t, const char* what) {

@@ -584,6 +584,10 @@ struct TcProblem {
 struct TcGemmArgs {
   int n_prob;
   TcProblem p[2];
+  // {next item, CTAs done}, zero between launches: CTAs claim work items with atomicAdd on [0]; the last CTA to
+  // finish zeroes both, so the next launch (or CUDA-graph replay) starts from item 0.  One buffer per plan, and a
+  // plan is never launched concurrently with itself.  nullptr = static striding (item = blockIdx.x + i * gridDim.x).
+  int* tickets;
 };
 struct alignas(64) TcGemmLaunch {
   unsigned char maps[6][128];   // CUtensorMap A0, B0, C0, A1, B1, C1

@@ -14,8 +14,13 @@
 //                           of the tile (N <= 256: up to 128 fp32 accumulator registers per thread), then the
 //                           epilogue: bias/ReLU -> bf16 -> swizzled smem staging -> TMA store, or fp32
 //                           red.global.add.v2 for the split-K weight gradients
-// Up to two independent problems share one launch (dW and dA of a layer both consume dPre): work items of both
-// are dealt round-robin to the CTAs.
+// Up to two independent problems share one launch (dW and dA of a layer both consume dPre): their work items form
+// one combined item space.  The producer claims items from a per-plan ticket (atomicAdd), so a CTA that starts late
+// -- its SM still held by a kernel of another stream (the sampler runs beside the training step) -- takes whatever
+// is left instead of holding up the whole GEMM on items dealt to it in advance.  It publishes each item id to the
+// consumers through a shared slot of the ring stage that carries the item's first k-block (written before the
+// stage's arrive, which releases it; the consumers' wait acquires it), and a stop sentinel (-1, a plain arrive with
+// no bytes) when the ticket runs past the end.
 //
 // The reference has no counterpart (its examples call PyG / cuBLAS through autograd).
 #include <cuda.h>
@@ -115,6 +120,7 @@ k_tc_gemm(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
   uint64_t* bars = reinterpret_cast<uint64_t*>(store0 + 2 * kStoreBytes);
   const uint32_t bar_full0 = smem_u32(bars + 0);               // + 8 * stage
   const uint32_t bar_empty0 = smem_u32(bars + kStages);        // + 8 * stage
+  volatile int* item_slot = reinterpret_cast<volatile int*>(bars + 2 * kStages);   // [kStages] item id or -1
 
   const int wg = threadIdx.x >> 7;
   const int warp = threadIdx.x >> 5;
@@ -150,7 +156,9 @@ k_tc_gemm(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
     // ------------------------------ TMA producer ------------------------------
     if (threadIdx.x == 0) {
       int fill = 0;   // k-blocks produced so far (ring position)
-      for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
+      for (int item = blockIdx.x;; item += gridDim.x) {
+        if (g.tickets) item = atomicAdd(g.tickets, 1);
+        if (item >= total_items) break;
         const Item it = decode(item, d0, d1);
         const TcProblem& p = g.p[it.prob];
         const CUtensorMap* ta = it.prob ? &tmA1 : &tmA0;
@@ -161,6 +169,7 @@ k_tc_gemm(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
           const uint32_t ph = (fill / kStages) & 1;
           mbar_wait(bar_empty0 + 8 * s, ph ^ 1);
           const uint32_t full = bar_full0 + 8 * s;
+          if (kb == it.kb0) item_slot[s] = item;
           mbar_expect_tx(full, bytes);
           const uint32_t sa = smem_u32(stage0 + s * kStageBytes);
           const uint32_t sb = sa + kABytes;
@@ -178,6 +187,19 @@ k_tc_gemm(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
           }
         }
       }
+      // stop sentinel in the next ring position: a plain arrive completes the stage's phase with no bytes
+      const int s = fill % kStages;
+      mbar_wait(bar_empty0 + 8 * s, ((fill / kStages) & 1) ^ 1);
+      item_slot[s] = -1;
+      mbar_arrive(bar_full0 + 8 * s);
+      if (g.tickets) {
+        // every CTA has made its last claim once all have counted themselves out: the last one resets the ticket
+        __threadfence();
+        if (atomicAdd(g.tickets + 1, 1) == static_cast<int>(gridDim.x) - 1) {
+          g.tickets[0] = 0;
+          g.tickets[1] = 0;
+        }
+      }
     }
   } else {
     // ------------------------------ consumers: wgmma + epilogue ------------------------------
@@ -187,7 +209,11 @@ k_tc_gemm(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
     const bool issuer = (et == 0);
     int drain = 0;
     int chunk_ctr = 0;                                 // staging double buffer position
-    for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
+    for (;;) {
+      // the item's first k-block stage carries its id (the k-block loop below waits on the same phase again)
+      mbar_wait(bar_full0 + 8 * (drain % kStages), (drain / kStages) & 1);
+      const int item = item_slot[drain % kStages];
+      if (item < 0) break;
       const Item it = decode(item, d0, d1);
       const TcProblem& p = g.p[it.prob];
       const CUtensorMap* tcm = it.prob ? &tmC1 : &tmC0;

@@ -102,6 +102,10 @@ class GraphSageEngine(object):
       fused and the unfused (aggregate kernel + cuBLAS) layer on real batches during warm-up and
       keep the faster one (remote-heavy multi-GPU runs can favour the unfused pair).
     use_cuda_graph: capture sample+forward+backward(+adam) into CUDA graphs.
+    preaggregate_layer1: pipelined engines whose layer 1 runs unfused aggregate layer 1 of the next batch on the
+      sampling stream, right after sampling it (the aggregation depends on the batch and the feature table only, not
+      on the weights), so the training chain starts with the layer-1 GEMM.  Each arena then has its own layer-1 A
+      buffer.  None = on where it applies, unless GLT_B200_PREAGG=0; False = aggregate inside the forward as usual.
   """
 
   def __init__(self, graph, feature_table, labels: torch.Tensor, in_dim: int, num_nodes: int,
@@ -113,7 +117,7 @@ class GraphSageEngine(object):
                use_peer_allreduce: bool = True, use_gather_bwd: Optional[bool] = None,
                check_every: int = 64, auto_regrow: bool = True, feature_format: str = 'bf16',
                deterministic_sampling: bool = False, stage_remote_rows: Optional[bool] = None,
-               dropout: float = 0.0):
+               dropout: float = 0.0, preaggregate_layer1: Optional[bool] = None):
     self.nat = require_native()
     # dropout on the hidden activations (the reference example trains with p = 0.5,
     # examples/train_sage_ogbn_products.py:58): one in-place Philox kernel per hidden layer in training steps,
@@ -148,6 +152,11 @@ class GraphSageEngine(object):
       import os as _os
       use_gather_bwd = _os.environ.get('GLT_B200_GATHER_BWD', '1') == '1'
     self.use_gather_bwd = bool(use_gather_bwd)
+    if preaggregate_layer1 is None:
+      import os as _os5
+      preaggregate_layer1 = _os5.environ.get('GLT_B200_PREAGG', '1') != '0'
+    self._preagg_opt = bool(preaggregate_layer1)
+    self.preaggregate = False         # resolved once the layer-1 variant is known (_resolve_preagg)
     # every dense contraction outside the fused layer-1 kernel runs on the TMA-fed wgmma GEMM kernel
     # (csrc/cuda/tc_gemm.cu); GLT_B200_TC_GEMM=0 falls back to cuBLAS for A/B measurements
     import os as _os2
@@ -213,6 +222,7 @@ class GraphSageEngine(object):
       self.w_packed = [None] + [torch.zeros(self.dims_out[l - 1] * 2 * self.dims_in[l - 1], dtype=bf, device=dev)
                                 if self.fused_ok[l] else None for l in range(1, self.L + 1)]
       self._repack()
+      self._resolve_preagg()
       if self.feature_format == 'mxfp8' and not self.fused_ok[1]:
         raise RuntimeError('MXFP8 features need the fused layer-1 kernel (in_dim 128, hidden multiple of 32, <= 256)')
     self._graph_fb = None
@@ -272,6 +282,8 @@ class GraphSageEngine(object):
     self.cap_T = [min(c, self.arena.cap_nodes) for c in self.cap_T]
     self.A = [None] + [torch.zeros(self.cap_T[l], 2 * self.dims_in[l - 1], dtype=bf, device=dev)
                        for l in range(1, self.L + 1)]
+    # layer-1 A operand per arena (see _A): pre-aggregation writes arena b+1's while arena b's is read
+    self._A1 = [self.A[1]] + [torch.zeros_like(self.A[1]) for _ in range(1, n_arenas) if self.preaggregate]
     self.Z = [None] + [torch.zeros(self.cap_T[l], self.dims_out[l - 1], dtype=bf, device=dev)
                        for l in range(1, self.L + 1)]
     self.dPre = [None] + [torch.zeros(self.cap_T[l], self.dims_out[l - 1], dtype=bf, device=dev)
@@ -363,6 +375,23 @@ class GraphSageEngine(object):
   def g32(self):
     """Flat fp32 gradient buffer of the batch being trained (per parity when double-buffered)."""
     return self._g[self._cur % len(self._g)]
+
+  def _A(self, l: int, parity: Optional[int] = None):
+    """A operand [mean | self] of layer l; layer 1 has one per arena when pre-aggregated."""
+    if l == 1 and self.preaggregate:
+      return self._A1[self._cur if parity is None else parity]
+    return self.A[l]
+
+  def _resolve_preagg(self):
+    """Pre-aggregation of layer 1 (see `preaggregate_layer1`) applies to pipelined engines whose layer 1 runs
+    unfused.  While `use_fused='auto'` has not decided, layer 1 aggregates inside the forward, so that the timed
+    unfused variant includes its aggregation."""
+    on = self._preagg_opt and self.pipeline and not self.fused_ok[1] and not self._autotune_fused
+    if on == self.preaggregate:
+      return
+    self.preaggregate = on
+    self._A1 = [self.A[1]] + [torch.zeros_like(self.A[1]) for _ in range(1, len(self._arenas)) if on]
+    self._tc_plans = {}
 
   # ------------------------------------------------------------------ capacity calibration
   def _calibrate(self, pool: torch.Tensor, num_nodes: int, margin: float, n_batches: int):
@@ -503,6 +532,17 @@ class GraphSageEngine(object):
     if self.stage_remote:
       self.feat.stage_remote_rows(ar.nodes, ar.counters, self.L + 1, self._xcache[which])
       self._k(1)
+    if self.preaggregate:
+      self._aggregate_layer1(which)
+
+  def _aggregate_layer1(self, which: int):
+    """Layer-1 aggregation of the batch in arena `which` into its A buffer, on the current stream (the sampling
+    stream of a pipelined step).  With several GPUs it reads the peers' feature rows in place."""
+    ar = self._arenas[which]
+    nh = self.L
+    self.nat.sage_aggregate(self.feat, ar.nodes, None, self.in_dim, ar.counters, nh, list(ar.ell[:nh]),
+                            self.fanouts[:nh], ar.deg, self._A1[which])
+    self._k(1)
 
   def _forward(self, train: bool = True):
     nat, ar = self.nat, self.arena
@@ -531,8 +571,9 @@ class GraphSageEngine(object):
                      self.b(l), relu, self.Z[l], self.A[l], xc)
       self._k(1)
     else:
-      nat.sage_aggregate(feat, nodes, src_local, d, ar.counters, nh, ell, ks, ar.deg, self.A[l])
-      self._k(1)
+      if not (l == 1 and self.preaggregate):     # pre-aggregated: _sample already wrote A1 of this arena
+        nat.sage_aggregate(feat, nodes, src_local, d, ar.counters, nh, ell, ks, ar.deg, self._A(l))
+        self._k(1)
       if self.use_tc_gemm:
         # Z = act(A . W^T + b) on wgmma (TMA-fed, bias/ReLU in the register epilogue, rows from the device counter)
         self._plan('fwd', l).run()
@@ -540,9 +581,9 @@ class GraphSageEngine(object):
       else:
         # library GEMM with the bias (+ ReLU) applied in the cuBLASLt epilogue
         if relu:
-          torch._addmm_activation(self.b(l), self.A[l], self.W(l).t(), out=self.Z[l])
+          torch._addmm_activation(self.b(l), self._A(l), self.W(l).t(), out=self.Z[l])
         else:
-          torch.addmm(self.b(l), self.A[l], self.W(l).t(), out=self.Z[l])
+          torch.addmm(self.b(l), self._A(l), self.W(l).t(), out=self.Z[l])
         self._lib(1)
 
   def _forward_loss(self, train: bool = True):
@@ -577,14 +618,14 @@ class GraphSageEngine(object):
     nh = self.L - l + 1                     # counters[nh] = number of target rows of layer l
     pl = nat.TcGemm(self.device.index)
     if kind == 'fwd':
-      pl.add_forward(self.A[l], self.W(l), self.b(l), l < self.L, self.Z[l], ar.counters, nh)
+      pl.add_forward(self._A(l), self.W(l), self.b(l), l < self.L, self.Z[l], ar.counters, nh)
     else:
       off, n, k = self._w_off[l - 1]
       gW = self.g32[off:off + n * k].view(n, k)
       # 'bwd': dW (split-K over the batch rows, fp32 red-add) and dA of the same layer share one launch;
       # 'wgrad' / 'dgrad': the two halves as separate launches (overlap_wgrad: dW leaves the critical chain)
       if kind in ('bwd', 'wgrad'):
-        pl.add_wgrad(self.dPre[l], self.A[l], gW, ar.counters, nh)
+        pl.add_wgrad(self.dPre[l], self._A(l), gW, ar.counters, nh)
       if l > 1 and kind in ('bwd', 'dgrad'):
         pl.add_dgrad(self.dPre[l], self.W(l), self.dA[l], ar.counters, nh)
     self._tc_plans[key] = pl
@@ -633,7 +674,7 @@ class GraphSageEngine(object):
       else:
         gW = self.g32[off:off + n * k].view(n, k)
         # dW = dPre^T A accumulated in fp32 straight into the flat gradient buffer
-        self._mm_f32(self.dPre[l].t(), self.A[l], gW)
+        self._mm_f32(self.dPre[l].t(), self._A(l), gW)
         self._lib(1)
         if l > 1:
           torch.mm(self.dPre[l], self.W(l), out=self.dA[l])
@@ -765,6 +806,7 @@ class GraphSageEngine(object):
         self._cur = 0
         self._autotune()
         self._autotune_fused = False
+        self._resolve_preagg()
         if self.pipeline:
           self._sample(0)
         self._tally = self._lib_tally = 0
@@ -877,7 +919,8 @@ class GraphSageEngine(object):
 
   def profile_sections(self, seeds: torch.Tensor, iters: int = 10):
     """Device time (ms) of each stage of an *eager, unpipelined* step (CUDA events; the other
-    ranks run the same sequence so the peer barriers inside are matched).  Diagnostic only."""
+    ranks run the same sequence so the peer barriers inside are matched).  Diagnostic only.  With pre-aggregation
+    (`preaggregate_layer1`) 'sample' includes the layer-1 aggregation and 'forward_l1' is its GEMM alone."""
     names = ['sample', 'forward_l1', 'forward_rest', 'backward', 'optimizer']
     acc = {n: 0.0 for n in names}
     self._cur = 0
@@ -951,6 +994,10 @@ class GraphSageEngine(object):
         log.append(('arena.sample (all sampling kernels)', e0, e1))
         if self.stage_remote:
           self.feat.stage_remote_rows(ar.nodes, ar.counters, self.L + 1, self._xcache[0])
+        if self.preaggregate:
+          # a pipelined step runs it on the sampling stream, outside the training chain
+          self._aggregate_layer1(0)
+          log[-1] = ('sage_aggregate (layer 1, sampling stream)',) + log[-1][1:]
         self._forward()
         self._backward()
         self._allreduce()

@@ -68,6 +68,8 @@ class GraphSageLinkEngine(GraphSageEngine):
       g = torch.Generator(device='cpu')
       g.manual_seed(int(engine_kwargs.get('seed', 0)) + 29)
       pool = torch.cat([pairs.flatten(), torch.randint(0, int(num_nodes), (2 * k * pairs.shape[1],), generator=g)])
+    # layer 1 aggregates inside the forward here (pre-aggregation on the sampling stream is a node-engine feature)
+    engine_kwargs.setdefault('preaggregate_layer1', False)
     super().__init__(graph, feature_table, torch.zeros(1, dtype=torch.int64), in_dim, num_nodes, fanouts=fanouts,
                      batch_size=2 * self.P, hidden=hidden, num_classes=C, calibration_seeds=pool, **engine_kwargs)
     dev = self.device
