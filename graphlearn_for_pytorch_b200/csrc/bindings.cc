@@ -838,27 +838,6 @@ static void sage_aggregate(RowTableHandle* feat, const c10::optional<Tensor>& no
   check_cuda_err("sage_aggregate");
 }
 
-static void sage_scatter_bwd(const Tensor& dA, int64_t d, const Tensor& counters, int64_t n_hops_targets,
-                             const std::vector<Tensor>& ell, const std::vector<int64_t>& ks,
-                             const Tensor& deg, Tensor dH) {
-  c10::cuda::CUDAGuard guard(dA.device());
-  check_sage_width(d, "sage_scatter_bwd: d must be a multiple of 8 in [8, 1024]");
-  TORCH_CHECK(dA.scalar_type() == torch::kBFloat16 && dA.is_contiguous() && dA.size(1) == 2 * d);
-  TORCH_CHECK(dH.scalar_type() == torch::kFloat32 && dH.is_contiguous() && dH.size(1) == d);
-  SageScatterArgs a{};
-  a.dA = dA.data_ptr();
-  a.d = d;
-  a.cum = counters.data_ptr<int32_t>();
-  a.n_hops_targets = n_hops_targets;
-  a.cap_targets = dA.size(0);
-  fill_ell(ell, ks, a.ell, a.k);
-  a.deg = deg.data_ptr<int32_t>();
-  a.dH = dH.data_ptr<float>();
-  launch_sage_scatter_bwd(a, cur_stream());
-  check_cuda_err("sage_scatter_bwd");
-}
-
-
 // ---- column-block variants used by the heterogeneous engine: A_t = [mean_rel1 | mean_rel2 | ... | self] ----
 static void sage_aggregate_block(RowTableHandle* feat, const c10::optional<Tensor>& nodes,
                                  const c10::optional<Tensor>& src_local, int64_t d, const Tensor& counters,
@@ -896,7 +875,6 @@ static void sage_scatter_block(const Tensor& dA, int64_t d, int64_t mean_col, co
   a.dH = dH.data_ptr<float>();
   a.dA_ld = static_cast<int>(dA.stride(0));
   a.mean_col = static_cast<int>(mean_col);
-  a.self_col = -1;
   launch_sage_scatter_bwd(a, cur_stream());
   check_cuda_err("sage_scatter_block");
 }
@@ -1639,10 +1617,6 @@ static void sage_fused(RowTableHandle* feat, const c10::optional<Tensor>& nodes,
   f.relu = relu;
   f.z = z.data_ptr();
   f.feat_fp8 = fp8 ? 1 : 0;
-  // The resolver-side prefetch.global.L2 of the next tile's rows lengthens the kernel's prologue, and the loaders are
-  // bound by bytes in flight rather than by DRAM-vs-L2 latency.  Off by default; GLT_B200_L2_PREFETCH=1 enables it.
-  static const bool l2pf = [] { const char* e = std::getenv("GLT_B200_L2_PREFETCH"); return e ? std::atoi(e) != 0 : false; }();
-  f.l2_prefetch = (l2pf && feat != nullptr && !(src_local.has_value() && src_local->defined())) ? 1 : 0;
   f.local_mask = feat != nullptr ? feat->local_mask : 0u;
   f.xcache = nullptr;
   f.cache_part = -1;
@@ -2115,7 +2089,6 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
 
   // ---- GraphSAGE engine ----
   m.def("sage_aggregate", &sage_aggregate);
-  m.def("sage_scatter_bwd", &sage_scatter_bwd);
   m.def("sage_full_aggregate", &sage_full_aggregate, py::arg("graph"), py::arg("feat"), py::arg("src"),
         py::arg("src_col"), py::arg("self_col"), py::arg("d"), py::arg("r0"), py::arg("r1"), py::arg("combine"),
         py::arg("bias"), py::arg("relu"), py::arg("out"));

@@ -214,8 +214,10 @@ struct SageFullAggArgs {
 };
 void launch_sage_full_aggregate(const SageFullAggArgs& a, cudaStream_t s);
 
+// dH[s, :] += dA[t, mean_col : mean_col + d] / deg[t] for every sampled edge t <- s of the targets t < cum[n_hops]
+// (the mean block of one relation of a heterogeneous layer; its self block is added by launch_add_block_f32)
 struct SageScatterArgs {
-  const void* dA;               // bf16 [cap_targets, 2d]
+  const void* dA;               // bf16 [cap_targets, dA_ld]
   int d;
   const int32_t* cum;
   int n_hops_targets;
@@ -223,8 +225,8 @@ struct SageScatterArgs {
   const int32_t* ell[4];
   int k[4];
   const int32_t* deg;
-  float* dH;                    // fp32 [cap_src, d], pre-zeroed
-  int dA_ld, mean_col, self_col;  // column-block input like SageAggArgs (dA_ld == 0: homogeneous [mean | self])
+  float* dH;                    // fp32 [cap_src, d]
+  int dA_ld, mean_col;          // row pitch of dA and first column of the mean block (elements)
 };
 void launch_sage_scatter_bwd(const SageScatterArgs& a, cudaStream_t s);
 // dH[t, :] += dA[t, col : col + d] for t < cum[n_hops] (self block of a heterogeneous layer)
@@ -276,7 +278,6 @@ struct SageGatherBwdArgs {
   float gscale;              // 1/(1-p) when Z is a post-dropout activation, else 1
 };
 // dPre[s] = relu'(Z[s]) * (dA_self[s] + sum_{t in in(s)} dA_mean[t] / deg[t]); rows >= sources are zero-filled.
-// Replaces zero_rows + sage_scatter_bwd (fp32 atomics) + relu_bwd_cast.
 void launch_sage_gather_bwd(const SageGatherBwdArgs& a, cudaStream_t s);
 
 // dPre = (Z > 0) ? bf16(dH) : 0 for rows < cum[n_hops]; 0 beyond.  relu = false: dPre = bf16(dH), Z is not read.
@@ -548,8 +549,7 @@ struct SageFusedArgs {
   void* a_save;                 // optional bf16 [cap_targets, 2d] for backward
   unsigned long long* trace;    // optional per-CTA clock64 timeline (diagnostics, see sage_fused_trace)
   int feat_fp8;                 // 1: agg.feat rows are MXFP8 (d e4m3 bytes + d/32 UE8M0 scales, 16-byte padded)
-  int l2_prefetch;              // resolver warps prefetch next tile's local feature rows into L2
-  unsigned local_mask;          // bit p set: part p of agg.feat lives in this GPU's HBM (prefetchable into its L2)
+  unsigned local_mask;          // bit p set: part p of agg.feat lives in this GPU's HBM
   // Staged remote rows: rows of the batch's nodes that live in PEER HBM, copied once per batch (on the sampling
   // stream, launch_stage_remote_rows) into a local buffer indexed by the node's LOCAL id.  nullptr = read peers in
   // place.  cache_part: index of a non-local part whose handle slot is reused for the cache.

@@ -104,8 +104,9 @@ __device__ __forceinline__ void atomic_add8(float* dst, const float* v) {
   atomicAdd(reinterpret_cast<float4*>(dst + 4), make_float4(v[4], v[5], v[6], v[7]));
 }
 
+// 8 blocks per SM: every width variant stays at <= 32 registers, i.e. 64 resident warps to cover the atomics' latency
 template <int LPR, int VPL>
-__global__ void __launch_bounds__(256) k_sage_scatter_bwd(SageScatterArgs a) {
+__global__ void __launch_bounds__(256, 8) k_sage_scatter_bwd(SageScatterArgs a) {
   pdl_enter();
   constexpr int RPW = 32 / LPR;
   const int lane = threadIdx.x & 31;
@@ -121,25 +122,18 @@ __global__ void __launch_bounds__(256) k_sage_scatter_bwd(SageScatterArgs a) {
     const int dg = a.deg[t];
     const int k = a.k[l.hop];
     const int32_t* ell = a.ell[l.hop] + static_cast<int64_t>(l.row) * k;
-    const int ld = a.dA_ld ? a.dA_ld : 2 * a.d;
-    const int mcol = a.dA_ld ? a.mean_col : 0;
-    const int scol = a.dA_ld ? a.self_col : a.d;
-    const uint8_t* g = reinterpret_cast<const uint8_t*>(a.dA) + static_cast<int64_t>(t) * ld * 2;
+    const uint8_t* g = reinterpret_cast<const uint8_t*>(a.dA) + static_cast<int64_t>(t) * a.dA_ld * 2;
     const float inv = dg > 0 ? 1.f / static_cast<float>(dg) : 0.f;
 #pragma unroll
     for (int v = 0; v < VPL; ++v) {
       const int c = v * LPR + gl;
       if (c >= nvec) continue;
-      float gn[8], gs[8];
+      float gn[8];
 #pragma unroll
-      for (int i = 0; i < 8; ++i) gn[i] = gs[i] = 0.f;
-      bf16x8_accum(reinterpret_cast<const uint4*>(g + mcol * 2)[c], gn);
+      for (int i = 0; i < 8; ++i) gn[i] = 0.f;
+      bf16x8_accum(reinterpret_cast<const uint4*>(g + a.mean_col * 2)[c], gn);
 #pragma unroll
       for (int i = 0; i < 8; ++i) gn[i] *= inv;
-      if (scol >= 0) {
-        bf16x8_accum(reinterpret_cast<const uint4*>(g + scol * 2)[c], gs);
-        atomic_add8(a.dH + static_cast<int64_t>(t) * a.d + c * 8, gs);
-      }
       for (int j = 0; j < dg; ++j) {
         const int s = ell[j];
         if (s >= 0) atomic_add8(a.dH + static_cast<int64_t>(s) * a.d + c * 8, gn);

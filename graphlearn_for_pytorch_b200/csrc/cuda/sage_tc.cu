@@ -634,27 +634,10 @@ __global__ void __launch_bounds__(kThreads3, 1) k_sage_fused3(SageFusedArgs f) {
         int64_t gid[kKP];
 #pragma unroll
         for (int j = 0; j < kKP; ++j) gid[j] = (j < dg && sidx[j] >= 0) ? __ldg(a.nodes + sidx[j]) : -1;
-        // The loaders will want these rows one tile (~7 us) from now: pull the LOCAL ones from DRAM into L2 already
-        // (the loader's three dependent batches per row then cost L2 latency instead of DRAM latency).  Peer rows
-        // are skipped: peer memory is not cached in the local L2.
         uint32_t hnd[kKP + 1];
 #pragma unroll
         for (int j = 0; j < kKP; ++j) hnd[j] = handle_of(gid[j], sidx[j]);
         hnd[kKP] = handle_of(self_gid, t);
-        if (f.l2_prefetch) {
-          const unsigned pf_mask = f.local_mask | (f.xcache ? (1u << f.cache_part) : 0u);
-#pragma unroll
-          for (int j = 0; j <= kKP; ++j) {
-            const uint32_t h = hnd[j];
-            if (h != kNoRow && ((pf_mask >> (h >> 28)) & 1u)) {
-              const uint8_t* p = reinterpret_cast<const uint8_t*>((f.xcache && static_cast<int>(h >> 28) == f.cache_part)
-                                                                      ? f.xcache : a.feat.base[h >> 28]) +
-                                 static_cast<int64_t>(h & 0x0FFFFFFFu) * row_bytes;
-              asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
-              if (row_bytes > 128) asm volatile("prefetch.global.L2 [%0];" ::"l"(p + 128));
-            }
-          }
-        }
 #pragma unroll
         for (int j = 0; j < kKP; ++j) sts32(trow + ((j ^ sw) << 2), static_cast<int32_t>(hnd[j]));
         sts32(trow + ((15 ^ sw) << 2), static_cast<int32_t>(hnd[kKP]));
@@ -747,13 +730,7 @@ size_t fused3_smem_bytes(int d, int n_out) {
 constexpr size_t kMaxSmem = 227 * 1024;
 
 // 3 = decoupled resolver/loader kernel, 2 = the earlier monolithic-producer kernel
-// (GLT_B200_FUSED_VERSION=2 selects it for A/B measurements).
 int fused_version(int d, int n_out) {
-  static const int forced = [] {
-    const char* e = std::getenv("GLT_B200_FUSED_VERSION");
-    return e ? std::atoi(e) : 0;
-  }();
-  if (forced == 2) return 2;
   return fused3_smem_bytes(d, n_out) <= kMaxSmem ? 3 : 2;
 }
 

@@ -1,8 +1,8 @@
 // Transposed per-batch adjacency and the atomics-free backward of the mean aggregation.
 //
-// The engine's default backward (GLT_B200_GATHER_BWD=0 selects the scatter formulation instead): it replaces
-// zero_rows + sage_scatter_bwd (fp32 float4 atomics) + relu_bwd_cast.  On an H100 (products shape, bench.py) the
-// step takes 0.297 ms with it and 0.409 ms with the scatter formulation.
+// The GraphSAGE engine's backward of the aggregation.  It replaced a zero fill, an fp32-atomic scatter over the edges
+// and a ReLU/cast kernel: on an H100 (products shape, bench.py) the step took 0.297 ms with it and 0.409 ms with
+// that scatter formulation.
 //
 //   build (sampling stream, overlapped with the training of the previous batch):
 //     k_tr_count   in-degree histogram of the local source ids, one histogram per hop
@@ -197,7 +197,6 @@ inline int grid_for(int64_t items, int per_block, int max_blocks = 132 * 16) {
 // ------------------------------------------------------------------------------------------
 // Gather-style backward of the mean aggregation:
 //   dPre[s] = relu'(Z[s]) * (dA_self[s] + sum_{t in in(s)} dA_mean[t] / deg[t])       (+ bias column sums)
-// replaces zero_rows + sage_scatter_bwd (fp32 RED.128) + relu_bwd_cast of the scatter formulation.
 //   * 32 consecutive source rows form a chunk served by a TEAM of warps; every warp of the team reads the chunk's
 //     records ({count, segment start, first two in-neighbours, their 1/deg}: built by k_tr_meta on the sampling
 //     stream, prefetched one chunk ahead) and takes every TEAM-th row;

@@ -8,7 +8,7 @@ fanout [15,10,5], batch 1024).  `GraphSAGE` below is the drop-in eager module fo
   sample (static-shape arena, no host sync)
     -> layer 1: ONE wgmma kernel = peer/local HBM row gather + neighbour mean +
        [mean | self] x W1 + bias + ReLU (csrc/cuda/sage_tc.cu)
-    -> layers 2..L: ELL aggregation kernel + cuBLAS GEMM (small)
+    -> layers 2..L: ELL aggregation kernel + wgmma GEMM (csrc/cuda/tc_gemm.cu)
     -> fused log-softmax/NLL fwd+bwd -> hand-written backward -> NCCL all-reduce -> fused Adam
 
 with every extent read from device counters, so the whole step is a fixed launch sequence
@@ -99,7 +99,7 @@ class GraphSageEngine(object):
       kernel supports raise ValueError here.
     group: torch.distributed group for the gradient all-reduce (None = single process).
     use_fused: True = use the wgmma gather+GEMM kernel where the shape allows; 'auto' = time the
-      fused and the unfused (aggregate kernel + cuBLAS) layer on real batches during warm-up and
+      fused and the unfused (aggregate kernel + wgmma GEMM) layer on real batches during warm-up and
       keep the faster one (remote-heavy multi-GPU runs can favour the unfused pair).
     use_cuda_graph: capture sample+forward+backward(+adam) into CUDA graphs.
     preaggregate_layer1: pipelined engines whose layer 1 runs unfused aggregate layer 1 of the next batch on the
@@ -107,6 +107,10 @@ class GraphSageEngine(object):
       on the weights), so the training chain starts with the layer-1 GEMM.  Each arena then has its own layer-1 A
       buffer.  None = on where it applies, unless GLT_B200_PREAGG=0; False = aggregate inside the forward as usual.
   """
+  # read by bench.py: the backward of the aggregation is always the atomics-free gather (csrc/cuda/transpose.cu)
+  use_gather_bwd = True
+  # read by bench.py and benchmarks/bench_link.py: every contraction runs on this project's kernels, none on cuBLAS
+  library_gemms_per_step = 0
 
   def __init__(self, graph, feature_table, labels: torch.Tensor, in_dim: int, num_nodes: int,
                fanouts: List[int] = (15, 10, 5), batch_size: int = 1024, hidden: int = 256,
@@ -114,14 +118,14 @@ class GraphSageEngine(object):
                device: Optional[torch.device] = None, group=None, use_fused: bool = True,
                use_cuda_graph: bool = True, calibration_seeds: Optional[torch.Tensor] = None,
                calibration_margin: float = 1.3, calibration_batches: int = 16, pipeline: bool = False,
-               use_peer_allreduce: bool = True, use_gather_bwd: Optional[bool] = None,
+               use_peer_allreduce: bool = True,
                check_every: int = 64, auto_regrow: bool = True, feature_format: str = 'bf16',
                deterministic_sampling: bool = False, stage_remote_rows: Optional[bool] = None,
                dropout: float = 0.0, preaggregate_layer1: Optional[bool] = None):
     self.nat = require_native()
     # dropout on the hidden activations (the reference example trains with p = 0.5,
     # examples/train_sage_ogbn_products.py:58): one in-place Philox kernel per hidden layer in training steps,
-    # mask keyed by (seed, layer, optimizer step, element); backward rescales inside relu_bwd_cast.
+    # mask keyed by (seed, layer, optimizer step, element); backward rescales inside sage_gather_bwd.
     assert 0.0 <= float(dropout) < 1.0
     self.dropout = float(dropout)
     # 'mxfp8': `feature_table` holds data.quantize_mxfp8 rows (uint8, in_dim + 16 bytes); the fused layer-1 kernel
@@ -138,31 +142,14 @@ class GraphSageEngine(object):
     # issued from inside the GEMM kernel are bound by NVLink latency, not bandwidth).  True = stage when the feature
     # table has non-local parts; None/False = in-kernel peer loads (the default, see _build_buffers).
     self._stage_remote_opt = stage_remote_rows
-    import os as _os3
-    # running the weight-gradient GEMMs and the zero fills on an auxiliary stream lets their CTAs compete with the
-    # critical dgrad -> scatter -> cast chain; off by default, kept as an option.
-    self.overlap_wgrad = _os3.environ.get('GLT_B200_OVERLAP_WGRAD', '0') != '0'
     self.deterministic_sampling = bool(deterministic_sampling)
     self.use_peer_allreduce = bool(use_peer_allreduce)
-    # use_gather_bwd (csrc/cuda/transpose.cu): the sampler also builds the transposed adjacency of the batch (on the
-    # sampling stream) and the backward of the aggregation is an atomics-free gather (replaces zero_rows + fp32-atomic
-    # scatter + relu_bwd_cast: 4 launches per hidden layer -> 2).  Default on (GLT_B200_GATHER_BWD=0 restores the
-    # scatter path).
-    if use_gather_bwd is None:
-      import os as _os
-      use_gather_bwd = _os.environ.get('GLT_B200_GATHER_BWD', '1') == '1'
-    self.use_gather_bwd = bool(use_gather_bwd)
     if preaggregate_layer1 is None:
       import os as _os5
       preaggregate_layer1 = _os5.environ.get('GLT_B200_PREAGG', '1') != '0'
     self._preagg_opt = bool(preaggregate_layer1)
     self.preaggregate = False         # resolved once the layer-1 variant is known (_resolve_preagg)
-    # every dense contraction outside the fused layer-1 kernel runs on the TMA-fed wgmma GEMM kernel
-    # (csrc/cuda/tc_gemm.cu); GLT_B200_TC_GEMM=0 falls back to cuBLAS for A/B measurements
-    import os as _os2
-    self.use_tc_gemm = _os2.environ.get('GLT_B200_TC_GEMM', '1') != '0'
     self._tc_plans = {}
-    self.library_gemms_per_step = 0
     self.peer_group = None
     self.graph = graph
     graph.lazy_init()
@@ -207,7 +194,6 @@ class GraphSageEngine(object):
       n_arenas = len(self._arenas)
       self._seeds = [torch.zeros(self.bs, dtype=torch.int64, device=dev) for _ in range(n_arenas)]
       self._side = torch.cuda.Stream(device=dev) if self.pipeline else None
-      self._aux = torch.cuda.Stream(device=dev)      # weight gradients + zero fills, off the critical chain
       self._primed = False
       self.loss = torch.zeros(1, dtype=torch.float32, device=dev)
       self.correct = torch.zeros(1, dtype=torch.int32, device=dev)
@@ -232,17 +218,15 @@ class GraphSageEngine(object):
   def _check_widths(self, use_fused):
     """Rejects, at construction, widths that a kernel of the step cannot run (instead of failing at the first step or
     silently computing on truncated rows).  `in_dim` and `hidden` are multiples of 8 up to 1024, the widest row of
-    the aggregation / scatter kernels.  With the wgmma GEMMs (the default), every layer's A operand [mean | self]
-    is a multiple of 64 wide (weight gradients), so `in_dim` and `hidden` are multiples of 32; and `hidden` is a
-    multiple of 64 when a hidden layer runs the unfused forward GEMM, i.e. unless each hidden layer fits the fused
-    layer kernel (input width 64 or 128, `hidden` <= 256)."""
+    the aggregation and gather-backward kernels.  The wgmma weight-gradient GEMM needs every layer's A operand
+    [mean | self] to be a multiple of 64 wide, so `in_dim` and `hidden` are multiples of 32; and the wgmma forward
+    GEMM needs `hidden` to be a multiple of 64 when a hidden layer runs unfused, i.e. unless each hidden layer fits
+    the fused layer kernel (input width 64 or 128, `hidden` <= 256)."""
     for name, d in (('in_dim', self.in_dim), ('hidden', self.hidden)):
       if d % 8 != 0 or not 8 <= d <= 1024:
         raise ValueError(f'{name} must be a multiple of 8 in [8, 1024] (got {d})')
     if self.C < 1:
       raise ValueError(f'num_classes must be >= 1 (got {self.C})')
-    if not self.use_tc_gemm:
-      return
     for name, d in (('in_dim', self.in_dim), ('hidden', self.hidden)):
       if name == 'hidden' and self.L == 1:
         continue
@@ -262,7 +246,7 @@ class GraphSageEngine(object):
     """(Re)creates everything whose size depends on the arena capacities: sampler arenas, activation /
     gradient buffers, cached GEMM launches.  Parameters and optimizer state are untouched."""
     dev = self.device
-    bf, f32 = torch.bfloat16, torch.float32
+    bf = torch.bfloat16
     # pipelined mode double-buffers the sampler state: batch i+1 is sampled on a side stream
     # while batch i trains (the reference's sampler<->trainer producer/consumer pipeline,
     # distributed/dist_sampling_producer.py:54-163, collapsed onto CUDA streams of one GPU)
@@ -274,8 +258,10 @@ class GraphSageEngine(object):
     for p_, ar_ in enumerate(self._arenas):
       ar_.step.fill_(p_ - n_arenas)          # disjoint Philox stream ids per arena
       ar_.deterministic = self.deterministic_sampling   # local ids of a hop in ascending global-id order
-      if self.use_gather_bwd and self.L >= 2:
-        ar_.enable_transpose(self.L - 1)     # layer 2 uses hops 0..L-2, deeper layers a prefix of them
+      if self.L >= 2:
+        # the sampler also builds the batch's transposed adjacency, which the gather backward of the aggregation
+        # reads (csrc/cuda/transpose.cu); layer 2 uses hops 0..L-2, deeper layers a prefix of them
+        ar_.enable_transpose(self.L - 1)
     self.cap_rows = list(self.arena.cap_rows)           # frontier capacity per hop (+ last-hop additions)
     # layer l (1-based) targets = nodes of hops 0..L-l
     self.cap_T = [0] + [int(sum(self.cap_rows[:self.L - l + 1])) for l in range(1, self.L + 1)]
@@ -290,8 +276,6 @@ class GraphSageEngine(object):
                           for l in range(1, self.L + 1)]
     self.dA = [None, None] + [torch.zeros(self.cap_T[l], 2 * self.dims_in[l - 1], dtype=bf, device=dev)
                               for l in range(2, self.L + 1)]
-    self.dH = [None] + [torch.zeros(self.cap_T[l], self.dims_out[l - 1], dtype=f32, device=dev)
-                        for l in range(1, self.L)]
     want = self._stage_remote_opt
     if want is None:
       import os as _os4
@@ -398,7 +382,7 @@ class GraphSageEngine(object):
     """Size the arena from observed frontier sizes instead of the worst case
     bs*prod(fanouts): sample a few batches of the seed pool with a worst-case arena, take the
     per-hop maxima (max over ranks), add a margin.  All buffers and every cap-proportional
-    launch (cuBLAS GEMMs, fills) shrink accordingly.  The kernels stay safe past the caps
+    launch (GEMMs, fills) shrink accordingly.  The kernels stay safe past the caps
     (excess nodes are dropped and counted in `overflow_count()`)."""
     dev = self.device
     tmp = self.nat.SamplerArena(dev.index, self.bs, self.fanouts, False, num_nodes)
@@ -509,12 +493,7 @@ class GraphSageEngine(object):
   def _k(self, n):
     self._tally += n
 
-  def _lib(self, n):
-    """Counts launches that go to a vendor library (cuBLAS/cuBLASLt) instead of this repo's kernels."""
-    self._lib_tally += n
-
   _tally = 0
-  _lib_tally = 0
 
   def _ell(self, l):
     """ELL blocks + strides used by layer l: hops 0..L-l."""
@@ -574,17 +553,9 @@ class GraphSageEngine(object):
       if not (l == 1 and self.preaggregate):     # pre-aggregated: _sample already wrote A1 of this arena
         nat.sage_aggregate(feat, nodes, src_local, d, ar.counters, nh, ell, ks, ar.deg, self._A(l))
         self._k(1)
-      if self.use_tc_gemm:
-        # Z = act(A . W^T + b) on wgmma (TMA-fed, bias/ReLU in the register epilogue, rows from the device counter)
-        self._plan('fwd', l).run()
-        self._k(1)
-      else:
-        # library GEMM with the bias (+ ReLU) applied in the cuBLASLt epilogue
-        if relu:
-          torch._addmm_activation(self.b(l), self._A(l), self.W(l).t(), out=self.Z[l])
-        else:
-          torch.addmm(self.b(l), self._A(l), self.W(l).t(), out=self.Z[l])
-        self._lib(1)
+      # Z = act(A . W^T + b) on wgmma (TMA-fed, bias/ReLU in the register epilogue, rows from the device counter)
+      self._plan('fwd', l).run()
+      self._k(1)
 
   def _forward_loss(self, train: bool = True):
     # labels[nodes[r]] is looked up inside the loss kernel (no gather launch)
@@ -622,99 +593,23 @@ class GraphSageEngine(object):
     else:
       off, n, k = self._w_off[l - 1]
       gW = self.g32[off:off + n * k].view(n, k)
-      # 'bwd': dW (split-K over the batch rows, fp32 red-add) and dA of the same layer share one launch;
-      # 'wgrad' / 'dgrad': the two halves as separate launches (overlap_wgrad: dW leaves the critical chain)
-      if kind in ('bwd', 'wgrad'):
-        pl.add_wgrad(self.dPre[l], self._A(l), gW, ar.counters, nh)
-      if l > 1 and kind in ('bwd', 'dgrad'):
+      # 'bwd': dW (split-K over the batch rows, fp32 red-add) and dA of the same layer share one launch
+      pl.add_wgrad(self.dPre[l], self._A(l), gW, ar.counters, nh)
+      if l > 1:
         pl.add_dgrad(self.dPre[l], self.W(l), self.dA[l], ar.counters, nh)
     self._tc_plans[key] = pl
     return pl
 
   def _backward(self):
-    nat, ar = self.nat, self.arena
-    overlap = self.overlap_wgrad and self.use_tc_gemm and not self.use_gather_bwd and self.L > 1
-    main = torch.cuda.current_stream()
-    if overlap:
-      # Only dA -> scatter -> ReLU-mask feeds the next layer; the weight gradients are consumed by Adam alone.  They
-      # run on an auxiliary stream (forked after dPre[l] exists, joined before the optimizer) together with the
-      # zero-fill of the fp32 scatter targets, so the critical chain per layer is dgrad -> scatter -> cast.
-      aux = self._aux
-      aux.wait_stream(main)
-      with torch.cuda.stream(aux):
-        for l in range(self.L, 1, -1):
-          nat.zero_rows(self.dH[l - 1], ar.counters, self.L - l + 2)
-        self._k(self.L - 1)
-      ev_zero = torch.cuda.Event()
-      ev_zero.record(aux)
+    # bias gradients are fused into the kernels that produce dPre (loss / sage_gather_bwd)
     for l in range(self.L, 0, -1):
-      ell, ks, nh = self._ell(l)
-      off, n, k = self._w_off[l - 1]
-      boff, _ = self._b_off[l - 1]
-      if overlap and l > 1:
-        ev = torch.cuda.Event()
-        ev.record(main)                     # dPre[l] (and everything before it) is complete
-        with torch.cuda.stream(aux):
-          aux.wait_event(ev)
-          self._plan('wgrad', l).run()
-        self._plan('dgrad', l).run()
-        self._k(2)
-        pboff, pn = self._b_off[l - 2]
-        if l == self.L:
-          main.wait_event(ev_zero)
-        nat.sage_scatter_bwd(self.dA[l], self.dims_in[l - 1], ar.counters, nh, ell, ks, ar.deg, self.dH[l - 1])
-        self._k(1 + nat.relu_bwd_cast(self.dH[l - 1], self.Z[l - 1], ar.counters, nh + 1, self.dPre[l - 1],
-                                      self.g32[pboff:pboff + pn], True, 1.0 / (1.0 - self.dropout)))
-        continue
-      if self.use_tc_gemm:
-        self._plan('wgrad' if overlap else 'bwd', l).run()
-        self._k(1)
-        if overlap:
-          main.wait_stream(aux)             # join: every weight gradient is in the flat buffer
-      else:
-        gW = self.g32[off:off + n * k].view(n, k)
-        # dW = dPre^T A accumulated in fp32 straight into the flat gradient buffer
-        self._mm_f32(self.dPre[l].t(), self._A(l), gW)
-        self._lib(1)
-        if l > 1:
-          torch.mm(self.dPre[l], self.W(l), out=self.dA[l])
-          self._lib(1)
-      # bias gradients are fused into the kernels that produce dPre (loss / relu_bwd_cast)
+      self._plan('bwd', l).run()
+      self._k(1)
       if l > 1:
         pboff, pn = self._b_off[l - 2]
-        if self.use_gather_bwd:
-          nat.sage_gather_bwd(self.dA[l], self.dims_in[l - 1], ar, nh, self.Z[l - 1], self.dPre[l - 1],
-                              self.g32[pboff:pboff + pn], True, 1.0 / (1.0 - self.dropout))
-          self._k(1)
-          continue
-        nat.zero_rows(self.dH[l - 1], ar.counters, nh + 1)
+        self.nat.sage_gather_bwd(self.dA[l], self.dims_in[l - 1], self.arena, self.L - l + 1, self.Z[l - 1],
+                                 self.dPre[l - 1], self.g32[pboff:pboff + pn], True, 1.0 / (1.0 - self.dropout))
         self._k(1)
-        nat.sage_scatter_bwd(self.dA[l], self.dims_in[l - 1], ar.counters, nh, ell, ks, ar.deg, self.dH[l - 1])
-        self._k(1 + nat.relu_bwd_cast(self.dH[l - 1], self.Z[l - 1], ar.counters, nh + 1, self.dPre[l - 1],
-                                      self.g32[pboff:pboff + pn], True, 1.0 / (1.0 - self.dropout)))
-
-  _f32_mode = None
-
-  def _mm_f32(self, a, b, out):
-    """out(fp32) = a(bf16) @ b(bf16) with fp32 accumulation/output when cuBLASLt offers it."""
-    if GraphSageEngine._f32_mode is None:
-      try:
-        torch.mm(a, b, out_dtype=torch.float32, out=out)
-        GraphSageEngine._f32_mode = 'out'
-        return
-      except Exception:
-        try:
-          out.copy_(torch.mm(a, b, out_dtype=torch.float32))
-          GraphSageEngine._f32_mode = 'ret'
-          return
-        except Exception:
-          GraphSageEngine._f32_mode = 'bf16'
-    if GraphSageEngine._f32_mode == 'out':
-      torch.mm(a, b, out_dtype=torch.float32, out=out)
-    elif GraphSageEngine._f32_mode == 'ret':
-      out.copy_(torch.mm(a, b, out_dtype=torch.float32))
-    else:
-      out.copy_(torch.mm(a, b))
 
   def _optimizer(self):
     # Adam's step counter is advanced by the kernel itself (last block to finish)
@@ -783,7 +678,7 @@ class GraphSageEngine(object):
 
   # ------------------------------------------------------------------ public API
   def warmup_and_capture(self, n_eager: int = 2):
-    """Run a few eager steps (lazy inits, cuBLAS workspaces), then capture the CUDA graphs.
+    """Run a few eager steps (lazy inits, GEMM plans), then capture the CUDA graphs.
     Pipelined engines capture one graph per buffer parity."""
     import os
     with torch.cuda.device(self.device):
@@ -794,10 +689,9 @@ class GraphSageEngine(object):
         if self.pipeline:
           self._sample(0)
         for _ in range(n_eager):
-          self._tally = self._lib_tally = 0
+          self._tally = 0
           self._step_eager()
           self.kernels_per_step = self._tally
-          self.library_gemms_per_step = self._lib_tally
           if self.pipeline:
             self._cur ^= 1
       torch.cuda.current_stream().wait_stream(side)
@@ -809,10 +703,9 @@ class GraphSageEngine(object):
         self._resolve_preagg()
         if self.pipeline:
           self._sample(0)
-        self._tally = self._lib_tally = 0
+        self._tally = 0
         self._step_eager()                      # re-count kernels with the chosen variants
         self.kernels_per_step = self._tally
-        self.library_gemms_per_step = self._lib_tally
         torch.cuda.synchronize()
         self._cur = 0
       self.load_state_dict(saved)

@@ -267,23 +267,17 @@ def test_transposed_adjacency_matches_ell(native):
   assert int(off[ar.tr_off.numel() - 1]) == sum(len(v) for e in exp for v in e.values())
 
 
-def _widths(in_dim, hidden, num_classes):
-  # the original three cases keep their ids ([hidden-gather])
-  legacy = in_dim == 128 and num_classes == 47
-  return pytest.param(in_dim, hidden, num_classes, id=str(hidden) if legacy else f'{in_dim}-{hidden}-{num_classes}')
-
-
 @experimental
-@pytest.mark.parametrize('gather', [True, False])
+@pytest.mark.parametrize('pipeline', [False, True])
 @pytest.mark.parametrize('in_dim,hidden,num_classes', [
-    _widths(128, 256, 47), _widths(128, 512, 47), _widths(128, 64, 47),
-    # together every lane-group shape of the aggregation / scatter kernels (LPR 4 .. VPL 4), hidden widths that do
-    # not divide 2048 (bias gradient in a second pass) and a classifier wider than 256 columns
-    _widths(32, 1024, 8), _widths(256, 192, 47), _widths(1024, 768, 300)])
-def test_backward_matches_pytorch_gather_and_scatter(native, in_dim, hidden, num_classes, gather):
-  """Weight / bias gradients of every layer against fp32 autograd on the same sampled batch, for the atomics-free
-  gather backward and the fp32-atomic scatter backward, at feature widths 32 to 1024, hidden widths 64 to 1024 and 8
-  to 300 classes."""
+    (128, 256, 47), (128, 512, 47), (128, 64, 47),
+    # together every lane-group shape of the aggregation / gather-backward kernels, hidden widths that do not divide
+    # 2048 (bias gradient in a second pass) and a classifier wider than 256 columns
+    (32, 1024, 8), (256, 192, 47), (1024, 768, 300)])
+def test_backward_matches_pytorch_at_every_width(native, in_dim, hidden, num_classes, pipeline):
+  """Weight / bias gradients of every layer against fp32 autograd on the same sampled batch, at feature widths 32 to
+  1024, hidden widths 64 to 1024 and 8 to 300 classes; pipelined engines whose layer 1 runs unfused take its weight
+  gradient from the per-arena, pre-aggregated A operand."""
   ei, topo = rmat_csr(6000, 120000, seed=3)
   g = glt.data.Graph(topo, 'CUDA', 0)
   torch.manual_seed(0)
@@ -293,8 +287,8 @@ def test_backward_matches_pytorch_gather_and_scatter(native, in_dim, hidden, num
   ut.append_shared_tensor(feats)
   eng = GraphSageEngine(g, ut._table(), labels, in_dim=in_dim, num_nodes=6000, fanouts=[5, 4, 3], batch_size=256,
                         hidden=hidden, num_classes=num_classes, device=DEV, use_fused=(hidden <= 256),
-                        use_cuda_graph=False, seed=5, use_gather_bwd=gather)
-  assert eng.use_gather_bwd == gather
+                        use_cuda_graph=False, seed=5, pipeline=pipeline)
+  assert eng.preaggregate == (pipeline and not eng.fused_ok[1])
   eng.seeds_dev.copy_(torch.randperm(6000, device=DEV)[:256])
   eng._sample(); eng._forward(); eng._backward()
   torch.cuda.synchronize()
@@ -320,7 +314,7 @@ def test_backward_matches_pytorch_gather_and_scatter(native, in_dim, hidden, num
     (dict(hidden=96, fanouts=[7, 6]), True),                 # the only hidden layer is the fused layer 1
     (dict(in_dim=200), False),                               # layer-1 weight gradient: A is 400 columns wide
     (dict(in_dim=2048), False),                              # wider than the aggregation kernels' rows
-    (dict(hidden=1536, use_gather_bwd=False), False),
+    (dict(hidden=1536), False),
     (dict(hidden=96), False),                                # layer 2 is unfused: forward GEMM with N = 96
     (dict(hidden=96, fanouts=[7, 6], use_fused=False), False),
     (dict(hidden=100), False),
@@ -499,10 +493,11 @@ def test_dropout_kernel_mask_is_keyed_by_step_and_scaled(native):
   assert torch.allclose(ve[ve > 0], torch.tensor(1.0 / 0.75, device=DEV), rtol=1e-2)
 
 
-@pytest.mark.parametrize('gather', [False, True])
-def test_engine_dropout_forward_backward_matches_pytorch_with_same_mask(native, gather):
-  eng, feats, labels = _setup(dropout=0.5, use_gather_bwd=gather)
-  assert eng.use_gather_bwd == gather
+@pytest.mark.parametrize('layer1', ['unfused', 'fused'])
+def test_engine_dropout_forward_backward_matches_pytorch_with_same_mask(native, layer1):
+  fused = layer1 == 'fused'
+  eng, feats, labels = _setup(dropout=0.5, fused=fused)
+  assert eng.fused_ok[1] == fused
   seeds = torch.randperm(6000, device=DEV)[:256]
   eng.seeds_dev.copy_(seeds)
   eng._sample(); eng._forward(); eng._backward()

@@ -126,9 +126,10 @@ def test_sage_aggregate_matches_fp64_mean(native, d, table, block):
 
 
 # --------------------------------------------------------------------------- scatter backward
-@pytest.mark.parametrize('block', [False, True])
+@pytest.mark.parametrize('layout', ['rows', 'block'])
 @pytest.mark.parametrize('d', AGG_WIDTHS)
-def test_sage_scatter_matches_fp64_sum(native, d, block):
+def test_sage_scatter_matches_fp64_sum(native, d, layout):
+  """rows: dA rows are [mean | self]; block: the mean and self blocks sit at offsets inside wider, padded rows."""
   n_src = 500                                  # ~1900 edges: sources are shared by many target rows
   cum, deg, ells = _structure(n_src, seed=d + 7)
   ell, ks, deg_d = _args(cum, deg, ells)
@@ -137,15 +138,12 @@ def test_sage_scatter_matches_fp64_sum(native, d, block):
   for cap, total in ((cum[-1] + 37, None), (cum[-1] - 20, cum[-1] + 1000)):
     ctr = _counters(cum, total)
     T = min(cum[-1] if total is None else total, cap)
-    ld, mcol, scol = (2 * d + 32, 8, d + 24) if block else (2 * d, 0, d)
+    ld, mcol, scol = (2 * d + 32, 8, d + 24) if layout == 'block' else (2 * d, 0, d)
     dA = (torch.randn(cap, ld, generator=g) * 0.5).to(torch.bfloat16).to(DEV)
     init = torch.randn(n_src, d, generator=g).to(DEV)
     dH = init.clone()
-    if block:
-      native.sage_scatter_block(dA, d, mcol, ctr, 3, ell, ks, deg_d, dH)
-      native.add_block_f32(dA, scol, d, ctr, 3, dH)
-    else:
-      native.sage_scatter_bwd(dA, d, ctr, 3, ell, ks, deg_d, dH)
+    native.sage_scatter_block(dA, d, mcol, ctr, 3, ell, ks, deg_d, dH)
+    native.add_block_f32(dA, scol, d, ctr, 3, dH)
     torch.cuda.synchronize()
     tg, sr = _edges(cum, deg, ells, T)
     dAd = dA.double()
@@ -163,11 +161,11 @@ def test_sage_scatter_matches_fp64_sum(native, d, block):
     # fp32 summation of n terms (the initial value, the self term and one term per edge), each rounded once
     bound = (n + 1).unsqueeze(1) * EPS32 * a
     r = bound_ratio(dH, ref, bound)
-    assert r <= 1.0, (d, block, cap, r)
+    assert r <= 1.0, (d, layout, cap, r)
     ratio = max(ratio, r)
     untouched = n == 1
     assert torch.equal(dH[untouched], init[untouched]), 'rows without a term must keep their value'
-  print(f'scatter d={d} block={block}: max error / bound = {ratio:.3f}')
+  print(f'scatter d={d} layout={layout}: max error / bound = {ratio:.3f}')
 
 
 # --------------------------------------------------------------------------- relu_bwd_cast
@@ -281,7 +279,6 @@ def test_aggregation_kernels_reject_rows_wider_than_1024(native, d):
   dH = torch.zeros(8, d, device=DEV)
   calls = [lambda: native.sage_aggregate(None, None, src, d, ctr, 1, ell, ks, deg, A),
            lambda: native.sage_aggregate_block(None, None, src, d, ctr, 1, ell, ks, deg, A, 0),
-           lambda: native.sage_scatter_bwd(A, d, ctr, 1, ell, ks, deg, dH),
            lambda: native.sage_scatter_block(A, d, 0, ctr, 1, ell, ks, deg, dH)]
   for call in calls:
     with pytest.raises(RuntimeError, match=r'multiple of 8 in \[8, 1024\]'):

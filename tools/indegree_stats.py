@@ -6,7 +6,6 @@ import bench
 
 args = bench.parse_args(['--no-pipeline'])
 dev = torch.device('cuda', 0)
-os.environ['GLT_B200_GATHER_BWD'] = '1'
 eng, pool = bench.build_ours(args, 0, 1, dev)
 ar = eng.arena
 for it in range(3):
