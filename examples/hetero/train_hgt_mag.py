@@ -113,6 +113,9 @@ def parse():
   p.add_argument('--zero-copy', action='store_true', help='keep the topology in pinned host memory (reference default)')
   p.add_argument('--mode', choices=['loader', 'engine'], default='loader',
                  help='loader: hetero NeighborLoader + models.HGT under autograd; engine: HeteroHgtEngine (one GPU)')
+  p.add_argument('--eval', choices=['sampled', 'full'], default='sampled',
+                 help='--mode engine: validation accuracy from sampled batches (evaluate_batch), or validation and test '
+                      'accuracy of exact layer-wise full-neighbourhood inference (HeteroHgtEngine.inference)')
   return p.parse_args()
 
 
@@ -128,10 +131,12 @@ def run_engine(args):
     split = None
   if split and 'train' in split and 'paper' in split['train']:
     train_idx, val_idx = split['train']['paper'], split.get('valid', split['train'])['paper']
+    test_idx = split.get('test', split.get('valid', split['train']))['paper']
   else:
     n = sizes['paper']
     perm = torch.randperm(n, generator=torch.Generator().manual_seed(1))
     train_idx, val_idx = perm[: n // 2], perm[n // 2: n // 2 + n // 10]
+    test_idx = perm[n // 2 + n // 10: n // 2 + n // 5]
   graphs, tables, keep = {}, {}, []
   for et, ei in edges.items():
     topo = glt.data.Topology(ei.to(dev), layout='CSC', num_nodes=sizes[et[2]])
@@ -154,6 +159,12 @@ def run_engine(args):
     perm = train_idx[torch.randperm(train_idx.numel())].to(dev)
     losses = [eng.train_step(perm[i:i + args.batch]).clone() for i in range(0, perm.numel(), args.batch)]
     loss = float(torch.stack(losses).mean())
+    if args.eval == 'full':
+      pred = eng.inference().argmax(-1).cpu()
+      val, test = (float((pred[idx] == y[idx]).float().mean()) for idx in (val_idx, test_idx))
+      print(f'Epoch: {epoch:02d}, Loss: {loss:.4f}, Val: {val:.4f}, Test: {test:.4f} (full-neighbourhood), '
+            f'Time: {time.time() - t0:.2f}s')
+      continue
     correct = seen = 0
     for i in range(0, val_idx.numel(), args.batch):
       _, c, n = eng.evaluate_batch(val_idx[i:i + args.batch].to(dev))

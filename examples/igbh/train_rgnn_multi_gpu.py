@@ -177,6 +177,13 @@ def run_engine(rank, world, igbh, a, port):
       print(f'epoch {epoch}: loss {float(loss.item()):.4f} ({time.time() - t0:.2f}s, '
             f'{steps * a.train_batch_size * world / (time.time() - t0):.0f} seeds/s, dropped={eng.overflow_count()})',
             flush=True)
+      # exact layer-wise full-neighbourhood inference (not collective: peer shards are read in place)
+      pred = eng.inference().argmax(-1).cpu()
+      acc = float((pred[val_idx] == label[val_idx]).float().mean())
+      log.event('EVAL_ACCURACY', acc, {'epoch_num': epoch + 1})
+      print(f'epoch {epoch}: val-acc {acc:.4f} (full-neighbourhood)', flush=True)
+    if world > 1:
+      dist.barrier()
   if rank == 0:
     log.end('RUN')
   eng.close()

@@ -883,16 +883,17 @@ static void sage_scatter_block(const Tensor& dA, int64_t d, int64_t mean_col, co
 // global id) is the source of deeper layers; without it the rows come from `feat` (bf16 or MXFP8 rows, layer 1).
 static void sage_full_aggregate(GraphHandle* graph, RowTableHandle* feat, const c10::optional<Tensor>& src,
                                 int64_t src_col, int64_t self_col, int64_t d, int64_t r0, int64_t r1, bool combine,
-                                const c10::optional<Tensor>& bias, bool relu, Tensor out) {
+                                const c10::optional<Tensor>& bias, bool relu, Tensor out, bool mean_only) {
   c10::cuda::CUDAGuard guard(out.device());
   TORCH_CHECK(graph != nullptr && graph->tbl.num_parts > 0, "sage_full_aggregate: graph has no shards");
+  TORCH_CHECK(!(combine && mean_only), "sage_full_aggregate: mean_only writes the mean block of the concat mode, not combine");
   TORCH_CHECK(d % 8 == 0 && d >= 8 && d <= 1024, "sage_full_aggregate: d must be a multiple of 8 in [8, 1024]");
   TORCH_CHECK(0 <= r0 && r0 <= r1 && r1 <= graph->num_rows, "sage_full_aggregate: rows [r0, r1) outside the graph");
   TORCH_CHECK(out.is_cuda() && out.scalar_type() == torch::kBFloat16 && out.dim() == 2 && out.stride(1) == 1 &&
               out.stride(0) % 8 == 0 && reinterpret_cast<uintptr_t>(out.data_ptr()) % 16 == 0 &&
-              out.size(0) >= r1 - r0 && out.size(1) >= (combine ? d : 2 * d),
-              "sage_full_aggregate: out must be bf16 [>= r1 - r0, >= ", combine ? "d" : "2d",
-              "] with unit inner stride and 16-byte aligned rows");
+              out.size(0) >= r1 - r0 && out.size(1) >= (combine || mean_only ? d : 2 * d),
+              combine || mean_only ? "sage_full_aggregate: out must be bf16 [>= r1 - r0, >= d] with unit inner stride and 16-byte aligned rows"
+                                   : "sage_full_aggregate: out must be bf16 [>= r1 - r0, >= 2d] with unit inner stride and 16-byte aligned rows");
   SageFullAggArgs a{};
   a.g = graph->tbl;
   a.d = static_cast<int>(d);
@@ -901,11 +902,13 @@ static void sage_full_aggregate(GraphHandle* graph, RowTableHandle* feat, const 
   a.combine = combine ? 1 : 0;
   a.out = out.data_ptr();
   a.out_ld = out.stride(0);
+  a.mean_only = mean_only ? 1 : 0;
   if (src.has_value() && src->defined()) {
     TORCH_CHECK(src->is_cuda() && src->scalar_type() == torch::kBFloat16 && src->dim() == 2 && src->stride(1) == 1 &&
                 src->stride(0) % 8 == 0 && reinterpret_cast<uintptr_t>(src->data_ptr()) % 16 == 0,
                 "sage_full_aggregate: src must be a bf16 CUDA table with unit inner stride and 16-byte aligned rows");
-    TORCH_CHECK(src->size(0) >= graph->num_rows, "sage_full_aggregate: src needs one row per graph node");
+    // (mean only: src is the source type's table, read only at neighbour ids -- those outside it read as zero rows)
+    TORCH_CHECK(mean_only || src->size(0) >= graph->num_rows, "sage_full_aggregate: src needs one row per graph node");
     TORCH_CHECK(src_col >= 0 && src_col % 8 == 0 && src_col + d <= src->size(1) && self_col >= 0 && self_col % 8 == 0 &&
                 self_col + d <= src->size(1), "sage_full_aggregate: column blocks outside src");
     a.src = src->data_ptr();
@@ -1338,6 +1341,96 @@ static void hgt_attention_bwd(const Tensor& du, const Tensor& qq, Tensor dqq, in
   }
   launch_hgt_attention_bwd(a, cur_stream());
   check_cuda_err("hgt_attention_bwd");
+}
+
+// ---- full-neighbourhood attention of the heterogeneous inference (cuda/hetero_infer.cu) ---------------------------
+// R-GAT, one relation: targets are the global rows [r0, r1) of `graph` (its columns index P / as), acc and Z are
+// chunk rows.  first / last / bias / act as in gat_aggregate, without dropout.
+static void gat_full_aggregate(GraphHandle* graph, const Tensor& P, const Tensor& as, const Tensor& ad, int64_t heads,
+                               int64_t r0, int64_t r1, const c10::optional<Tensor>& acc, bool first, bool last,
+                               const c10::optional<Tensor>& bias, bool act, const c10::optional<Tensor>& Z) {
+  c10::cuda::CUDAGuard guard(P.device());
+  TORCH_CHECK(graph != nullptr && graph->tbl.num_parts > 0, "gat_full_aggregate: graph has no shards");
+  TORCH_CHECK(0 <= r0 && r0 <= r1 && r1 <= graph->num_rows, "gat_full_aggregate: rows [r0, r1) outside the graph");
+  const int64_t H = P.size(1);
+  check_gat_width(H, heads);
+  check_rows(P, torch::kBFloat16, H, "gat_full_aggregate: P must be contiguous bf16 [rows, H]");
+  check_rows(as, torch::kFloat32, heads, "gat_full_aggregate: as must be contiguous fp32 [rows, heads]");
+  check_rows(ad, torch::kFloat32, heads, "gat_full_aggregate: ad must be contiguous fp32 [rows, heads]");
+  TORCH_CHECK(as.size(0) >= P.size(0), "gat_full_aggregate: as has fewer rows than P");
+  TORCH_CHECK(ad.size(0) >= r1, "gat_full_aggregate: ad needs a row for every target id below r1");
+  GatFullAggArgs a{};
+  a.g = graph->tbl;
+  a.P = P.data_ptr(); a.as = as.data_ptr<float>(); a.ad = ad.data_ptr<float>();
+  a.n_src = P.size(0);
+  a.H = H; a.heads = heads;
+  a.r0 = r0; a.r1 = r1;
+  a.first = first ? 1 : 0; a.last = last ? 1 : 0;
+  if (!(first && last)) {
+    TORCH_CHECK(has(acc), "gat_full_aggregate: a relation sum over several launches needs acc");
+    check_rows(*acc, torch::kFloat32, H, "gat_full_aggregate: acc must be contiguous fp32 [rows, H]");
+    TORCH_CHECK(acc->size(0) >= r1 - r0, "gat_full_aggregate: acc needs r1 - r0 rows");
+    a.acc = acc->data_ptr<float>();
+  }
+  if (last) {
+    TORCH_CHECK(has(Z), "gat_full_aggregate: the last relation writes Z");
+    check_rows(*Z, torch::kBFloat16, H, "gat_full_aggregate: Z must be contiguous bf16 [rows, H]");
+    TORCH_CHECK(Z->size(0) >= r1 - r0, "gat_full_aggregate: Z needs r1 - r0 rows");
+    a.z = Z->data_ptr();
+    if (has(bias)) {
+      TORCH_CHECK(bias->is_cuda() && bias->scalar_type() == torch::kBFloat16 && bias->is_contiguous() &&
+                  bias->numel() % H == 0 && reinterpret_cast<uintptr_t>(bias->data_ptr()) % 16 == 0,
+                  "gat_full_aggregate: bias must be 16-byte aligned bf16 [n_bias * H]");
+      a.bias = bias->data_ptr();
+      a.n_bias = bias->numel() / H;
+    }
+    a.act = act ? 1 : 0;
+  }
+  launch_gat_full_aggregate(a, cur_stream());
+  check_cuda_err("gat_full_aggregate");
+}
+
+// HGT, one destination type: graphs[r] (targets [r0, r1) are its rows) with the source type's [K | Q | V] table kv[r]
+// and prior[r]; qq / u are chunk rows [r1 - r0, n_rel * H].
+static void hgt_full_attention(const std::vector<GraphHandle*>& graphs, const Tensor& qq, Tensor u, int64_t heads,
+                               int64_t r0, int64_t r1, const std::vector<Tensor>& kv, const std::vector<Tensor>& prior) {
+  c10::cuda::CUDAGuard guard(qq.device());
+  const int64_t R = static_cast<int64_t>(kv.size());
+  TORCH_CHECK(R >= 1 && R <= kHgtMaxRel, "hgt: a destination type takes 1 to 8 relations");
+  TORCH_CHECK(graphs.size() == static_cast<size_t>(R) && prior.size() == static_cast<size_t>(R),
+              "hgt_full_attention: graphs, kv and prior need one entry per relation");
+  TORCH_CHECK(qq.dim() == 2 && qq.size(1) % R == 0, "hgt_full_attention: qq must be [rows, n_rel * H]");
+  const int64_t H = qq.size(1) / R;
+  check_hgt_width(H, heads);
+  check_rows(qq, torch::kBFloat16, R * H, "hgt_full_attention: qq must be contiguous bf16 [rows, n_rel * H]");
+  check_rows(u, torch::kBFloat16, R * H, "hgt_full_attention: u must be contiguous bf16 [rows, n_rel * H]");
+  TORCH_CHECK(0 <= r0 && r0 <= r1 && qq.size(0) >= r1 - r0 && u.size(0) >= r1 - r0,
+              "hgt_full_attention: qq and u need r1 - r0 rows");
+  HgtFullAttnArgs a{};
+  std::vector<GraphTable> tbl(R);
+  for (int64_t r = 0; r < R; ++r) {
+    TORCH_CHECK(graphs[r] != nullptr && graphs[r]->tbl.num_parts > 0, "hgt_full_attention: graph has no shards");
+    TORCH_CHECK(r1 <= graphs[r]->num_rows, "hgt_full_attention: rows [r0, r1) outside a relation graph");
+    check_rows(kv[r], torch::kBFloat16, 3 * H, "hgt_full_attention: kv must be contiguous bf16 [rows, 3H]");
+    TORCH_CHECK(prior[r].is_cuda() && prior[r].scalar_type() == torch::kFloat32 && prior[r].numel() == heads &&
+                prior[r].is_contiguous(), "hgt_full_attention: prior must be fp32 [heads]");
+    tbl[r] = graphs[r]->tbl;
+    a.kv[r] = kv[r].data_ptr();
+    a.n_src[r] = kv[r].size(0);
+    a.prior[r] = prior[r].data_ptr<float>();
+  }
+  // the relation tables (up to 8 x 776 bytes) go to the device in one stream-ordered copy
+  Tensor host = torch::empty({static_cast<int64_t>(R * sizeof(GraphTable))},
+                             torch::TensorOptions().dtype(torch::kUInt8).pinned_memory(true));
+  std::memcpy(host.data_ptr(), tbl.data(), R * sizeof(GraphTable));
+  Tensor dev_tbl = host.to(qq.device(), /*non_blocking=*/true);
+  a.g = reinterpret_cast<const GraphTable*>(dev_tbl.data_ptr());
+  a.n_rel = R; a.H = H; a.heads = heads; a.kv_ld = 3 * H; a.v_off = 2 * H;
+  a.scale = static_cast<float>(1.0 / std::sqrt(static_cast<double>(H / heads)));
+  a.qq = qq.data_ptr(); a.u = u.data_ptr();
+  a.r0 = r0; a.r1 = r1;
+  launch_hgt_full_attention(a, cur_stream());
+  check_cuda_err("hgt_full_attention");
 }
 
 static void hgt_gelu(const Tensor& X, Tensor Y, const Tensor& counters, int64_t n_hops, const c10::optional<Tensor>& dY) {
@@ -2091,7 +2184,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("sage_aggregate", &sage_aggregate);
   m.def("sage_full_aggregate", &sage_full_aggregate, py::arg("graph"), py::arg("feat"), py::arg("src"),
         py::arg("src_col"), py::arg("self_col"), py::arg("d"), py::arg("r0"), py::arg("r1"), py::arg("combine"),
-        py::arg("bias"), py::arg("relu"), py::arg("out"));
+        py::arg("bias"), py::arg("relu"), py::arg("out"), py::arg("mean_only") = false);
   m.def("sage_aggregate_block", &sage_aggregate_block);
   m.def("sage_scatter_block", &sage_scatter_block);
   m.def("add_block_f32", &add_block_f32);
@@ -2126,6 +2219,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("gat_act_bwd", &gat_act_bwd, py::arg("dH"), py::arg("Z"), py::arg("dPre"), py::arg("counters"),
         py::arg("n_hops"), py::arg("p") = 0.0, py::arg("seed") = 0, py::arg("layer") = 0,
         py::arg("step_dev") = py::none(), py::arg("bias_g") = py::none());
+  m.def("gat_full_aggregate", &gat_full_aggregate, py::arg("graph"), py::arg("P"), py::arg("as_"), py::arg("ad"),
+        py::arg("heads"), py::arg("r0"), py::arg("r1"), py::arg("acc") = py::none(), py::arg("first") = true,
+        py::arg("last") = true, py::arg("bias") = py::none(), py::arg("act") = false, py::arg("Z") = py::none());
+  m.def("hgt_full_attention", &hgt_full_attention, py::arg("graphs"), py::arg("qq"), py::arg("u"), py::arg("heads"),
+        py::arg("r0"), py::arg("r1"), py::arg("kv"), py::arg("prior"));
   m.def("hgt_attention", &hgt_attention, py::arg("qq"), py::arg("u"), py::arg("heads"), py::arg("counters"),
         py::arg("n_hops_targets"), py::arg("kv"), py::arg("prior"), py::arg("ell"), py::arg("ks"), py::arg("deg"),
         py::arg("alpha"));

@@ -194,6 +194,8 @@ void launch_sage_aggregate(const SageAggArgs& a, cudaStream_t s);
 // multiplicity, degree 0 -> 0), accumulated in fp32 in a fixed order and rounded once:
 //   concat  (combine = 0): out[r - r0] = bf16([mean_u x_u | x_r])                       (out width >= 2d)
 //   combine (combine = 1): out[r - r0] = bf16(act(mean_u src[u, src_col:] + src[r, self_col:] + bias))
+//   mean only (combine = 0, mean_only = 1): out[r - r0, :d] = bf16(mean_u x_u), nothing else is written (one relation's
+//                                           column block of a heterogeneous layer's wider A operand)
 // Sources: the dense bf16 table `src` (row u at src + u * src_ld, ids outside [0, n_src) read as zero rows), or,
 // when src == nullptr, the feature table `feat` (bf16 rows of d elements, or MXFP8 rows with feat_fp8 = 1, d = 128).
 struct SageFullAggArgs {
@@ -211,6 +213,7 @@ struct SageFullAggArgs {
   int relu;                     // combine: ReLU after the bias
   void* out;                    // bf16 [r1 - r0, out_ld]
   int64_t out_ld;
+  int mean_only;                // concat without the self block
 };
 void launch_sage_full_aggregate(const SageFullAggArgs& a, cudaStream_t s);
 
@@ -615,6 +618,53 @@ struct TcMxArgs {
   int relu;
 };
 void launch_tc_gemm_mx(const void* maps3, const TcMxArgs& a, int num_sms, cudaStream_t s);
+// ---- hetero_infer.cu (full-neighbourhood attention of the heterogeneous engines' layer-wise inference) ----------
+// Both kernels walk the COMPLETE CSR row of every target r in [r0, r1) (global ids of the destination type; rows of the
+// relation graph are targets, columns are global source ids, ids outside [0, n_src) are skipped).  A row is reduced by
+// one lane group, or, above kHeteroHubDeg neighbours (HGT: summed over its relations), by the whole CTA with per-group
+// partials merged in group order.  The path depends on the degree alone, so every row has one fixed reduction order:
+// no floating-point atomics, bitwise identical for any chunking.  Every exp is of a score minus its row maximum.
+constexpr int kHeteroHubDeg = 256;
+
+// R-GAT, one relation r = (s -> t):  e_ij,h = leaky_relu(as[j, h] + ad[i, h], 0.2),  alpha = softmax over i's complete
+// in-row per head,  out_i = concat_h sum_j alpha_ij,h P[j, h-block]  (fp32).  first / last as in GatAggArgs:
+// acc[i - r0] = out (first) or += out; the last relation writes z[i - r0] = bf16(act(acc + out + sum_b bias[b])),
+// act = leaky_relu(., 0.01).  A target without neighbours in r contributes 0 (its output is the bias sum).
+struct GatFullAggArgs {
+  GraphTable g;
+  const void* P;                // bf16 [n_src, H] source projections
+  const float* as;              // fp32 [n_src, heads]
+  const float* ad;              // fp32 [>= r1, heads] target scores, by global target id
+  int64_t n_src;
+  int H, heads;
+  int64_t r0, r1;
+  float* acc;                   // fp32 [r1 - r0, H]
+  int first, last;
+  const void* bias;             // bf16 [n_bias, H]
+  int n_bias;
+  int act;
+  void* z;                      // bf16 [r1 - r0, H]
+};
+void launch_gat_full_aggregate(const GatFullAggArgs& a, cudaStream_t s);
+
+// HGT, one destination type with n_rel <= kHgtMaxRel relations (g[r]: device array of their CSR tables):
+//   s_ij,h = <qq_r[i, h], k_j,h> prior_r[h] scale   for every neighbour j of i in every relation r
+//   alpha  = one softmax per (i, h) over all of them,   u_r[i, h] = bf16(sum_{j in r} alpha_ij,h v_j,h)
+// qq and u are chunk rows ([r1 - r0, n_rel * H]); kv[r] is the source type's [K | Q | V] table (bf16 [n_src, kv_ld],
+// V at column v_off) by global id.
+struct HgtFullAttnArgs {
+  const GraphTable* g;          // device [n_rel]
+  const void* kv[kHgtMaxRel];
+  int64_t n_src[kHgtMaxRel];
+  const float* prior[kHgtMaxRel];   // fp32 [heads]
+  int n_rel, H, heads, kv_ld, v_off;
+  float scale;                  // 1 / sqrt(D)
+  const void* qq;
+  void* u;
+  int64_t r0, r1;
+};
+void launch_hgt_full_attention(const HgtFullAttnArgs& a, cudaStream_t s);
+
 // programmatic-dependent-launch switch (launch_utils.h); returns the previous value
 int set_pdl(int on);
 void launch_tc_gemm(const TcGemmLaunch& L, int num_sms, cudaStream_t s);

@@ -82,7 +82,7 @@ struct FullAgg {
     }
   }
 
-  // concat: out = bf16([mean | self]);  combine: out = act(mean + src[r, self_col:] + b)
+  // concat: out = bf16([mean | self]) (mean only: bf16(mean));  combine: out = act(mean + src[r, self_col:] + b)
   __device__ static void epilogue(const SageFullAggArgs& a, int64_t r, int deg, int gl, const float (&acc)[VPL][EPV]) {
     const float inv = deg > 0 ? 1.f / static_cast<float>(deg) : 0.f;
     uint8_t* o = reinterpret_cast<uint8_t*>(a.out) + (r - a.r0) * a.out_ld * 2;
@@ -94,13 +94,16 @@ struct FullAgg {
       if (sp) mxfp8x16_accum(ld_nc_v4(sp + gl * 16), ld_nc_u32(sp + a.d), gl, self);
       reinterpret_cast<uint4*>(o)[gl * 2] = pack_bf16x8(acc[0], inv);
       reinterpret_cast<uint4*>(o)[gl * 2 + 1] = pack_bf16x8(acc[0] + 8, inv);
+      if (a.mean_only) return;
       reinterpret_cast<uint4*>(o + a.d * 2)[gl * 2] = pack_bf16x8(self, 1.f);
       reinterpret_cast<uint4*>(o + a.d * 2)[gl * 2 + 1] = pack_bf16x8(self + 8, 1.f);
       return;
     }
     const int nvec = a.d >> 3;
     const uint8_t* sp;
-    if (a.src)
+    if (a.mean_only)
+      sp = nullptr;
+    else if (a.src)
       sp = reinterpret_cast<const uint8_t*>(a.src) + (r * a.src_ld + a.self_col) * 2;
     else
       sp = row_ptr(a.feat, r);
@@ -111,7 +114,7 @@ struct FullAgg {
       const uint4 sv = sp ? ld_nc_v4(sp + c * 16) : make_uint4(0, 0, 0, 0);
       if (!a.combine) {
         reinterpret_cast<uint4*>(o)[c] = pack_bf16x8(acc[v], inv);
-        reinterpret_cast<uint4*>(o + a.d * 2)[c] = sv;
+        if (!a.mean_only) reinterpret_cast<uint4*>(o + a.d * 2)[c] = sv;
       } else {
         float z[8], b[8];
 #pragma unroll

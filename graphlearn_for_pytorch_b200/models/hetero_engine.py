@@ -112,6 +112,7 @@ class HeteroSageEngine(object):
         graphs[et].lazy_init()
         handles.append(graphs[et].graph_handler)
       nn_list = [int(num_nodes[t]) for t in self.ntypes]
+      self._n_nodes = nn_list
       max_seeds = [self.bs if t == seed_type else 0 for t in self.ntypes]
       self.arena = self.nat.HeteroArena(dev.index, NT, handles, self.kt, self.nt, self.fan, nn_list, max_seeds,
                                         False, self.seed, False, False, int(cap_limit), [])
@@ -388,6 +389,109 @@ class HeteroSageEngine(object):
     self._forward()
     st = self.tid[self.seed_type]
     return float(self.loss.item()), int(self.correct.item()), int(self._ctr[st][1].item())
+
+  # ------------------------------------------------------------------ full-neighbourhood inference
+  @torch.no_grad()
+  def inference(self, chunk_rows: Optional[int] = None) -> torch.Tensor:
+    """Exact layer-wise full-neighbourhood inference: bf16 logits [num_nodes[seed_type], num_classes] of every node of
+    the seed type.
+
+    Every layer uses each node's complete CSR row in every relation (the `fanout >= degree` limit of the training
+    forward), with the bf16 parameters of the training forward, no dropout and the same activations (R-SAGE: ReLU;
+    R-GAT: leaky_relu(0.01); HGT: GELU, the skip gate, and ReLU on the input layer).  Layer l computes every node of
+    every type in `targets[l]` from exactly the relations `in_rel[l][t]`, and the last layer only the seed type, so the
+    model is the sampled one: `inference()[seeds]` equals the sampled forward when every relation's fan-out is at least
+    every in-degree and is positive at every hop.
+
+    Runs on the current stream, so it sees every step queued before it.  The per-type activation tables (one or two
+    per type: ping-pong between layers), the per-relation projection / score / attention buffers of the layer being
+    computed and one chunk of `chunk_rows` rows for the aggregation operands are allocated for the call only;
+    parameters, optimizer state, gradients, arenas, `step_dev`, the sampler step and captured graphs are not touched,
+    and training can continue afterwards.  No reduction uses floating-point atomics, so the result is bitwise identical
+    from call to call and for any `chunk_rows` (None sizes the chunk from free device memory).
+
+    Not collective: with several GPUs a rank reads peer graph shards and feature rows in place."""
+    dev, L = self.device, self.L
+    st = self.tid[self.seed_type]
+    with torch.cuda.device(dev):
+      if chunk_rows is None:
+        free, _ = torch.cuda.mem_get_info(dev)
+        chunk_rows = max(4096, min(1 << 19, free // 4 // self._infer_chunk_row_bytes()))
+      chunk_rows = max(1, min(int(chunk_rows), max(self._n_nodes)))
+      # TcGemm / elementwise row counts read on the device: [0] one chunk, [1 + t] every node of type t
+      self._rows_dev = torch.tensor([chunk_rows] + self._n_nodes, dtype=torch.int32, device=dev)
+      self._ids = torch.arange(max(self._n_nodes), dtype=torch.int64, device=dev)
+      X = self._infer_input(chunk_rows)
+      for l in range(1, L + 1):
+        Z = {t: torch.empty(self._n_nodes[t], self._infer_width(l), dtype=torch.bfloat16, device=dev)
+             for t in self.targets[l]}
+        self._infer_layer(l, X, Z, chunk_rows)
+        X = Z
+      out = self._infer_head(X[st])
+      self._rows_dev = self._ids = None
+      return out[:, :self.C].contiguous()
+
+  def _chunks(self, n: int, chunk_rows: int):
+    for r0 in range(0, n, chunk_rows):
+      yield r0, min(n, r0 + chunk_rows)
+
+  def _gh(self, r: int):
+    return self.graphs[self.edge_types[r]].graph_handler
+
+  def _infer_chunk_row_bytes(self) -> int:
+    """Bytes per chunk row of the call's chunk buffers (sizes the default chunk)."""
+    return 2 * max(A.shape[1] for l in range(1, self.L + 1) for A in self.A[l].values())
+
+  def _infer_width(self, l: int) -> int:
+    return self.hidden if l < self.L else self.n_out_pad
+
+  def _infer_input(self, chunk_rows: int):
+    """Input tables of layer 1 (None: layer 1 reads the feature tables)."""
+    return None
+
+  def _infer_head(self, X: torch.Tensor) -> torch.Tensor:
+    return X
+
+  def _gather_chunk(self, t: int, r0: int, r1: int, buf: torch.Tensor) -> torch.Tensor:
+    """bf16 feature rows [r0, r1) of type t, gathered from its feature table (any memory tier) into buf."""
+    d = self.dim_in[self.ntypes[t]]
+    x = buf[:(r1 - r0) * d].view(r1 - r0, d)
+    self.feat[self.ntypes[t]].gather_into(self._ids[r0:r1], None, None, x)
+    return x
+
+  def _gemm(self, A, W, b, relu, out, idx):
+    g = self.nat.TcGemm(self.device.index)
+    g.add_forward(A, W, b, relu, out, self._rows_dev, idx)
+    g.run()
+
+  def _infer_layer(self, l: int, X, Z, chunk_rows: int):
+    """R-SAGE layer l: A_t = [mean_r1 | ... | mean_rk | self] per chunk (sage_full_aggregate, mean-only blocks), then
+    one TcGemm against W_t with the bias and, below the top layer, ReLU."""
+    nat, dev = self.nat, self.device
+    K_max = max(self.A[l][t].shape[1] for t in self.targets[l])
+    buf = torch.empty(chunk_rows * K_max, dtype=torch.bfloat16, device=dev)
+    for t in self.targets[l]:
+      offs, self_col = self.col[l][t]
+      d_t = self._width_in(l, t)
+      K = self_col + d_t
+      for r0, r1 in self._chunks(self._n_nodes[t], chunk_rows):
+        a = buf[:(r1 - r0) * K].view(r1 - r0, K)
+        for j, r in enumerate(self.in_rel[l][t]):
+          s = self.nt[r]
+          d = self._width_in(l, s)
+          blk = a[:, offs[j]:offs[j] + d]
+          if l == 1:
+            nat.sage_full_aggregate(self._gh(r), self.feat[self.ntypes[s]], None, 0, 0, d, r0, r1, False, None, False,
+                                    blk, mean_only=True)
+          else:
+            nat.sage_full_aggregate(self._gh(r), None, X[s], 0, 0, d, r0, r1, False, None, False, blk,
+                                    mean_only=True)
+        blk = a[:, self_col:K]
+        if l == 1:
+          self.feat[self.ntypes[t]].gather_into(self._ids[r0:r1], None, None, blk)
+        else:
+          blk.copy_(X[t][r0:r1])
+        self._gemm(a, self.W(l, t), self.b(l, t), l < self.L, Z[t][r0:r1], 0)
 
   def overflow_count(self) -> int:
     return int(self.arena.counters[self._ovf_idx].item())

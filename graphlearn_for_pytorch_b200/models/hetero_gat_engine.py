@@ -311,6 +311,56 @@ class HeteroGatEngine(HeteroSageEngine):
                           bias_g=self._bias(l - 1, u, True))
           self._k()
 
+  # ------------------------------------------------------------------ full-neighbourhood inference
+  def _infer_chunk_row_bytes(self) -> int:
+    return 2 * max(self.dim_in.values()) + 4 * self.hidden
+
+  def _infer_width(self, l: int) -> int:
+    return self.hidden
+
+  def _infer_project(self, l: int, X, s: int, W: torch.Tensor, buf: torch.Tensor, chunk_rows: int) -> torch.Tensor:
+    """bf16 [N_s, H] projection X_s W^T of every node of type s (layer 1: feature chunks gathered into buf first)."""
+    P = torch.empty(self._n_nodes[s], self.hidden, dtype=torch.bfloat16, device=self.device)
+    if l > 1:
+      self._gemm(X[s], W, None, False, P, 1 + s)
+      return P
+    for r0, r1 in self._chunks(self._n_nodes[s], chunk_rows):
+      self._gemm(self._gather_chunk(s, r0, r1, buf), W, None, False, P[r0:r1], 0)
+    return P
+
+  def _infer_layer(self, l: int, X, Z, chunk_rows: int):
+    """R-GAT layer l, per relation r = (s -> t): projections over every source (and every target when W_dst is a
+    separate weight), per-node scores (gat_scores), then per chunk of targets the attention over complete rows
+    (gat_full_aggregate), summed over t's relations in relation order; the last adds the biases and the activation."""
+    nat, dev, H, hd = self.nat, self.device, self.hidden, self.heads
+    buf = torch.empty(chunk_rows * max(self.dim_in.values()), dtype=torch.bfloat16, device=dev) if l == 1 else None
+    for t in self.targets[l]:
+      rels = self.in_rel[l][t]
+      ops = []
+      for r in rels:
+        s = self.nt[r]
+        Ps = self._infer_project(l, X, s, self.param(('W_src', l, r)), buf, chunk_rows)
+        Pd = Ps if s == t and ('W_dst', l, r) not in self.param_index else \
+            self._infer_project(l, X, t, self._w_dst(l, r), buf, chunk_rows)
+        as_ = torch.empty(self._n_nodes[s], hd, dtype=torch.float32, device=dev)
+        ad = torch.empty(self._n_nodes[t], hd, dtype=torch.float32, device=dev)
+        nat.gat_scores(Ps, self.param(('att_src', l, r)), as_, self._rows_dev, 1 + s, Pd, self.param(('att_dst', l, r)),
+                       ad, self._rows_dev, 1 + t, heads=hd)
+        del Pd
+        ops.append((r, Ps, as_, ad))
+      acc = torch.empty(chunk_rows, H, dtype=torch.float32, device=dev) if len(rels) > 1 else None
+      for r0, r1 in self._chunks(self._n_nodes[t], chunk_rows):
+        for j, (r, Ps, as_, ad) in enumerate(ops):
+          last = j == len(ops) - 1
+          nat.gat_full_aggregate(self._gh(r), Ps, as_, ad, hd, r0, r1, acc=acc[:r1 - r0] if acc is not None else None,
+                                 first=j == 0, last=last, bias=self._bias(l, t) if last else None, act=l < self.L,
+                                 Z=Z[t][r0:r1] if last else None)
+
+  def _infer_head(self, X: torch.Tensor) -> torch.Tensor:
+    out = torch.empty(X.shape[0], self.n_out_pad, dtype=torch.bfloat16, device=self.device)
+    self._gemm(X, self.param(('head_W',)), self.param(('head_b',)), False, out, 1 + self.tid[self.seed_type])
+    return out
+
   # ------------------------------------------------------------------ public API
   @torch.no_grad()
   def evaluate_batch(self, seeds: torch.Tensor):

@@ -356,3 +356,59 @@ class HeteroHgtEngine(HeteroSageEngine):
                                 self.param(('in_b', u), True), True, 1.0, True))
       self._hgt_plan('in_bwd', 0, u).run()
       self._k()
+
+  # ------------------------------------------------------------------ full-neighbourhood inference
+  def _infer_chunk_row_bytes(self) -> int:
+    R = max(len(self.in_rel[l][t]) for l in range(1, self.L + 1) for t in self.targets[l])
+    return 2 * max(max(self.dim_in.values()), (2 * R + 3) * self.hidden)
+
+  def _infer_width(self, l: int) -> int:
+    return self.hidden
+
+  def _infer_input(self, chunk_rows: int):
+    """Input layer: relu(x W_in^T + b_in) of every node of the input types, from gathered feature chunks."""
+    dev = self.device
+    buf = torch.empty(chunk_rows * max(self.dim_in.values()), dtype=torch.bfloat16, device=dev)
+    X = {}
+    for u in self.in_types:
+      X[u] = torch.empty(self._n_nodes[u], self.hidden, dtype=torch.bfloat16, device=dev)
+      for r0, r1 in self._chunks(self._n_nodes[u], chunk_rows):
+        self._gemm(self._gather_chunk(u, r0, r1, buf), self.param(('in_W', u)), self.param(('in_b', u)), True,
+                   X[u][r0:r1], 0)
+    return X
+
+  def _infer_layer(self, l: int, X, Z, chunk_rows: int):
+    """HGT layer l: K/Q/V of every node of the layer's types, then per destination type and chunk of targets the qq
+    GEMM, the attention over the complete rows of every relation into t (hgt_full_attention), the message GEMM, GELU,
+    Lin_a and the skip gate."""
+    nat, dev, H, hd = self.nat, self.device, self.hidden, self.heads
+    bf = torch.bfloat16
+    KQV = {}
+    for u in self.kqv_types[l]:
+      KQV[u] = torch.empty(self._n_nodes[u], 3 * H, dtype=bf, device=dev)
+      self._gemm(X[u], self.param(('kqv_W', l, u)), self.param(('kqv_b', l, u)), False, KQV[u], 1 + u)
+    for t in self.targets[l]:
+      rels = self.in_rel[l][t]
+      R = len(rels)
+      att_img = torch.empty(R * H, H, dtype=bf, device=dev)
+      msg_img = torch.empty(H, R * H, dtype=bf, device=dev)
+      nat.hgt_blocks(self._blocks('att', l, t), self._blocks('msg', l, t), att_img, msg_img)
+      qq = torch.empty(chunk_rows, R * H, dtype=bf, device=dev)
+      U = torch.empty(chunk_rows, R * H, dtype=bf, device=dev)
+      AGG, GE, A = (torch.empty(chunk_rows, H, dtype=bf, device=dev) for _ in range(3))
+      graphs = [self._gh(r) for r in rels]
+      kv = [KQV[self.nt[r]] for r in rels]
+      prior = [self._p32(('prior', l, r)) for r in rels]
+      for r0, r1 in self._chunks(self._n_nodes[t], chunk_rows):
+        n = r1 - r0
+        self._gemm(KQV[t][r0:r1, H:2 * H], att_img, None, False, qq[:n], 0)
+        nat.hgt_full_attention(graphs, qq[:n], U[:n], hd, r0, r1, kv, prior)
+        self._gemm(U[:n], msg_img, None, False, AGG[:n], 0)
+        nat.hgt_gelu(AGG[:n], GE[:n], self._rows_dev, 0)
+        self._gemm(GE[:n], self.param(('a_W', l, t)), self.param(('a_b', l, t)), False, A[:n], 0)
+        nat.hgt_gate(A[:n], X[t][r0:r1], Z[t][r0:r1], self._p32(('skip', l, t)), self._rows_dev, 0)
+
+  def _infer_head(self, X: torch.Tensor) -> torch.Tensor:
+    out = torch.empty(X.shape[0], self.n_out_pad, dtype=torch.bfloat16, device=self.device)
+    self._gemm(X, self.param(('head_W',)), self.param(('head_b',)), False, out, 1 + self.tid[self.seed_type])
+    return out
