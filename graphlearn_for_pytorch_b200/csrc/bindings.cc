@@ -2135,11 +2135,21 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def_readonly("seed_local", &SamplerArena::seed_local)
       .def_readonly("step", &SamplerArena::step)
       .def("enable_transpose", &SamplerArena::enable_transpose)
+      // rebuilds the transposed adjacency from `counters`, `deg` and `ell` as they stand (sample() builds it itself);
+      // lets a batch laid out by hand be transposed
+      .def("build_transpose", [](SamplerArena& a) {
+        c10::cuda::CUDAGuard guard(a.device);
+        TORCH_CHECK(a.tr_hops > 0, "call enable_transpose(n_hops) first");
+        a.build_transpose(cur_stream());
+        check_cuda_err("build_transpose");
+      })
       .def_readwrite("deterministic", &SamplerArena::deterministic)
       .def_readonly("tr_hops", &SamplerArena::tr_hops)
       .def_readonly("tr_off", &SamplerArena::tr_off)
       .def_readonly("tr_cnt", &SamplerArena::tr_cnt)
       .def_readonly("tr_tgt", &SamplerArena::tr_tgt)
+      .def_readonly("tr_meta", &SamplerArena::tr_meta)
+      .def_readonly("tr_meta_inv", &SamplerArena::tr_meta_inv)
       .def_readonly("ell", &SamplerArena::ell)
       .def_readonly("ell_eids", &SamplerArena::ell_eids)
       .def_readonly("cap_rows", &SamplerArena::cap_rows)

@@ -196,7 +196,8 @@ inline int grid_for(int64_t items, int per_block, int max_blocks = 132 * 16) {
 
 // ------------------------------------------------------------------------------------------
 // Gather-style backward of the mean aggregation:
-//   dPre[s] = relu'(Z[s]) * (dA_self[s] + sum_{t in in(s)} dA_mean[t] / deg[t])       (+ bias column sums)
+//   dPre[s] = relu'(Z[s]) * gscale * (dA_self[s] + sum_{t in in(s)} dA_mean[t] / deg[t])       (+ bias column sums)
+//   (without Z there is no mask, but gscale -- the dropout rescale -- still applies)
 //   * 32 consecutive source rows form a chunk served by a TEAM of warps; every warp of the team reads the chunk's
 //     records ({count, segment start, first two in-neighbours, their 1/deg}: built by k_tr_meta on the sampling
 //     stream, prefetched one chunk ahead) and takes every TEAM-th row;
@@ -369,13 +370,15 @@ __global__ void __launch_bounds__(256, 2) k_sage_gather_bwd(SageGatherBwdArgs a)
         for (int v = 0; v < VPL; ++v) {
           const int c = v * LPR + gl;
           if (c >= nvec) continue;
+#pragma unroll
+          for (int i = 0; i < 8; ++i) acc[v][i] *= gscale;
           if (Zb) {
             float z[8];
 #pragma unroll
             for (int i = 0; i < 8; ++i) z[i] = 0.f;
             bf16x8_accum(vz[u][v], z);
 #pragma unroll
-            for (int i = 0; i < 8; ++i) acc[v][i] = z[i] > 0.f ? acc[v][i] * gscale : 0.f;
+            for (int i = 0; i < 8; ++i) acc[v][i] = z[i] > 0.f ? acc[v][i] : 0.f;
           }
           const uint4 packed = pack_bf16x8(acc[v], 1.f);   // rows in [S, cap_src) come out as zeros
           reinterpret_cast<uint4*>(o)[c] = packed;
@@ -469,13 +472,15 @@ __global__ void __launch_bounds__(256, 2) k_sage_gather_bwd(SageGatherBwdArgs a)
             for (int w = 0; w < TEAM; ++w)
 #pragma unroll
               for (int i = 0; i < 8; ++i) tot[i] += s_col[(w0 + w) * a.d + c * 8 + i];
+#pragma unroll
+            for (int i = 0; i < 8; ++i) tot[i] *= gscale;
             if (Zb) {
               float z[8];
 #pragma unroll
               for (int i = 0; i < 8; ++i) z[i] = 0.f;
               bf16x8_accum(ld_nc_v4(Zb + s * z_row + c * 16), z);
 #pragma unroll
-              for (int i = 0; i < 8; ++i) tot[i] = z[i] > 0.f ? tot[i] * gscale : 0.f;
+              for (int i = 0; i < 8; ++i) tot[i] = z[i] > 0.f ? tot[i] : 0.f;
             }
             const uint4 packed = pack_bf16x8(tot, 1.f);
             reinterpret_cast<uint4*>(o)[c] = packed;
