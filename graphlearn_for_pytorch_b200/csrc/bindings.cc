@@ -267,7 +267,7 @@ struct SamplerArena {
   Tensor nodes, deg, counters, seed_local, scratch, step;
   std::vector<Tensor> ell, ell_eids;
   std::unique_ptr<DeviceTable> table;
-  // optional transposed adjacency (EXPERIMENTAL, see cuda/transpose.cu): built after the hops of
+  // optional transposed adjacency (see cuda/transpose.cu): built after the hops of
   // every sample() once enable_transpose(n_hops) was called
   int tr_hops = 0;
   int64_t tr_cap_edges = 0;
@@ -741,16 +741,6 @@ struct RowTableHandle {
     return out;
   }
 
-  // copy the rows of the batch's nodes that are NOT in this GPU's HBM into xcache[local id] (see launch_stage_remote_rows)
-  void stage_remote_rows(const Tensor& nodes, const Tensor& counters, int64_t n_idx, Tensor xcache) {
-    c10::cuda::CUDAGuard guard(device);
-    TORCH_CHECK(nodes.is_cuda() && nodes.scalar_type() == torch::kInt64 && nodes.is_contiguous());
-    TORCH_CHECK(xcache.is_cuda() && xcache.is_contiguous() &&
-                xcache.numel() * xcache.element_size() >= nodes.numel() * tbl.row_bytes && tbl.row_bytes % 16 == 0);
-    launch_stage_remote_rows(tbl, local_mask, nodes.data_ptr<int64_t>(), counters.data_ptr<int32_t>(), n_idx,
-                             nodes.numel(), xcache.data_ptr(), cur_stream());
-    check_cuda_err("stage_remote_rows");
-  }
   bool all_local() const { return local_mask == ((tbl.num_parts >= 32) ? ~0u : ((1u << tbl.num_parts) - 1u)); }
 
   // rows are MXFP8 (d e4m3 bytes + d/32 UE8M0 scales + padding to 16 bytes): dequantised bf16 [n, d]
@@ -947,7 +937,7 @@ static void add_block_f32(const Tensor& dA, int64_t col, int64_t d, const Tensor
   check_cuda_err("add_block_f32");
 }
 
-// EXPERIMENTAL atomics-free backward of the mean aggregation over the arena's transposed adjacency
+// Atomics-free backward of the mean aggregation over the arena's transposed adjacency
 static void sage_gather_bwd(const Tensor& dA, int64_t d, SamplerArena& ar, int64_t n_hops_targets,
                             const c10::optional<Tensor>& Z, Tensor dPre, const c10::optional<Tensor>& colsum,
                             bool prezeroed, double gscale) {
@@ -1612,15 +1602,6 @@ static void dropout_bf16(Tensor Z, const Tensor& counters, int64_t n_hops, doubl
   check_cuda_err("dropout_bf16");
 }
 
-static void bias_relu(Tensor Z, const Tensor& bias, const Tensor& counters, int64_t n_hops, bool relu) {
-  c10::cuda::CUDAGuard guard(Z.device());
-  TORCH_CHECK(Z.scalar_type() == torch::kBFloat16 && bias.scalar_type() == torch::kBFloat16);
-  TORCH_CHECK(Z.size(1) % 8 == 0 && bias.numel() == Z.size(1));
-  launch_bias_relu(Z.data_ptr(), bias.data_ptr(), counters.data_ptr<int32_t>(), n_hops, Z.size(0),
-                   Z.size(1), relu, cur_stream());
-  check_cuda_err("bias_relu");
-}
-
 // Returns the number of kernels launched (2 when the bias gradient takes a separate column-sum pass).
 static int64_t softmax_nll(const Tensor& logits, int64_t C, const c10::optional<Tensor>& y,
                         const c10::optional<Tensor>& labels_all, const c10::optional<Tensor>& nodes,
@@ -1693,14 +1674,17 @@ static void sage_fused(RowTableHandle* feat, const c10::optional<Tensor>& nodes,
                        const c10::optional<Tensor>& src_local, int64_t d, const Tensor& counters,
                        int64_t n_hops_targets, const std::vector<Tensor>& ell,
                        const std::vector<int64_t>& ks, const Tensor& deg, const Tensor& w_packed,
-                       const Tensor& bias, bool relu, Tensor z, const c10::optional<Tensor>& a_save,
-                       const c10::optional<Tensor>& xcache) {
+                       const Tensor& bias, bool relu, Tensor z, const c10::optional<Tensor>& a_save) {
   c10::cuda::CUDAGuard guard(z.device());
-  const bool fp8 = feat != nullptr && !(src_local.has_value() && src_local->defined()) && feat->dtype == torch::kUInt8;
+  const bool local = src_local.has_value() && src_local->defined();
+  const bool fp8 = feat != nullptr && !local && feat->dtype == torch::kUInt8;
   TORCH_CHECK(!fp8 || d == 128, "the MXFP8 loader of the fused kernel supports d = 128");
   TORCH_CHECK(z.scalar_type() == torch::kBFloat16 && z.is_contiguous());
   const int64_t n_out = z.size(1);
   TORCH_CHECK(sage_fused_supported(d, n_out), "unsupported fused shape d=", d, " n_out=", n_out);
+  TORCH_CHECK(local || feat == nullptr || sage_fused_supported(d, n_out, &feat->tbl),
+              "sage_fused: the fused kernel's 32-bit row handles cannot address this feature table "
+              "(more than 16 parts, or a part of 2^28 rows or more)");
   TORCH_CHECK(w_packed.numel() == 2 * d * n_out && w_packed.scalar_type() == torch::kBFloat16);
   SageFusedArgs f{};
   f.agg = make_agg(feat, nodes, src_local, d, counters, n_hops_targets, z.size(0), ell, ks, deg, nullptr);
@@ -1710,20 +1694,6 @@ static void sage_fused(RowTableHandle* feat, const c10::optional<Tensor>& nodes,
   f.relu = relu;
   f.z = z.data_ptr();
   f.feat_fp8 = fp8 ? 1 : 0;
-  f.local_mask = feat != nullptr ? feat->local_mask : 0u;
-  f.xcache = nullptr;
-  f.cache_part = -1;
-  if (feat != nullptr && xcache.has_value() && xcache->defined()) {
-    // remote rows of the batch were staged into `xcache` (indexed by local node id): reuse a remote part's slot
-    for (int p = 0; p < feat->tbl.num_parts; ++p)
-      if (!((feat->local_mask >> p) & 1u)) { f.cache_part = p; break; }
-    if (f.cache_part >= 0) {
-      TORCH_CHECK(xcache->is_cuda() && xcache->is_contiguous() &&
-                  xcache->numel() * xcache->element_size() >= static_cast<int64_t>(nodes->numel()) * feat->tbl.row_bytes,
-                  "sage_fused: xcache must hold one feature row per arena node");
-      f.xcache = xcache->data_ptr();
-    }
-  }
   f.a_save = nullptr;
   if (a_save.has_value() && a_save->defined()) {
     TORCH_CHECK(a_save->size(0) >= z.size(0) && a_save->size(1) == 2 * d && a_save->is_contiguous());
@@ -1739,8 +1709,7 @@ static void sage_fused(RowTableHandle* feat, const c10::optional<Tensor>& nodes,
 // Tensor maps are encoded once; the batch-dependent extent is read from the sampler's device counters, so
 // run() is a single static launch (CUDA-graph capturable).  Up to two problems share a launch.  The plan owns the
 // kernel's 8-byte work ticket, which the kernel leaves zeroed: launches of one plan must therefore be ordered (never
-// two in flight at once; every engine runs a plan on one stream).  GLT_B200_GEMM_TICKETS=0 keeps the static
-// item striding instead, for A/B measurements.
+// two in flight at once; every engine runs a plan on one stream).
 // ---------------------------------------------------------------------------
 struct TcGemm {
   TcGemmLaunch L;
@@ -1749,11 +1718,8 @@ struct TcGemm {
   Tensor tickets;
   explicit TcGemm(int dev) : device(dev) {
     std::memset(&L, 0, sizeof(L));
-    const char* env = std::getenv("GLT_B200_GEMM_TICKETS");
-    if (!env || std::atoi(env) != 0) {
-      tickets = torch::zeros({2}, torch::dtype(torch::kInt32).device(torch::kCUDA, dev));
-      L.args.tickets = tickets.data_ptr<int32_t>();
-    }
+    tickets = torch::zeros({2}, torch::dtype(torch::kInt32).device(torch::kCUDA, dev));
+    L.args.tickets = tickets.data_ptr<int32_t>();
   }
   static int pick_bn(int64_t n) { return n % 256 == 0 ? 256 : (n % 128 == 0 ? 128 : 64); }
   void check_bf16(const Tensor& t, const char* what) {
@@ -1853,62 +1819,6 @@ struct TcGemm {
   }
 };
 
-
-// ---------------------------------------------------------------------------
-// TcGemmMx: block-scaled MXFP8 forward GEMM (csrc/cuda/tc_gemm_mx.cu).  A / W are e4m3 bytes [rows, K]; sfa / sfb are
-// the UE8M0 scales packed into the tensor core's 512-byte block layout (data/quantize.py pack_mx_scale_blocks).
-// ---------------------------------------------------------------------------
-struct TcGemmMx {
-  alignas(64) unsigned char maps[3][128];
-  TcMxArgs a{};
-  int device;
-  std::vector<Tensor> keep;
-  TcGemmMx(int dev, const Tensor& A, const Tensor& sfa, const Tensor& W, const Tensor& sfb,
-           const c10::optional<Tensor>& bias, bool relu, Tensor Z, const c10::optional<Tensor>& counters,
-           int64_t dyn_idx) : device(dev) {
-    c10::cuda::CUDAGuard guard(static_cast<c10::DeviceIndex>(dev));
-    auto ok8 = [](const Tensor& t) {
-      return t.is_cuda() && t.scalar_type() == torch::kUInt8 && t.dim() == 2 && t.stride(1) == 1 && t.stride(0) % 16 == 0 &&
-             reinterpret_cast<uintptr_t>(t.data_ptr()) % 16 == 0;
-    };
-    TORCH_CHECK(ok8(A) && ok8(W), "TcGemmMx: A / W must be uint8 (e4m3) [rows, K] CUDA tensors, 16-byte aligned rows");
-    const int64_t M = A.size(0), K = A.size(1), N = W.size(0);
-    TORCH_CHECK(W.size(1) == K && K % 128 == 0 && N % 128 == 0 && M >= 128, "TcGemmMx: K, N multiples of 128, M >= 128");
-    TORCH_CHECK(Z.is_cuda() && Z.scalar_type() == torch::kBFloat16 && Z.dim() == 2 && Z.size(0) >= M && Z.size(1) == N &&
-                Z.stride(1) == 1);
-    const int64_t mb = (M + 127) / 128, kb = K / 128;
-    TORCH_CHECK(sfa.is_cuda() && sfa.scalar_type() == torch::kUInt8 && sfa.is_contiguous() && sfa.numel() == mb * kb * 512,
-                "TcGemmMx: sfa must hold ceil(M/128) * K/128 blocks of 512 bytes");
-    TORCH_CHECK(sfb.is_cuda() && sfb.scalar_type() == torch::kUInt8 && sfb.is_contiguous() && sfb.numel() == (N / 128) * kb * 512,
-                "TcGemmMx: sfb must hold N/128 * K/128 blocks of 512 bytes");
-    a.m = M; a.n = N; a.k = K;
-    a.bn = 128;
-    a.dyn = nullptr; a.dyn_idx = 0;
-    if (counters.has_value() && counters->defined()) {
-      TORCH_CHECK(counters->scalar_type() == torch::kInt32 && dyn_idx >= 0 && dyn_idx < counters->numel());
-      a.dyn = counters->data_ptr<int32_t>();
-      a.dyn_idx = static_cast<int>(dyn_idx);
-      keep.push_back(*counters);
-    }
-    a.sfa = sfa.data_ptr(); a.sfb = sfb.data_ptr();
-    a.bias = nullptr;
-    if (bias.has_value() && bias->defined()) {
-      TORCH_CHECK(bias->scalar_type() == torch::kBFloat16 && bias->numel() == N);
-      a.bias = bias->data_ptr();
-      keep.push_back(*bias);
-    }
-    a.relu = relu ? 1 : 0;
-    TORCH_CHECK(make_tmap_u8_2d(maps[0], A.data_ptr(), M, K, A.stride(0), 128, 128) == 0, "tensor map A");
-    TORCH_CHECK(make_tmap_u8_2d(maps[1], W.data_ptr(), N, K, W.stride(0), 128, a.bn) == 0, "tensor map W");
-    TORCH_CHECK(make_tmap_bf16_2d(maps[2], Z.data_ptr(), Z.size(0), N, Z.stride(0), 64, 128) == 0, "tensor map Z");
-    keep.insert(keep.end(), {A, sfa, W, sfb, Z});
-  }
-  void run() {
-    c10::cuda::CUDAGuard guard(static_cast<c10::DeviceIndex>(device));
-    launch_tc_gemm_mx(maps, a, at::cuda::getCurrentDeviceProperties()->multiProcessorCount, cur_stream());
-    check_cuda_err("tc_gemm_mx");
-  }
-};
 
 static void enable_peer_access(int dev, int peer) {
   if (dev == peer) return;
@@ -2187,7 +2097,6 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            py::arg("out_width") = 0)
       .def("gather_into", &RowTableHandle::gather_into)
       .def("gather_mxfp8", &RowTableHandle::gather_mxfp8)
-      .def("stage_remote_rows", &RowTableHandle::stage_remote_rows)
       .def("all_local", &RowTableHandle::all_local);
 
   // ---- GraphSAGE engine ----
@@ -2249,7 +2158,6 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("msg_g") = py::none());
   m.def("hgt_kqv_cast", &hgt_kqv_cast, py::arg("dkv"), py::arg("dq"), py::arg("out"), py::arg("bias_g"),
         py::arg("counters"), py::arg("idx"), py::arg("idx_q"));
-  m.def("bias_relu", &bias_relu);
   m.def("softmax_nll", &softmax_nll, py::arg("logits"), py::arg("C"), py::arg("y"), py::arg("labels_all"),
         py::arg("nodes"), py::arg("counters"), py::arg("loss"), py::arg("dlogits"), py::arg("correct"),
         py::arg("colsum"), py::arg("prezeroed") = false);
@@ -2258,15 +2166,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("zero_rows", &zero_rows);
   m.def("sage_fused", &sage_fused, py::arg("feat"), py::arg("nodes"), py::arg("src_local"), py::arg("d"),
         py::arg("counters"), py::arg("n_hops_targets"), py::arg("ell"), py::arg("ks"), py::arg("deg"),
-        py::arg("w_packed"), py::arg("bias"), py::arg("relu"), py::arg("z"), py::arg("a_save") = py::none(),
-        py::arg("xcache") = py::none());
-  m.def("sage_fused_supported", &sage_fused_supported);
-  m.def("sage_fused_trace", []() {
-    // [132, 32] int64 clock64 timeline of the last fused launch made with GLT_B200_FUSED_TRACE=1
-    Tensor t = torch::zeros({kFusedTraceCtas, kFusedTraceSlots}, torch::kInt64);
-    sage_fused_trace_copy(reinterpret_cast<unsigned long long*>(t.data_ptr<int64_t>()));
-    return t;
-  });
+        py::arg("w_packed"), py::arg("bias"), py::arg("relu"), py::arg("z"), py::arg("a_save") = py::none());
+  m.def("sage_fused_supported",
+        [](int64_t d, int64_t n_out, const RowTableHandle* feat) {
+          return sage_fused_supported(static_cast<int>(d), static_cast<int>(n_out), feat ? &feat->tbl : nullptr);
+        },
+        py::arg("d"), py::arg("n_out"), py::arg("feat") = py::none());
   py::class_<PeerBuffer, std::shared_ptr<PeerBuffer>>(m, "PeerBuffer")
       .def_static("allocate", &PeerBuffer::allocate)
       .def_static("open", &PeerBuffer::open)
@@ -2281,12 +2186,6 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def("adam", &PeerGroup::adam)
       .def_readonly("err", &PeerGroup::err)
       .def_readonly("epoch", &PeerGroup::epoch);
-  py::class_<TcGemmMx>(m, "TcGemmMx")
-      .def(py::init<int, const Tensor&, const Tensor&, const Tensor&, const Tensor&, const c10::optional<Tensor>&, bool,
-                    Tensor, const c10::optional<Tensor>&, int64_t>(),
-           py::arg("device"), py::arg("A"), py::arg("sfa"), py::arg("W"), py::arg("sfb"), py::arg("bias") = py::none(),
-           py::arg("relu") = false, py::arg("Z"), py::arg("counters") = py::none(), py::arg("dyn_idx") = 0)
-      .def("run", &TcGemmMx::run);
   py::class_<TcGemm>(m, "TcGemm")
       .def(py::init<int>())
       .def("add_forward", &TcGemm::add_forward)

@@ -8,7 +8,6 @@
 // rows are narrow, every lane keeps up to four loads in flight, and the row
 // count can stay on the device (n_dev) so the launch is CUDA-graph capturable.
 #include "device_utils.cuh"
-#include "launch_utils.h"
 
 namespace glt {
 
@@ -103,47 +102,6 @@ inline int grid_for(int64_t items, int per_block, int max_blocks = 132 * 16) {
   if (b < 1) b = 1;
   if (b > max_blocks) b = max_blocks;
   return static_cast<int>(b);
-}
-
-// LPR lanes per row, R rows in flight per lane group (same latency x parallelism reasoning as k_gather_vec): only rows
-// that live outside this GPU's HBM are copied.
-template <int LPR, int R>
-__global__ void __launch_bounds__(256) k_stage_remote_rows(RowTable t, unsigned local_mask, const int64_t* nodes,
-                                                           const int32_t* cum, int n_idx, int cap_nodes, uint8_t* xcache) {
-  pdl_enter();
-  constexpr int RPW = 32 / LPR;
-  const int lane = threadIdx.x & 31;
-  const int gl = lane % LPR, gw = lane / LPR;
-  const int n = min(cum[n_idx], cap_nodes);
-  const int nvec = static_cast<int>(t.row_bytes >> 4);
-  const int wpb = blockDim.x >> 5;
-  for (int base = (blockIdx.x * wpb + (threadIdx.x >> 5)) * (RPW * R); base < n; base += gridDim.x * wpb * (RPW * R)) {
-    const uint4* src[R];
-#pragma unroll
-    for (int k = 0; k < R; ++k) {
-      const int s = base + k * RPW + gw;
-      src[k] = nullptr;
-      if (s < n) {
-        const int64_t gid = nodes[s];
-#pragma unroll 1
-        for (int p = 0; p < t.num_parts; ++p)
-          if (gid >= t.row_begin[p] && gid < t.row_begin[p + 1]) {
-            if (!((local_mask >> p) & 1u))
-              src[k] = reinterpret_cast<const uint4*>(reinterpret_cast<const uint8_t*>(t.base[p]) +
-                                                      (gid - t.row_begin[p]) * t.row_bytes);
-            break;
-          }
-      }
-    }
-    for (int c = gl; c < nvec; c += LPR) {
-      uint4 v[R];
-#pragma unroll
-      for (int k = 0; k < R; ++k) v[k] = src[k] ? ld_nc_v4(src[k] + c) : make_uint4(0, 0, 0, 0);
-#pragma unroll
-      for (int k = 0; k < R; ++k)
-        if (src[k]) reinterpret_cast<uint4*>(xcache + static_cast<int64_t>(base + k * RPW + gw) * t.row_bytes)[c] = v[k];
-    }
-  }
 }
 
 // 8 lanes per row, 16 e4m3 elements per lane and iteration (d multiple of 128 keeps every lane busy)
@@ -250,19 +208,6 @@ void launch_gather_mxfp8(RowTable t, const int64_t* idx, int64_t n, int d, void*
   int64_t blocks = (n + 31) / 32;
   if (blocks > 132 * 16) blocks = 132 * 16;
   k_gather_mxfp8<<<static_cast<int>(blocks), 256, 0, s>>>(t, idx, n, d, reinterpret_cast<__nv_bfloat16*>(out));
-}
-
-void launch_stage_remote_rows(RowTable t, unsigned local_mask, const int64_t* nodes, const int32_t* cum, int n_idx,
-                              int cap_nodes, void* xcache, cudaStream_t s) {
-  if (cap_nodes <= 0) return;
-  int blocks = (cap_nodes + 127) / 128;
-  if (blocks > 132 * 8) blocks = 132 * 8;
-  if (t.row_bytes <= 128)
-    launch_k(k_stage_remote_rows<8, 4>, dim3(blocks), dim3(256), 0, s, t, local_mask, nodes, cum, n_idx, cap_nodes,
-             reinterpret_cast<uint8_t*>(xcache));
-  else
-    launch_k(k_stage_remote_rows<16, 4>, dim3(blocks), dim3(256), 0, s, t, local_mask, nodes, cum, n_idx, cap_nodes,
-             reinterpret_cast<uint8_t*>(xcache));
 }
 
 }  // namespace glt

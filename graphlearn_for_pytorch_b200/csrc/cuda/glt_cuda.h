@@ -159,11 +159,6 @@ void launch_gather_i64(RowTable t, const int64_t* idx, int64_t n, const int32_t*
 void launch_multimem_copy(const void* src, void* mc_dst, int64_t nbytes, cudaStream_t s);
 // out[i, 0..d) (bf16) = dequantised MXFP8 row idx[i] of `t` (rows of d + 16 bytes, see data/quantize.py)
 void launch_gather_mxfp8(RowTable t, const int64_t* idx, int64_t n, int d, void* out, cudaStream_t s);
-// xcache[s, :] = row nodes[s] of `t` for every local id s < cum[n_idx] whose row is NOT in a part of `local_mask`
-// (peer HBM / host): one bulk, bandwidth-efficient pass over the batch's unique remote rows (each is needed ~2.5x by
-// the layer-1 kernel), run on the sampling stream one batch ahead of the training step.
-void launch_stage_remote_rows(RowTable t, unsigned local_mask, const int64_t* nodes, const int32_t* cum, int n_idx,
-                              int cap_nodes, void* xcache, cudaStream_t s);
 
 // ---- sage.cu (GraphSAGE engine kernels) ---------------------------------------
 struct SageAggArgs {
@@ -236,7 +231,7 @@ void launch_sage_scatter_bwd(const SageScatterArgs& a, cudaStream_t s);
 void launch_add_block_f32(const void* dA, int dA_ld, int col, int d, const int32_t* cum, int n_hops, int cap,
                           float* dH, cudaStream_t s);
 
-// ---- transpose.cu: per-batch transposed adjacency + atomics-free backward (EXPERIMENTAL) ----------
+// ---- transpose.cu: per-batch transposed adjacency + atomics-free backward ----------
 // The forward ELL blocks are keyed by TARGET (row t lists its sampled sources).  The backward of the
 // mean aggregation needs the opposite view (for a source s: all targets that sampled it).  It is
 // built once per batch on the sampling stream as a CSR over local source ids, ordered by hop inside
@@ -297,9 +292,6 @@ void launch_dropout_bf16(void* Z, const int32_t* cum, int n_hops, int cap, int d
 // g[0..n) = 0, *loss = 0, *correct = 0 (one launch at the start of the gradient phase; the *_prezeroed variants of
 // the kernels below then skip their own memsets, which keeps the step a pure kernel chain)
 void launch_zero_grads(float* g, int64_t n, float* loss, int32_t* correct, cudaStream_t s);
-// bias + relu epilogue over valid rows (zero beyond): Z = relu(Z + b)
-void launch_bias_relu(void* Z, const void* bias, const int32_t* cum, int n_hops, int cap, int d,
-                      int relu, cudaStream_t s);
 // loss = mean NLL(log_softmax(logits[:n0, :C]), y); dlogits = (softmax - onehot)/n0
 // labels come from y[r], or (labels_all != nullptr) from labels_all[nodes[r]].
 // colsum (optional, fp32 [ld]): bias gradient = column sums of the bf16 dlogits, any ld (multiple of 8): fused into
@@ -550,21 +542,11 @@ struct SageFusedArgs {
   int relu;
   void* z;                      // bf16 [cap_targets, N]
   void* a_save;                 // optional bf16 [cap_targets, 2d] for backward
-  unsigned long long* trace;    // optional per-CTA clock64 timeline (diagnostics, see sage_fused_trace)
   int feat_fp8;                 // 1: agg.feat rows are MXFP8 (d e4m3 bytes + d/32 UE8M0 scales, 16-byte padded)
-  unsigned local_mask;          // bit p set: part p of agg.feat lives in this GPU's HBM
-  // Staged remote rows: rows of the batch's nodes that live in PEER HBM, copied once per batch (on the sampling
-  // stream, launch_stage_remote_rows) into a local buffer indexed by the node's LOCAL id.  nullptr = read peers in
-  // place.  cache_part: index of a non-local part whose handle slot is reused for the cache.
-  const void* xcache;
-  int cache_part;
 };
-int sage_fused_supported(int d, int n_out);
-// Copies the per-CTA timeline of the last traced launch (GLT_B200_FUSED_TRACE=1) to `host` [132*32]
-// (one row per SM of an H100 SXM; launches with more CTAs are not traced).
-void sage_fused_trace_copy(unsigned long long* host);
-constexpr int kFusedTraceSlots = 32;
-constexpr int kFusedTraceCtas = 132;
+// 1 if the fused kernel takes layer width d -> n_out (its shared memory fits) and, when `feat` is given, can address
+// every row of that feature table with its 32-bit row handles (4-bit part, 28-bit row inside the part).
+int sage_fused_supported(int d, int n_out, const RowTable* feat = nullptr);
 void launch_sage_fused(const SageFusedArgs& a, int num_sms, cudaStream_t s);
 // W [N, K] row-major bf16 -> packed swizzled image used by launch_sage_fused.
 void launch_pack_weight(const void* w, int n, int k, void* packed, cudaStream_t s);
@@ -589,7 +571,7 @@ struct TcGemmArgs {
   TcProblem p[2];
   // {next item, CTAs done}, zero between launches: CTAs claim work items with atomicAdd on [0]; the last CTA to
   // finish zeroes both, so the next launch (or CUDA-graph replay) starts from item 0.  One buffer per plan, and a
-  // plan is never launched concurrently with itself.  nullptr = static striding (item = blockIdx.x + i * gridDim.x).
+  // plan is never launched concurrently with itself.
   int* tickets;
 };
 struct alignas(64) TcGemmLaunch {
@@ -601,23 +583,8 @@ struct alignas(64) TcGemmLaunch {
 // Returns 0 on success (1: driver entry point unavailable, 2: encode failed).
 int make_tmap_bf16_2d(void* out_map, const void* base, int64_t rows, int64_t cols, int64_t ld, int box_cols,
                       int box_rows);
-// uint8 (e4m3) [rows, cols] row-major tensor map with a {box_cols = 128 bytes, box_rows} SWIZZLE_128B box
-int make_tmap_u8_2d(void* out_map, const void* base, int64_t rows, int64_t cols, int64_t ld, int box_cols,
-                    int box_rows);
 size_t tc_gemm_smem_bytes();
 
-// ---- tc_gemm_mx.cu (block-scaled MXFP8 forward GEMM, wgmma e4m3 with per-32-K-group scale promotion) -------------
-struct TcMxArgs {
-  int m, n, k;              // rows of A (capacity), rows of W, contraction length (multiple of 128)
-  int bn;                   // tile width: 128 (divides n)
-  const int32_t* dyn;       // optional device counter for the valid rows of A
-  int dyn_idx;
-  const void* sfa;          // packed UE8M0 scale blocks of A: [ceil(m/128)][k/128][512 B]
-  const void* sfb;          // packed UE8M0 scale blocks of W: [n/128][k/128][512 B]
-  const void* bias;         // bf16 [n] or nullptr
-  int relu;
-};
-void launch_tc_gemm_mx(const void* maps3, const TcMxArgs& a, int num_sms, cudaStream_t s);
 // ---- hetero_infer.cu (full-neighbourhood attention of the heterogeneous engines' layer-wise inference) ----------
 // Both kernels walk the COMPLETE CSR row of every target r in [r0, r1) (global ids of the destination type; rows of the
 // relation graph are targets, columns are global source ids, ids outside [0, n_src) are skipped).  A row is reduced by

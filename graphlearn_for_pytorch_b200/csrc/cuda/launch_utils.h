@@ -1,14 +1,12 @@
 // Host-side launch helper: every engine kernel goes through launch_k(), which sets the programmatic-stream-
-// serialization attribute (PDL, see device_utils.cuh) unless GLT_B200_PDL=0.  Under stream capture consecutive
-// launches become programmatic edges of the CUDA graph.
+// serialization attribute (PDL, see device_utils.cuh) unless set_pdl(0) turned it off.  Under stream capture
+// consecutive launches become programmatic edges of the CUDA graph.
 #pragma once
 #include <cuda_runtime.h>
 
-#include <cstdlib>
-
 namespace glt {
 
-// Process-wide switch (default: GLT_B200_PDL, on).  Read at every launch, so a caller can turn it off around the
+// Process-wide switch (default on, set_pdl).  Read at every launch, so a caller can turn it off around the
 // capture of a CUDA graph: programmatic edges help single-stream chains (hetero engine, the unpipelined step) but can
 // cost when two streams interleave kernels (sample || train), because early-launched dependents hold SM slots that
 // the other stream's kernels could have used.

@@ -8,7 +8,6 @@
 // does gather -> scatter-mean -> two Linear); the aggregation here consumes the
 // feature table *in place* (local or peer HBM) like GatherTensorKernel
 // (csrc/cuda/unified_tensor.cu:47-81) but never materialises x[n_id].
-#include <cstdlib>
 
 #include "device_utils.cuh"
 #include "launch_utils.h"
@@ -196,25 +195,6 @@ __global__ void __launch_bounds__(256) k_relu_bwd_cast(const float* dH, const __
     float v = 0.f;
     for (int t = c >> 3; t < static_cast<int>(blockDim.x); t += groups) v += s_acc[t][c & 7];
     if (v != 0.f) atomicAdd(colsum + c, v);
-  }
-}
-
-__global__ void k_bias_relu(__nv_bfloat16* Z, const __nv_bfloat16* bias, const int32_t* cum,
-                            int n_hops, int cap, int d, int relu) {
-  const int T = min(cum[n_hops], cap);
-  const int64_t n8 = static_cast<int64_t>(T) * d / 8;
-  for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < n8;
-       i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
-    const int64_t e = i * 8;
-    const int col = static_cast<int>(e % d);
-    float z[8], b[8];
-#pragma unroll
-    for (int q = 0; q < 8; ++q) z[q] = b[q] = 0.f;
-    bf16x8_accum(*reinterpret_cast<const uint4*>(Z + e), z);
-    bf16x8_accum(*reinterpret_cast<const uint4*>(bias + col), b);
-#pragma unroll
-    for (int q = 0; q < 8; ++q) { z[q] += b[q]; if (relu) z[q] = fmaxf(z[q], 0.f); }
-    *reinterpret_cast<uint4*>(Z + e) = pack_bf16x8(z, 1.f);
   }
 }
 
@@ -412,10 +392,7 @@ inline int grid_for(int64_t items, int per_block, int max_blocks = 132 * 16) {
 }  // namespace
 
 int& pdl_flag() {
-  static int flag = [] {
-    const char* e = std::getenv("GLT_B200_PDL");
-    return e ? (std::atoi(e) != 0 ? 1 : 0) : 1;
-  }();
+  static int flag = 1;
   return flag;
 }
 
@@ -513,13 +490,6 @@ int launch_relu_bwd_cast(const float* dH, const void* Z, const int32_t* cum, int
   if (colsum == nullptr || fused) return 1;
   launch_colsum_accum(dPre, cum, n_hops, cap, d, colsum, s);
   return 2;
-}
-
-void launch_bias_relu(void* Z, const void* bias, const int32_t* cum, int n_hops, int cap, int d,
-                      int relu, cudaStream_t s) {
-  k_bias_relu<<<grid_for(static_cast<int64_t>(cap) * d / 8, 256), 256, 0, s>>>(
-      reinterpret_cast<__nv_bfloat16*>(Z), reinterpret_cast<const __nv_bfloat16*>(bias), cum, n_hops,
-      cap, d, relu);
 }
 
 int launch_softmax_nll(const void* logits, int ld, int C, const int64_t* y, const int64_t* labels_all,

@@ -13,12 +13,6 @@
 // It replaces, in one launch, the reference's GatherTensorKernel
 // (csrc/cuda/unified_tensor.cu:47-81) + PyG scatter-mean + two cuBLAS GEMMs +
 // bias/ReLU elementwise kernels, and keeps the row count on the device.
-//
-// Roles (640 threads, one persistent CTA per SM):
-//   warps 0-15  producers   (8-lane group per target row, 2 rows per group per tile)
-//   warps 16-19 one warpgroup: weight bulk-load (one lane), wgmma + epilogue
-#include <cstdlib>
-
 #include "launch_utils.h"
 #include "tc_utils.cuh"
 
@@ -30,8 +24,6 @@ using namespace tc;
 
 constexpr int kTileM = 128;
 constexpr int kProducerWarps = 16;
-constexpr int kMmaWarp = 16;
-constexpr int kThreads = 20 * 32;
 constexpr int kChunkBytes = 128;                    // 64 bf16 = one SWIZZLE_128B atom row
 constexpr int kAChunkTile = kTileM * kChunkBytes;   // 16 KB per K-chunk of an A tile
 constexpr int kMmaStageBytes = 16 * 128;            // per-warp epilogue staging: 16 rows x 64 bf16
@@ -114,183 +106,12 @@ __device__ __forceinline__ void wg_mma_half(uint32_t a_u32, uint32_t w_u32, int 
   }
 }
 
-// NC = d / 64 (K chunks of the mean half; the self half has NC more)
-template <int NC>
-__global__ void __launch_bounds__(kThreads, 1) k_sage_fused(SageFusedArgs f) {
-  extern __shared__ uint8_t smem_raw[];
-  // 1024-B alignment required by SWIZZLE_128B
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int N = f.n_out;
-  constexpr int NKC = 2 * NC;                      // K chunks of [mean | self]
-  uint8_t* smem_w = smem;                          // NKC x [N x 128 B]
-  uint8_t* smem_a = smem_w + NKC * N * kChunkBytes;  // NKC x [128 x 128 B]
-  uint8_t* stg = smem_a + NKC * kAChunkTile;         // [4 warps][16 rows][128 B]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(stg + 4 * kMmaStageBytes);
-  const uint32_t bar_w = smem_u32(bars + 0);
-  const uint32_t bar_a_full = smem_u32(bars + 1);
-  const uint32_t bar_a_empty = smem_u32(bars + 2);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const SageAggArgs& a = f.agg;
-  const int T = min(a.cum[a.n_hops_targets], a.cap_targets);
-  const int n_tiles = (T + kTileM - 1) / kTileM;
-
-  if (threadIdx.x == 0) {
-    mbar_init(bar_w, 1);
-    mbar_init(bar_a_full, kProducerWarps);
-    mbar_init(bar_a_empty, 4);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-
-  if (warp < kProducerWarps) {
-    // ------------------------------ producers ------------------------------
-    // 64 eight-lane groups; each owns rows {g, g+64} of the 128-row tile.  The pointer
-    // chase (deg -> ELL -> node id -> owner shard) of both rows is issued up front so
-    // the four dependent-load chains overlap; feature rows then stream in batches of
-    // four neighbours x NC 16-byte vectors per lane.
-    const int gl = lane & 7;
-    const int gw = lane >> 3;
-    const unsigned gmask = 0xFFu << (gw * 8);
-    const int group = warp * 4 + gw;  // 0..63
-    constexpr int RPG = kTileM / (kProducerWarps * 4);  // rows per group per tile (2)
-    int it = 0;
-    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
-      int dg[RPG];
-      const int32_t* ell[RPG];
-      const uint8_t* p_lo[RPG];
-      const uint8_t* p_hi[RPG];
-      const uint8_t* p_self[RPG];
-#pragma unroll
-      for (int q = 0; q < RPG; ++q) {
-        const int t = tile * kTileM + group + q * (kTileM / RPG);
-        dg[q] = 0; ell[q] = nullptr; p_lo[q] = p_hi[q] = p_self[q] = nullptr;
-        if (t < T) {
-          const HopLoc2 l = locate2(a.cum, a.n_hops_targets, t);
-          dg[q] = a.deg[t];
-          ell[q] = a.ell[l.hop] + static_cast<int64_t>(l.row) * a.k[l.hop];
-        }
-      }
-      int s_lo[RPG], s_hi[RPG];
-#pragma unroll
-      for (int q = 0; q < RPG; ++q) {
-        s_lo[q] = (gl < dg[q]) ? ell[q][gl] : -1;
-        s_hi[q] = (gl + 8 < dg[q]) ? ell[q][gl + 8] : -1;
-      }
-#pragma unroll
-      for (int q = 0; q < RPG; ++q) {
-        const int t = tile * kTileM + group + q * (kTileM / RPG);
-        if (s_lo[q] >= 0) p_lo[q] = src_row2(a, s_lo[q]);
-        if (s_hi[q] >= 0) p_hi[q] = src_row2(a, s_hi[q]);
-        if (t < T && gl == 0) p_self[q] = src_row2(a, t);
-        p_self[q] = reinterpret_cast<const uint8_t*>(
-            __shfl_sync(gmask, reinterpret_cast<unsigned long long>(p_self[q]), 0, 8));
-      }
-      bool waited = false;
-#pragma unroll
-      for (int q = 0; q < RPG; ++q) {
-        const int r = group + q * (kTileM / RPG);
-        const int t = tile * kTileM + r;
-        float acc[NC][8];
-#pragma unroll
-        for (int c = 0; c < NC; ++c)
-#pragma unroll
-          for (int i = 0; i < 8; ++i) acc[c][i] = 0.f;
-        for (int j0 = 0; j0 < dg[q]; j0 += 8) {
-          const uint8_t* my_ptr = (j0 == 0) ? p_lo[q] : p_hi[q];
-          if (j0 >= 16) {
-            my_ptr = nullptr;
-            if (j0 + gl < dg[q]) {
-              const int s = ell[q][j0 + gl];
-              if (s >= 0) my_ptr = src_row2(a, s);
-            }
-          }
-          const int cnt = min(8, dg[q] - j0);
-#pragma unroll
-          for (int jb = 0; jb < 8; jb += 4) {
-            uint4 v[4][NC];
-#pragma unroll
-            for (int jj = 0; jj < 4; ++jj) {
-              const uint8_t* p = reinterpret_cast<const uint8_t*>(
-                  __shfl_sync(gmask, reinterpret_cast<unsigned long long>(my_ptr), jb + jj, 8));
-#pragma unroll
-              for (int c = 0; c < NC; ++c)
-                v[jj][c] = (jb + jj < cnt && p) ? ld_nc_v4(p + c * kChunkBytes + gl * 16) : make_uint4(0, 0, 0, 0);
-            }
-#pragma unroll
-            for (int jj = 0; jj < 4; ++jj)
-#pragma unroll
-              for (int c = 0; c < NC; ++c) bf16x8_accum(v[jj][c], acc[c]);
-          }
-        }
-        const float inv = dg[q] > 0 ? 1.f / static_cast<float>(dg[q]) : 0.f;
-        uint4 res_mean[NC], res_self[NC];
-#pragma unroll
-        for (int c = 0; c < NC; ++c) {
-          res_mean[c] = pack_bf16x8(acc[c], inv);
-          res_self[c] = p_self[q] ? ld_nc_v4(p_self[q] + c * kChunkBytes + gl * 16) : make_uint4(0, 0, 0, 0);
-        }
-        if (t < T && f.a_save) {
-          uint8_t* o = reinterpret_cast<uint8_t*>(f.a_save) + static_cast<int64_t>(t) * a.d * 4;
-#pragma unroll
-          for (int c = 0; c < NC; ++c) {
-            *reinterpret_cast<uint4*>(o + c * kChunkBytes + gl * 16) = res_mean[c];
-            *reinterpret_cast<uint4*>(o + a.d * 2 + c * kChunkBytes + gl * 16) = res_self[c];
-          }
-        }
-        // the single A buffer is free once the previous tile's MMAs have retired
-        if (!waited) { mbar_wait(bar_a_empty, (it & 1) ^ 1); waited = true; }
-        const uint32_t off = r * kChunkBytes + ((gl ^ (r & 7)) << 4);
-#pragma unroll
-        for (int c = 0; c < NC; ++c) {
-          *reinterpret_cast<uint4*>(smem_a + c * kAChunkTile + off) = res_mean[c];
-          *reinterpret_cast<uint4*>(smem_a + (NC + c) * kAChunkTile + off) = res_self[c];
-        }
-      }
-      fence_proxy_async();  // generic-proxy writes -> visible to the tensor-core (async) proxy
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_a_full);
-    }
-  } else {
-    // ------------------------------ MMA + epilogue warpgroup ------------------------------
-    if (static_cast<int>(blockIdx.x) < n_tiles) {
-      if (threadIdx.x == kMmaWarp * 32) {
-        const uint32_t w_bytes = NKC * N * kChunkBytes;
-        mbar_expect_tx(bar_w, w_bytes);
-        // one TMA bulk copy per K chunk (each <= 32 KB)
-        for (int kc = 0; kc < NKC; ++kc)
-          bulk_g2s(smem_u32(smem_w + kc * N * kChunkBytes),
-                   reinterpret_cast<const uint8_t*>(f.w_packed) + static_cast<size_t>(kc) * N * kChunkBytes,
-                   N * kChunkBytes, bar_w);
-      }
-      mbar_wait(bar_w, 0);
-    }
-    const uint32_t stg_u32 = smem_u32(stg) + (warp - kMmaWarp) * kMmaStageBytes;
-    int it = 0;
-    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
-      mbar_wait(bar_a_full, it & 1);
-      const __nv_bfloat16* bias = reinterpret_cast<const __nv_bfloat16*>(f.bias);
-      uint8_t* z = reinterpret_cast<uint8_t*>(f.z);
-      wg_mma_half<NKC>(smem_u32(smem_a), smem_u32(smem_w), N, bias, f.relu, 0, stg_u32, z, tile * kTileM, T, [] {});
-      wg_mma_half<NKC>(smem_u32(smem_a), smem_u32(smem_w), N, bias, f.relu, 1, stg_u32, z, tile * kTileM, T, [&] {
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar_a_empty);   // A buffer reusable
-      });
-    }
-  }
-}
-
-// ---------------------------------------------------------------------------------------------
-// v3: decoupled address resolution.
-//
-// Profiles of v2 showed the producers spending about
-// half of every tile in the dependent pointer chase (deg/ELL -> node id -> owner shard) with no
-// feature bytes in flight.  v3 gives the chase to four dedicated RESOLVER warps (one thread per
-// tile row) that run one tile AHEAD of the loaders and publish, per row, 15 neighbour row pointers
-// + the self-row pointer + the degree into a double-buffered shared-memory table.  The 16 LOADER
-// warps then do nothing but stream 16-byte feature vectors (6 rows in flight per lane: the self
-// row rides in slot 0 of the first batch and goes straight to the A tile) and reduce them.
+// Decoupled address resolution.  A producer that chases its own pointers (deg/ELL -> node id -> owner shard)
+// spends about half of every tile in that dependent chain with no feature bytes in flight.  The chase therefore
+// belongs to four dedicated RESOLVER warps (one thread per tile row) that run one tile AHEAD of the loaders and
+// publish, per row, 15 neighbour row pointers + the self-row pointer + the degree into a double-buffered
+// shared-memory table.  The 16 LOADER warps then do nothing but stream 16-byte feature vectors (6 rows in flight
+// per lane: the self row rides in slot 0 of the first batch and goes straight to the A tile) and reduce them.
 // Resolver warp 0 also issues the weight bulk copy.  The tile's GEMM + epilogue is split over two warpgroups:
 // the last one takes rows 0-63, the resolvers take rows 64-127 once they have published the next tile's table,
 // which halves the time the A buffer stays locked.  The CTA stays at 24 warps (80 registers per thread).
@@ -298,13 +119,6 @@ __global__ void __launch_bounds__(kThreads, 1) k_sage_fused(SageFusedArgs f) {
 //   warps 0-15  loaders   (8-lane group per target row, 2 rows per group per tile)
 //   warps 16-19 resolvers (warp 16, lane 0: TMA weight load) + wgmma / epilogue of tile rows 64-127
 //   warps 20-23 wgmma / epilogue of tile rows 0-63
-__device__ unsigned long long g_fused_trace[kFusedTraceCtas * kFusedTraceSlots];
-__device__ __forceinline__ void trace_at(unsigned long long* tr, int slot) {
-  if (tr && slot < kFusedTraceSlots) tr[slot] = static_cast<unsigned long long>(clock64());
-}
-// timeline slots: 0 start, 1 end, 2 #tiles, then per tile i < 4 at 4 + 7 i:
-//   +0 table published  +1 loaders start  +2 first row done  +3 tile loaded  +4 MMA start
-//   +5 A released (last MMA done)   +6 tile stored
 constexpr int kResolverWarps = 4;
 constexpr int kThreads3 = (kProducerWarps + kResolverWarps + 4) * 32;
 constexpr int kKP = 15;                      // neighbour handles published per row (+1 self)
@@ -347,8 +161,6 @@ __global__ void __launch_bounds__(kThreads3, 1) k_sage_fused3(SageFusedArgs f) {
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  unsigned long long* tr = f.trace ? f.trace + blockIdx.x * kFusedTraceSlots : nullptr;
-  if (threadIdx.x == 0) trace_at(tr, 0);
   const SageAggArgs& a = f.agg;
   const int64_t row_bytes = FP8 ? static_cast<int64_t>(a.feat.row_bytes) : static_cast<int64_t>(a.d) * 2;
   // Tile order.  Low tile indices hold the early hops (largest fan-out = most neighbour rows per
@@ -379,8 +191,6 @@ __global__ void __launch_bounds__(kThreads3, 1) k_sage_fused3(SageFusedArgs f) {
       b = reinterpret_cast<const uint8_t*>(a.src_local) +
           static_cast<int64_t>(threadIdx.x) * (int64_t(1) << 28) * row_bytes;
     else if (static_cast<int>(threadIdx.x) < a.feat.num_parts) b = a.feat.base[threadIdx.x];
-    // staged remote rows (see SageFusedArgs::xcache): the slot of one (never referenced) remote part points at the cache
-    if (f.xcache && static_cast<int>(threadIdx.x) == f.cache_part) b = f.xcache;
     sts64(base_u32 + threadIdx.x * 8, reinterpret_cast<uint64_t>(b));
   }
   // programmatic dependent launch: barrier init and shard base table above overlap with the tail
@@ -409,7 +219,6 @@ __global__ void __launch_bounds__(kThreads3, 1) k_sage_fused3(SageFusedArgs f) {
     for (int tile = tile_of(0); tile < n_tiles; tile = tile_of(++it)) {
       const int stage = it & 1;
       mbar_wait(bar_p_full0 + 8 * stage, (it >> 1) & 1);
-      if (threadIdx.x == 0) trace_at(tr, 4 + 7 * it + 1);
       const uint32_t tb = tab_u32 + stage * kTabStageBytes;
       const uint32_t dgt = deg_u32 + stage * (kTileM * 4);
       bool waited = false;
@@ -494,7 +303,6 @@ __global__ void __launch_bounds__(kThreads3, 1) k_sage_fused3(SageFusedArgs f) {
             *reinterpret_cast<uint4*>(save) = m0;
             *reinterpret_cast<uint4*>(save + 16) = m1;
           }
-          if (threadIdx.x == 0 && q == 0) trace_at(tr, 4 + 7 * it + 2);
         }
       } else {
 #pragma unroll 1
@@ -573,11 +381,9 @@ __global__ void __launch_bounds__(kThreads3, 1) k_sage_fused3(SageFusedArgs f) {
           sts128(a_u32 + c * kAChunkTile + off, m);
           if (save) *reinterpret_cast<uint4*>(save + c * kChunkBytes) = m;
         }
-        if (threadIdx.x == 0 && q == 0) trace_at(tr, 4 + 7 * it + 2);
       }
       }  // !FP8
       __syncwarp();
-      if (threadIdx.x == 0) trace_at(tr, 4 + 7 * it + 3);
       if (lane == 0) mbar_arrive(bar_p_empty0 + 8 * stage);  // table stage may be refilled
       fence_proxy_async();  // generic-proxy writes -> visible to the tensor-core (async) proxy
       __syncwarp();
@@ -595,17 +401,13 @@ __global__ void __launch_bounds__(kThreads3, 1) k_sage_fused3(SageFusedArgs f) {
                  reinterpret_cast<const uint8_t*>(f.w_packed) + static_cast<size_t>(kc) * N * kChunkBytes,
                  N * kChunkBytes, bar_w);
     }
-    // global row id (+ the node's local id in the batch) -> (shard, row in shard); with a staged remote-row cache
-    // every row that is not in this GPU's HBM is read from the cache at its local id instead of from the peer
-    auto handle_of = [&](int64_t gid, int local_id) -> uint32_t {
+    // global row id -> (shard, row in shard)
+    auto handle_of = [&](int64_t gid) -> uint32_t {
       if (gid < 0) return kNoRow;
 #pragma unroll 1
       for (int p = 0; p < a.feat.num_parts; ++p)
-        if (gid >= a.feat.row_begin[p] && gid < a.feat.row_begin[p + 1]) {
-          if (f.xcache && !((f.local_mask >> p) & 1u))
-            return (static_cast<uint32_t>(f.cache_part) << 28) | static_cast<uint32_t>(local_id);
+        if (gid >= a.feat.row_begin[p] && gid < a.feat.row_begin[p + 1])
           return (static_cast<uint32_t>(p) << 28) | static_cast<uint32_t>(gid - a.feat.row_begin[p]);
-        }
       return kNoRow;
     };
     auto resolve = [&](int tile, int stage) {
@@ -636,8 +438,8 @@ __global__ void __launch_bounds__(kThreads3, 1) k_sage_fused3(SageFusedArgs f) {
         for (int j = 0; j < kKP; ++j) gid[j] = (j < dg && sidx[j] >= 0) ? __ldg(a.nodes + sidx[j]) : -1;
         uint32_t hnd[kKP + 1];
 #pragma unroll
-        for (int j = 0; j < kKP; ++j) hnd[j] = handle_of(gid[j], sidx[j]);
-        hnd[kKP] = handle_of(self_gid, t);
+        for (int j = 0; j < kKP; ++j) hnd[j] = handle_of(gid[j]);
+        hnd[kKP] = handle_of(self_gid);
 #pragma unroll
         for (int j = 0; j < kKP; ++j) sts32(trow + ((j ^ sw) << 2), static_cast<int32_t>(hnd[j]));
         sts32(trow + ((15 ^ sw) << 2), static_cast<int32_t>(hnd[kKP]));
@@ -649,7 +451,6 @@ __global__ void __launch_bounds__(kThreads3, 1) k_sage_fused3(SageFusedArgs f) {
     if (tile < n_tiles) {
       resolve(tile, 0);
       __syncwarp();
-      if (w_thread) trace_at(tr, 4 + 0);
       if (lane == 0) mbar_arrive(bar_p_full0);
     }
     for (; tile < n_tiles; tile = tile_of(++it)) {
@@ -660,7 +461,6 @@ __global__ void __launch_bounds__(kThreads3, 1) k_sage_fused3(SageFusedArgs f) {
         mbar_wait(bar_p_empty0 + 8 * ns, (nu & 1) ^ 1);
         resolve(next, ns);
         __syncwarp();
-        if (w_thread) trace_at(tr, 4 + 7 * (it + 1) + 0);
         if (lane == 0) mbar_arrive(bar_p_full0 + 8 * ns);
       }
       if (it == 0) mbar_wait(bar_w, 0);
@@ -675,28 +475,16 @@ __global__ void __launch_bounds__(kThreads3, 1) k_sage_fused3(SageFusedArgs f) {
   } else {
     // ------------------------------ MMA + epilogue warpgroup ------------------------------
     const uint32_t stg_u32 = smem_u32(stg) + (warp - kEpiWarp0) * kStageWarpBytes;
-    const bool tracer = (warp == kEpiWarp0 && lane == 0);
     int it = 0;
     for (int tile = tile_of(0); tile < n_tiles; tile = tile_of(++it)) {
       if (it == 0) mbar_wait(bar_w, 0);
       mbar_wait(bar_a_full, it & 1);
-      if (tracer) trace_at(tr, 4 + 7 * it + 4);
       wg_mma_half<NKC>(a_u32, smem_u32(smem_w), N, reinterpret_cast<const __nv_bfloat16*>(bias_s), f.relu, 0, stg_u32,
                        reinterpret_cast<uint8_t*>(f.z), tile * kTileM, T, [&] {
                          __syncwarp();
-                         if (tracer) trace_at(tr, 4 + 7 * it + 5);
                          if (lane == 0) mbar_arrive(bar_a_empty);   // A buffer reusable
                        });
-      if (tracer) trace_at(tr, 4 + 7 * it + 6);
     }
-  }
-
-  __syncthreads();
-  if (threadIdx.x == 0 && tr) {
-    trace_at(tr, 1);
-    int cnt = 0;
-    while (tile_of(cnt) < n_tiles) ++cnt;
-    tr[2] = cnt;
   }
 }
 
@@ -715,12 +503,6 @@ __global__ void k_pack_weight(const __nv_bfloat16* w, int n, int k, __nv_bfloat1
   }
 }
 
-size_t fused_smem_bytes(int d, int n_out) {
-  const int nkc = 2 * (d / 64);
-  return static_cast<size_t>(nkc) * n_out * kChunkBytes + static_cast<size_t>(nkc) * kAChunkTile +
-         4 * kMmaStageBytes + 128 + 1024;
-}
-
 size_t fused3_smem_bytes(int d, int n_out) {
   const int nkc = 2 * (d / 64);
   return static_cast<size_t>(nkc) * n_out * kChunkBytes + static_cast<size_t>(nkc) * kAChunkTile +
@@ -729,78 +511,33 @@ size_t fused3_smem_bytes(int d, int n_out) {
 
 constexpr size_t kMaxSmem = 227 * 1024;
 
-// 3 = decoupled resolver/loader kernel, 2 = the earlier monolithic-producer kernel
-int fused_version(int d, int n_out) {
-  return fused3_smem_bytes(d, n_out) <= kMaxSmem ? 3 : 2;
-}
-
-// v3 publishes 32-bit row handles (4-bit shard, 28-bit row inside the shard)
-bool handles_fit(const SageAggArgs& a) {
-  if (a.src_local) return true;
-  if (a.feat.num_parts > 16) return false;
-  for (int p = 0; p < a.feat.num_parts; ++p)
-    if (a.feat.row_begin[p + 1] - a.feat.row_begin[p] >= (int64_t(1) << 28)) return false;
-  return true;
+template <int NC, bool FP8>
+void launch_fused3(const SageFusedArgs& a, int grid, cudaStream_t s) {
+  const size_t smem = fused3_smem_bytes(a.agg.d, a.n_out);
+  cudaFuncSetAttribute(k_sage_fused3<NC, FP8>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+  launch_k(k_sage_fused3<NC, FP8>, dim3(grid), dim3(kThreads3), smem, s, a);
 }
 
 }  // namespace
 
-int sage_fused_supported(int d, int n_out) {
+int sage_fused_supported(int d, int n_out, const RowTable* feat) {
   if (d != 64 && d != 128) return 0;
   if (n_out % 32 != 0 || n_out < 32 || n_out > 256) return 0;
-  return fused_smem_bytes(d, n_out) <= kMaxSmem ? 1 : 0;
-}
-
-template <int NC>
-static void launch_fused_nc(const SageFusedArgs& a_in, int grid, cudaStream_t s) {
-  SageFusedArgs a = a_in;
-  static const bool trace_on = [] {
-    const char* e = std::getenv("GLT_B200_FUSED_TRACE");
-    return e && std::atoi(e) != 0;
-  }();
-  a.trace = nullptr;
-  if (trace_on && grid <= kFusedTraceCtas) {
-    // resolved per device on its first (eager) launch, i.e. outside any stream capture
-    static unsigned long long* sym[64] = {};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev >= 0 && dev < 64) {
-      if (sym[dev] == nullptr) {
-        void* p = nullptr;
-        if (cudaGetSymbolAddress(&p, g_fused_trace) == cudaSuccess) sym[dev] = reinterpret_cast<unsigned long long*>(p);
-      }
-      a.trace = sym[dev];
-    }
+  if (fused3_smem_bytes(d, n_out) > kMaxSmem) return 0;
+  if (feat != nullptr) {  // row handles: 4-bit part, 28-bit row inside the part
+    if (feat->num_parts > 16) return 0;
+    for (int p = 0; p < feat->num_parts; ++p)
+      if (feat->row_begin[p + 1] - feat->row_begin[p] >= (int64_t(1) << 28)) return 0;
   }
-  if (a.feat_fp8) {
-    // MXFP8 feature rows: only the decoupled (v3) kernel has the de-quantising loader, d = 128
-    if constexpr (NC == 2) {
-      const size_t smem = fused3_smem_bytes(a.agg.d, a.n_out);
-      cudaFuncSetAttribute(k_sage_fused3<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
-      launch_k(k_sage_fused3<2, true>, dim3(grid), dim3(kThreads3), smem, s, a);
-    }
-    return;
-  }
-  if (fused_version(a.agg.d, a.n_out) == 3 && handles_fit(a.agg)) {
-    const size_t smem = fused3_smem_bytes(a.agg.d, a.n_out);
-    cudaFuncSetAttribute(k_sage_fused3<NC, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
-    launch_k(k_sage_fused3<NC, false>, dim3(grid), dim3(kThreads3), smem, s, a);
-  } else {
-    const size_t smem = fused_smem_bytes(a.agg.d, a.n_out);
-    cudaFuncSetAttribute(k_sage_fused<NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
-    k_sage_fused<NC><<<grid, kThreads, smem, s>>>(a);
-  }
-}
-
-void sage_fused_trace_copy(unsigned long long* host) {
-  cudaMemcpyFromSymbol(host, g_fused_trace, sizeof(unsigned long long) * kFusedTraceCtas * kFusedTraceSlots);
+  return 1;
 }
 
 void launch_sage_fused(const SageFusedArgs& a, int num_sms, cudaStream_t s) {
   const int max_tiles = (a.agg.cap_targets + kTileM - 1) / kTileM;
   const int grid = max_tiles < num_sms ? max_tiles : num_sms;
-  if (a.agg.d == 64) launch_fused_nc<1>(a, grid, s);
-  else launch_fused_nc<2>(a, grid, s);
+  if (a.feat_fp8) launch_fused3<2, true>(a, grid, s);  // the MXFP8 loader is written for d = 128
+  else if (a.agg.d == 64) launch_fused3<1, false>(a, grid, s);
+  else launch_fused3<2, false>(a, grid, s);
 }
 
 void launch_pack_weight(const void* w, int n, int k, void* packed, cudaStream_t s) {

@@ -156,8 +156,8 @@ k_tc_gemm(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
     // ------------------------------ TMA producer ------------------------------
     if (threadIdx.x == 0) {
       int fill = 0;   // k-blocks produced so far (ring position)
-      for (int item = blockIdx.x;; item += gridDim.x) {
-        if (g.tickets) item = atomicAdd(g.tickets, 1);
+      for (;;) {
+        const int item = atomicAdd(g.tickets, 1);
         if (item >= total_items) break;
         const Item it = decode(item, d0, d1);
         const TcProblem& p = g.p[it.prob];
@@ -192,13 +192,11 @@ k_tc_gemm(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUte
       mbar_wait(bar_empty0 + 8 * s, ((fill / kStages) & 1) ^ 1);
       item_slot[s] = -1;
       mbar_arrive(bar_full0 + 8 * s);
-      if (g.tickets) {
-        // every CTA has made its last claim once all have counted themselves out: the last one resets the ticket
-        __threadfence();
-        if (atomicAdd(g.tickets + 1, 1) == static_cast<int>(gridDim.x) - 1) {
-          g.tickets[0] = 0;
-          g.tickets[1] = 0;
-        }
+      // every CTA has made its last claim once all have counted themselves out: the last one resets the ticket
+      __threadfence();
+      if (atomicAdd(g.tickets + 1, 1) == static_cast<int>(gridDim.x) - 1) {
+        g.tickets[0] = 0;
+        g.tickets[1] = 0;
       }
     }
   } else {
@@ -349,21 +347,6 @@ int make_tmap_bf16_2d(void* out_map, const void* base, int64_t rows, int64_t col
   cuuint32_t box[2] = {static_cast<cuuint32_t>(box_cols), static_cast<cuuint32_t>(box_rows)};
   cuuint32_t estr[2] = {1, 1};
   const CUresult r = fn(reinterpret_cast<CUtensorMap*>(out_map), CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2,
-                        const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                        CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? 0 : 2;
-}
-
-int make_tmap_u8_2d(void* out_map, const void* base, int64_t rows, int64_t cols, int64_t ld, int box_cols,
-                    int box_rows) {
-  EncodeTiledFn fn = encode_fn();
-  if (!fn) return 1;
-  cuuint64_t dims[2] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows)};
-  cuuint64_t strides[1] = {static_cast<cuuint64_t>(ld)};
-  cuuint32_t box[2] = {static_cast<cuuint32_t>(box_cols), static_cast<cuuint32_t>(box_rows)};
-  cuuint32_t estr[2] = {1, 1};
-  const CUresult r = fn(reinterpret_cast<CUtensorMap*>(out_map), CU_TENSOR_MAP_DATA_TYPE_UINT8, 2,
                         const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);

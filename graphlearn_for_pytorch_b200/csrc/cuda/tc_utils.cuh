@@ -1,5 +1,5 @@
 // wgmma / TMA / mbarrier PTX wrappers shared by the sm_90a tensor-core kernels
-// (sage_tc.cu: fused gather+aggregate+GEMM; tc_gemm.cu / tc_gemm_mx.cu: TMA-fed dense GEMMs of the engine).
+// (sage_tc.cu: fused gather+aggregate+GEMM; tc_gemm.cu: TMA-fed dense GEMMs of the engine).
 #pragma once
 #include "device_utils.cuh"
 
@@ -88,19 +88,6 @@ __device__ __forceinline__ void wgmma_m64n32k16_bf16(float (&d)[32], uint64_t da
       "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n"
       "}\n"
       : GLT_ACC16(d, 0)
-      : "l"(da), "l"(db), "r"(accumulate));
-}
-// D[64 x 64] (+)= A[64 x 32] . B[64 x 32]^T, e4m3 in (K-major), fp32 accumulate
-__device__ __forceinline__ void wgmma_m64n64k32_e4m3(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %34, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n64k32.f32.e4m3.e4m3 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1;\n"
-      "}\n"
-      : GLT_ACC16(d, 0), GLT_ACC16(d, 16)
       : "l"(da), "l"(db), "r"(accumulate));
 }
 #undef GLT_ACC16

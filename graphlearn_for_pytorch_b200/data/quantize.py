@@ -43,23 +43,3 @@ def dequantize_mxfp8(rows: torch.Tensor, d: int) -> torch.Tensor:
   e = rows[:, d:d + d // BLOCK].float() - 127.0
   return (q * torch.exp2(e).unsqueeze(2)).view(n, d)
 
-
-def quantize_mxfp8_parts(x: torch.Tensor):
-  """[N, d] -> (e4m3 bytes uint8 [N, d], UE8M0 scale bytes uint8 [N, d / 32]): the operands of a block-scaled
-  wgmma GEMM (`TcGemmMx`); the scale bytes still have to be packed with `pack_mx_scale_blocks`."""
-  rows = quantize_mxfp8(x)
-  d = x.shape[1]
-  return rows[:, :d].contiguous(), rows[:, d:d + d // BLOCK].contiguous()
-
-
-def pack_mx_scale_blocks(sf: torch.Tensor) -> torch.Tensor:
-  """UE8M0 scale bytes [rows, K / 32] -> the tensor core's block layout: uint8 [ceil(rows/128), K/128, 512], where
-  byte (r % 32) * 16 + (r // 32) * 4 + k of block (mb, kb) is the scale of row mb * 128 + r, K-group kb * 4 + k
-  (CUTLASS Sm1xxBlockScaledBasicChunk; rows are padded with the neutral scale 2^0)."""
-  rows, g = sf.shape
-  assert g % 4 == 0, 'K must be a multiple of 128'
-  mb, kb = (rows + 127) // 128, g // 4
-  pad = torch.full((mb * 128, g), 127, dtype=torch.uint8, device=sf.device)
-  pad[:rows] = sf
-  v = pad.view(mb, 4, 32, kb, 4)                 # [mb, r // 32, r % 32, kb, k]
-  return v.permute(0, 3, 2, 1, 4).contiguous().view(mb, kb, 512)

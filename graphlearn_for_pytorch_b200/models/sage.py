@@ -105,7 +105,7 @@ class GraphSageEngine(object):
     preaggregate_layer1: pipelined engines whose layer 1 runs unfused aggregate layer 1 of the next batch on the
       sampling stream, right after sampling it (the aggregation depends on the batch and the feature table only, not
       on the weights), so the training chain starts with the layer-1 GEMM.  Each arena then has its own layer-1 A
-      buffer.  None = on where it applies, unless GLT_B200_PREAGG=0; False = aggregate inside the forward as usual.
+      buffer.  None = on where it applies; False = aggregate inside the forward as usual.
   """
   # read by bench.py: the backward of the aggregation is always the atomics-free gather (csrc/cuda/transpose.cu)
   use_gather_bwd = True
@@ -120,7 +120,7 @@ class GraphSageEngine(object):
                calibration_margin: float = 1.3, calibration_batches: int = 16, pipeline: bool = False,
                use_peer_allreduce: bool = True,
                check_every: int = 64, auto_regrow: bool = True, feature_format: str = 'bf16',
-               deterministic_sampling: bool = False, stage_remote_rows: Optional[bool] = None,
+               deterministic_sampling: bool = False,
                dropout: float = 0.0, preaggregate_layer1: Optional[bool] = None):
     self.nat = require_native()
     # dropout on the hidden activations (the reference example trains with p = 0.5,
@@ -136,18 +136,9 @@ class GraphSageEngine(object):
       assert int(in_dim) == 128, 'MXFP8 features: in_dim must be 128'
       use_fused = True
     self.pipeline = bool(pipeline)
-    # Multi-GPU: the rows of a batch's nodes that live in PEER HBM are copied once per batch into a local buffer
-    # indexed by local node id -- by a bulk gather kernel on the SAMPLING stream, one batch ahead of the training
-    # step -- and the fused layer-1 kernel reads them from there (each is needed ~2.5x, and 256-byte random reads
-    # issued from inside the GEMM kernel are bound by NVLink latency, not bandwidth).  True = stage when the feature
-    # table has non-local parts; None/False = in-kernel peer loads (the default, see _build_buffers).
-    self._stage_remote_opt = stage_remote_rows
     self.deterministic_sampling = bool(deterministic_sampling)
     self.use_peer_allreduce = bool(use_peer_allreduce)
-    if preaggregate_layer1 is None:
-      import os as _os5
-      preaggregate_layer1 = _os5.environ.get('GLT_B200_PREAGG', '1') != '0'
-    self._preagg_opt = bool(preaggregate_layer1)
+    self._preagg_opt = preaggregate_layer1 is None or bool(preaggregate_layer1)
     self.preaggregate = False         # resolved once the layer-1 variant is known (_resolve_preagg)
     self._tc_plans = {}
     self.peer_group = None
@@ -201,16 +192,17 @@ class GraphSageEngine(object):
       self._health_dev = torch.zeros(2, dtype=torch.int32, device=dev)
       self._health_host = torch.zeros(2, dtype=torch.int32).pin_memory()
       self._autotune_fused = (use_fused == 'auto')
-      self.fused_ok = [False] + [bool(use_fused and self.nat.sage_fused_supported(self.dims_in[l - 1],
-                                                                                    self.dims_out[l - 1]))
-                                 for l in range(1, self.L + 1)]
+      # layer 1 also needs a feature table that the fused kernel's 32-bit row handles can address
+      self.fused_ok = [False] + [bool(use_fused and self.nat.sage_fused_supported(
+          self.dims_in[l - 1], self.dims_out[l - 1], self.feat if l == 1 else None)) for l in range(1, self.L + 1)]
       bf = torch.bfloat16
       self.w_packed = [None] + [torch.zeros(self.dims_out[l - 1] * 2 * self.dims_in[l - 1], dtype=bf, device=dev)
                                 if self.fused_ok[l] else None for l in range(1, self.L + 1)]
       self._repack()
       self._resolve_preagg()
       if self.feature_format == 'mxfp8' and not self.fused_ok[1]:
-        raise RuntimeError('MXFP8 features need the fused layer-1 kernel (in_dim 128, hidden multiple of 32, <= 256)')
+        raise RuntimeError('MXFP8 features need the fused layer-1 kernel (in_dim 128, hidden multiple of 32, <= 256, '
+                           'at most 16 feature parts of fewer than 2^28 rows each)')
     self._graph_fb = None
     self._graph_opt = None
     self._graph_full = None
@@ -237,7 +229,7 @@ class GraphSageEngine(object):
       dims_in = [self.in_dim] + [self.hidden] * (self.L - 1)
       for l in range(1, self.L):          # hidden layers (the last layer's output is padded to 64 columns)
         fused = use_fused != 'auto' and bool(use_fused) and \
-            bool(self.nat.sage_fused_supported(dims_in[l - 1], self.hidden))
+            bool(self.nat.sage_fused_supported(dims_in[l - 1], self.hidden, self.feat if l == 1 else None))
         if not fused:
           raise ValueError(f'hidden = {self.hidden}: layer {l} runs the unfused forward GEMM, whose output width must '
                            f'be a multiple of 64')
@@ -276,18 +268,6 @@ class GraphSageEngine(object):
                           for l in range(1, self.L + 1)]
     self.dA = [None, None] + [torch.zeros(self.cap_T[l], 2 * self.dims_in[l - 1], dtype=bf, device=dev)
                               for l in range(2, self.L + 1)]
-    want = self._stage_remote_opt
-    if want is None:
-      import os as _os4
-      # the staging kernel competes with the sampler for the side stream, and the unfused layer 1 already hides the
-      # NVLink latency behind its occupancy -> opt-in
-      want = _os4.environ.get('GLT_B200_STAGE_REMOTE', '0') != '0'
-    has_remote = hasattr(self.feat, 'all_local') and not self.feat.all_local()
-    self.stage_remote = bool(want and has_remote)
-    self._xcache = None
-    if self.stage_remote:
-      row_bytes = self.in_dim * 2 if self.feature_format == 'bf16' else self.in_dim + 16
-      self._xcache = [torch.zeros(int(a_.cap_nodes), row_bytes, dtype=torch.uint8, device=dev) for a_ in self._arenas]
     self._tc_plans = {}
     self._graphs = []
     self._graph_fb = self._graph_opt = self._graph_full = None
@@ -508,9 +488,6 @@ class GraphSageEngine(object):
     # (the increment itself is folded into the first sampling kernel: step_inc)
     ar.sample(self.gh, self._seeds[which], None, self.seed, 0, False, False, True, len(self._arenas))
     self._k(2 + 2 * self.L)  # table clear + init_seeds + (sample, relabel) per hop
-    if self.stage_remote:
-      self.feat.stage_remote_rows(ar.nodes, ar.counters, self.L + 1, self._xcache[which])
-      self._k(1)
     if self.preaggregate:
       self._aggregate_layer1(which)
 
@@ -545,9 +522,8 @@ class GraphSageEngine(object):
     nodes = ar.nodes if l == 1 else None
     src_local = None if l == 1 else self.Z[l - 1]
     if self.fused_ok[l]:
-      xc = self._xcache[self._cur] if (l == 1 and self.stage_remote) else None
       nat.sage_fused(feat, nodes, src_local, d, ar.counters, nh, ell, ks, ar.deg, self.w_packed[l],
-                     self.b(l), relu, self.Z[l], self.A[l], xc)
+                     self.b(l), relu, self.Z[l], self.A[l])
       self._k(1)
     else:
       if not (l == 1 and self.preaggregate):     # pre-aggregated: _sample already wrote A1 of this arena
@@ -715,7 +691,7 @@ class GraphSageEngine(object):
         return
       # programmatic dependent launch helps single-stream chains and costs ~2 % when the sampling and training
       # streams interleave (measured, csrc/cuda/launch_utils.h): captured without it in pipelined mode
-      prev_pdl = self.nat.set_pdl(not self.pipeline) if hasattr(self.nat, 'set_pdl') else None
+      prev_pdl = self.nat.set_pdl(not self.pipeline)
       # capturing NCCL collectives works but makes process-group teardown hang on this stack
       # (measured: bench exit blocked until the timeout), so it is opt-in for world > 1
       single = self.world == 1 or self.peer_group is not None or \
@@ -739,8 +715,7 @@ class GraphSageEngine(object):
             self._optimizer()
         self._graphs.append((g, None if single else g_opt))
       torch.cuda.synchronize()
-      if prev_pdl is not None:
-        self.nat.set_pdl(prev_pdl)
+      self.nat.set_pdl(prev_pdl)
       self.load_state_dict(saved)
       self._cur, self._primed = 0, False
       self._graph_fb = self._graphs[0][0]
@@ -852,7 +827,7 @@ class GraphSageEngine(object):
 
       def __getattr__(self, name):
         f = getattr(self._o, name)
-        if name in ('TcGemm', 'TcGemmMx'):
+        if name == 'TcGemm':
           return lambda *a, **k: _Timed(f(*a, **k), name + '.')
         if not callable(f) or name.startswith('_') or isinstance(f, type) or name in ('set_pdl',):
           return f
@@ -885,8 +860,6 @@ class GraphSageEngine(object):
         ar.sample(self.gh, self._seeds[0], None, self.seed, 0, False, False, True, len(self._arenas))
         e1.record()
         log.append(('arena.sample (all sampling kernels)', e0, e1))
-        if self.stage_remote:
-          self.feat.stage_remote_rows(ar.nodes, ar.counters, self.L + 1, self._xcache[0])
         if self.preaggregate:
           # a pipelined step runs it on the sampling stream, outside the training chain
           self._aggregate_layer1(0)

@@ -129,12 +129,7 @@ def main():
     assert torch.allclose(e.Z[1][:T].float(), Z_ref, atol=8e-2, rtol=3e-2), f'fused layer output mismatch ({what})'
     ok(f'fused layer-1 numerics, {what}')
 
-  assert not eng.stage_remote, 'in-kernel peer loads are the default'
   check_fused(eng, 'peer rows read in place over NVLink from inside the fused wgmma kernel')
-  eng_st = GraphSageEngine(pg.graph, pf2.table, labels, in_dim=128, num_nodes=N, fanouts=[4, 3], batch_size=256,
-                           hidden=256, num_classes=8, device=dev, use_cuda_graph=False, stage_remote_rows=True)
-  assert eng_st.stage_remote
-  check_fused(eng_st, 'remote rows staged into the local cache on the sampling stream')
   # parameters stay identical across ranks (all-reduced gradients)
   p = eng.p32.clone()
   dist.all_reduce(p, op=dist.ReduceOp.MAX)

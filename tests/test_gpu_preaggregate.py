@@ -234,29 +234,6 @@ def test_ticket_resets_across_graph_replays(native):
     assert torch.equal(first[0], Z) and torch.equal(first[1], dA), rep
 
 
-def test_ticketed_and_static_claiming_agree_bitwise(native, monkeypatch):
-  T, K, N = 30000, 512, 256
-  A = _rand((T, K), seed=4)
-  W = _rand((N, K), 0.05, seed=5)
-  b = _rand((N,), seed=6)
-  dPre = _rand((T, N), 0.1, seed=7)
-  Wd = _rand((N, K), 0.05, seed=8)
-  c = _counters(2, T - 77)
-  outs = []
-  for tickets in ('1', '0'):
-    monkeypatch.setenv('GLT_B200_GEMM_TICKETS', tickets)
-    Z = torch.zeros(T, N, dtype=torch.bfloat16, device=DEV)
-    dA = torch.zeros(T, K, dtype=torch.bfloat16, device=DEV)
-    f = native.TcGemm(0)
-    f.add_forward(A, W, b, True, Z, c, 2)
-    d = native.TcGemm(0)
-    d.add_dgrad(dPre, Wd, dA, c, 2)
-    f.run(); d.run(); f.run()
-    torch.cuda.synchronize()
-    outs.append((Z, dA))
-  assert torch.equal(outs[0][0], outs[1][0]) and torch.equal(outs[0][1], outs[1][1])
-
-
 def test_gemm_with_late_starting_ctas_matches_fp32(native):
   """Sleeping kernels on other streams hold SM slots while a GEMM with more items than CTAs starts: whichever CTAs
   start late, the items they did not claim are done by the others and the result is complete."""

@@ -116,7 +116,7 @@ def test_hgt_trains_on_hetero_batches():
 
 
 def test_transposed_gather_backward_equals_scatter_backward():
-  """Algorithm behind csrc/cuda/transpose.cu (EXPERIMENTAL kernels): the backward of the ELL mean aggregation
+  """Algorithm behind csrc/cuda/transpose.cu: the backward of the ELL mean aggregation
   computed as an atomics-free GATHER over a transposed adjacency (sources -> targets, hop-ordered segments)
   equals the scatter formulation the engine uses today, for every layer's hop prefix."""
   torch.manual_seed(0)
