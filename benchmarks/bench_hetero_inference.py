@@ -86,7 +86,7 @@ def torch_rsage(eng, csr, feats, n):
         dst, src, deg = csr[r]
         blocks.append(torch.zeros(n[t], X[eng.nt[r]].shape[1], device=dst.device)
                       .index_add_(0, dst, X[eng.nt[r]][src].float()) / deg)
-      z = bf16_mm(torch.cat(blocks + [X[t].float()], 1), eng.W(l, t), eng.b(l, t))
+      z = bf16_mm(torch.cat(blocks + [X[t].float()], 1), eng.param(('W', l, t)), eng.param(('b', l, t)))
       Z[t] = (F.relu(z) if l < eng.L else z).to(torch.bfloat16)
     X = Z
   return X[eng.tid[eng.seed_type]][:, :eng.C]

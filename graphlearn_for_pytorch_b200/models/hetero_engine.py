@@ -49,6 +49,8 @@ class HeteroSageEngine(object):
 
   Widths outside these limits raise ValueError at construction.
     fanouts: [k per hop] (all relations) or {etype: [k per hop]}.
+
+  Parameters are named ('W', l, t) and ('b', l, t) per layer and destination type; `param(name, grad=False)`.
   """
 
   def __init__(self, graphs: Dict[EdgeType, object], feature_tables: Dict[str, object], labels: torch.Tensor,
@@ -140,20 +142,50 @@ class HeteroSageEngine(object):
     self.kernels_per_step = 0
 
   # ------------------------------------------------------------------ buffers / parameters
-  def _cap_T(self, l: int, t: int) -> int:
-    return int(min(self.cap_nodes[t], sum(self.cap_rows[t][:self.L - l + 1])))
+  def _rows(self, l: int, t: int) -> int:
+    """Rows of type t's layer-l buffers (l = 0: the input layer, every sampled node)."""
+    return max(int(min(self.cap_nodes[t], sum(self.cap_rows[t][:self.L - l + 1]))), 128)
 
   def _width_in(self, l: int, t: int) -> int:
     return self.dim_in[self.ntypes[t]] if l == 1 else self.hidden
 
+  def _zeros(self, *shape, dt=torch.bfloat16) -> torch.Tensor:
+    return torch.zeros(*shape, dtype=dt, device=self.device)
+
+  @staticmethod
+  def _check_heads(heads: int, hidden: int) -> int:
+    """The attention engines' head count, which must split hidden into head widths that are multiples of 8."""
+    heads = int(heads)
+    if heads < 1 or int(hidden) % heads != 0 or (int(hidden) // heads) % 8 != 0:
+      raise ValueError(f'heads must divide hidden into head widths that are multiples of 8 (hidden {hidden}, '
+                       f'heads {heads})')
+    return heads
+
+  def _check_attention_schema(self):
+    """The attention engines take in_dim multiples of 64 in [64, 1024] and need an incoming relation into every
+    destination type at every layer."""
+    for t, d in self.dim_in.items():
+      if d % 64 != 0 or not 64 <= d <= 1024:
+        raise ValueError(f'in_dim of node type {t!r} must be a multiple of 64 in [64, 1024] (got {d})')
+    for l in range(1, self.L + 1):
+      for t in self.targets[l]:
+        if not self.in_rel[l][t]:
+          raise ValueError(f'node type {self.ntypes[t]!r} has no incoming relation at layer {l}')
+
+  def _alloc_head(self):
+    """Output and gradient of the attention engines' Linear head on the seed type."""
+    rows = self._rows(self.L, self.tid[self.seed_type])
+    self.logits = self._zeros(rows, self.n_out_pad)
+    self.dlogits = self._zeros(rows, self.n_out_pad)
+
   def _alloc(self):
-    dev, bf, f32 = self.device, torch.bfloat16, torch.float32
+    z, f32 = self._zeros, torch.float32
     self.A, self.Z, self.dPre, self.dA, self.dH, self.col = [None], [None], [None], [None], [None], [None]
     for l in range(1, self.L + 1):
       n_out = self.hidden if l < self.L else self.n_out_pad
       A, Z, dP, dA, dH, col = {}, {}, {}, {}, {}, {}
       for t in self.targets[l]:
-        cap = max(self._cap_T(l, t), 128)
+        cap = self._rows(l, t)
         offs, c = [], 0
         for r in self.in_rel[l][t]:
           offs.append(c)
@@ -163,37 +195,50 @@ class HeteroSageEngine(object):
         if K % 64 != 0:                          # weight-gradient GEMM: N = K
           raise ValueError(f'layer {l} operand of node type {self.ntypes[t]!r} is {K} columns wide (the widths of its '
                            f'incoming relations\' source types plus its own); it must be a multiple of 64')
-        A[t] = torch.zeros(cap, K, dtype=bf, device=dev)
-        Z[t] = torch.zeros(cap, n_out, dtype=bf, device=dev)
-        dP[t] = torch.zeros(cap, n_out, dtype=bf, device=dev)
+        A[t] = z(cap, K)
+        Z[t] = z(cap, n_out)
+        dP[t] = z(cap, n_out)
         if l > 1:
-          dA[t] = torch.zeros(cap, K, dtype=bf, device=dev)
+          dA[t] = z(cap, K)
         if l < self.L:
-          dH[t] = torch.zeros(cap, n_out, dtype=f32, device=dev)   # gradient wrt Z[l][t], filled by layer l+1
+          dH[t] = z(cap, n_out, dt=f32)         # gradient wrt Z[l][t], filled by layer l+1
       self.A.append(A); self.Z.append(Z); self.dPre.append(dP); self.dA.append(dA); self.dH.append(dH)
       self.col.append(col)
 
-  def _init_params(self):
-    dev = self.device
-    self._w_off, self._b_off, sizes = {}, {}, 0
+  def _param_layout(self):
+    """(name, shape) of every parameter in layout and initialisation order: ('W', l, t) [n_out, K] and ('b', l, t)
+    [n_out] per layer and destination type."""
     for l in range(1, self.L + 1):
       for t in self.targets[l]:
-        n, k = self.Z[l][t].shape[1], self.A[l][t].shape[1]
-        self._w_off[(l, t)] = (sizes, n, k); sizes += n * k
-        self._b_off[(l, t)] = (sizes, n); sizes += n
-    self.p32 = torch.zeros(sizes, dtype=torch.float32, device=dev)
+        yield ('W', l, t), (self.Z[l][t].shape[1], self.A[l][t].shape[1])
+        yield ('b', l, t), (self.Z[l][t].shape[1],)
+
+  def _param_init(self, name, shape, g: torch.Generator) -> torch.Tensor:
+    """Initial fp32 value of a parameter (weights drawn from g; zero biases and zero padding class rows)."""
+    kind, l, t = name
+    if kind == 'b':
+      return torch.zeros(shape)
+    w = (torch.rand(*shape, generator=g) * 2 - 1) / math.sqrt(max(shape[1] // (len(self.in_rel[l][t]) + 1), 1))
+    if l == self.L:
+      w[self.C:] = 0
+    return w
+
+  def _init_params(self):
+    """Flat fp32 parameters `p32`, laid out by `_param_layout()`: `param_index[name] = (offset, shape)`, every
+    parameter starting at a multiple of 8 floats (16-byte aligned bf16 shadow).  Checkpoints, the peer all-reduce and
+    Adam rely on this layout.  Initial values are drawn in layout order from one generator seeded with `seed`.  Then the
+    bf16 shadow, gradient and Adam buffers (and the peer group when world > 1)."""
+    dev = self.device
+    self.param_index, off = {}, 0
+    for name, shape in self._param_layout():
+      off = _round_up(off, 8)
+      self.param_index[name] = (off, shape)
+      off += math.prod(shape)
+    self.p32 = torch.zeros(_round_up(off, 8), dtype=torch.float32, device=dev)
     g = torch.Generator(device='cpu')
     g.manual_seed(self.seed)
-    for (l, t), (off, n, k) in self._w_off.items():
-      w = (torch.rand(n, k, generator=g) * 2 - 1) / math.sqrt(max(k // (len(self.in_rel[l][t]) + 1), 1))
-      if l == self.L and self.n_out_pad > self.C:
-        w[self.C:] = 0
-      self.p32[off:off + n * k].copy_(w.flatten())
-    self._init_optimizer_state()
-
-  def _init_optimizer_state(self):
-    """bf16 shadow, gradient and Adam buffers of the flat fp32 parameters `p32` (and the peer group when world > 1)."""
-    dev = self.device
+    for name, (o, shape) in self.param_index.items():
+      self.p32[o:o + math.prod(shape)].copy_(self._param_init(name, shape, g).flatten())
     pad = (-self.p32.numel()) % 4
     self.p16 = self.p32.to(torch.bfloat16)
     self.g32 = torch.zeros_like(self.p32)
@@ -211,13 +256,24 @@ class HeteroSageEngine(object):
     self.m = torch.zeros_like(self.p32)
     self.v = torch.zeros_like(self.p32)
 
-  def W(self, l, t):
-    off, n, k = self._w_off[(l, t)]
-    return self.p16[off:off + n * k].view(n, k)
+  def param(self, name, grad: bool = False) -> torch.Tensor:
+    """bf16 view of a parameter (grad=True: its fp32 gradient slot)."""
+    o, shape = self.param_index[name]
+    buf = self.g32 if grad else self.p16
+    return buf[o:o + math.prod(shape)].view(*shape)
 
-  def b(self, l, t):
-    off, n = self._b_off[(l, t)]
-    return self.p16[off:off + n]
+  def _p32(self, name, grad: bool = False) -> torch.Tensor:
+    o, shape = self.param_index[name]
+    return (self.g32 if grad else self.p32)[o:o + math.prod(shape)]
+
+  def _rel_params(self, kind, l: int, t: int, grad: bool = False) -> torch.Tensor:
+    """Flat bf16 view (grad=True: fp32 gradient) of the parameters (kind, l, r) of the relations r into (l, t), which
+    the layout places back to back."""
+    rels = self.in_rel[l][t]
+    o, shape = self.param_index[(kind, l, rels[0])]
+    n = math.prod(shape)
+    assert all(self.param_index[(kind, l, r)][0] == o + i * n for i, r in enumerate(rels))
+    return (self.g32 if grad else self.p16)[o:o + n * len(rels)]
 
   def state_dict(self):
     return {'p32': self.p32.clone(), 'm': self.m.clone(), 'v': self.v.clone(), 'step': int(self.step_dev[0].item()),
@@ -250,15 +306,50 @@ class HeteroSageEngine(object):
     if pl is None:
       nh = self.L - l + 1
       pl = self.nat.TcGemm(self.device.index)
+      W = self.param(('W', l, t))
       if kind == 'fwd':
-        pl.add_forward(self.A[l][t], self.W(l, t), self.b(l, t), l < self.L, self.Z[l][t], self._ctr[t], nh)
+        pl.add_forward(self.A[l][t], W, self.param(('b', l, t)), l < self.L, self.Z[l][t], self._ctr[t], nh)
       else:
-        off, n, k = self._w_off[(l, t)]
-        pl.add_wgrad(self.dPre[l][t], self.A[l][t], self.g32[off:off + n * k].view(n, k), self._ctr[t], nh)
+        pl.add_wgrad(self.dPre[l][t], self.A[l][t], self.param(('W', l, t), True), self._ctr[t], nh)
         if l > 1:
-          pl.add_dgrad(self.dPre[l][t], self.W(l, t), self.dA[l][t], self._ctr[t], nh)
+          pl.add_dgrad(self.dPre[l][t], W, self.dA[l][t], self._ctr[t], nh)
       self._plans[key] = pl
     return pl
+
+  def _head_plan(self, dZ: Optional[torch.Tensor] = None):
+    """TcGemm of the Linear head of the attention engines over the seed type's batch rows: the forward into `logits`,
+    or (dZ given) the weight gradient and the dgrad into dZ."""
+    key = ('head', dZ is None)
+    pl = self._plans.get(key)
+    if pl is None:
+      st = self.tid[self.seed_type]
+      Z, c = self.Z[self.L][st], self._ctr[st]
+      pl = self.nat.TcGemm(self.device.index)
+      if dZ is None:
+        pl.add_forward(Z, self.param(('head_W',)), self.param(('head_b',)), False, self.logits, c, 1)
+      else:
+        pl.add_wgrad(self.dlogits, Z, self.param(('head_W',), True), c, 1)
+        pl.add_dgrad(self.dlogits, self.param(('head_W',)), dZ, c, 1)
+      self._plans[key] = pl
+    return pl
+
+  def _gather_input(self, u: int):
+    """Layer-1 input of the attention engines: the feature rows of every sampled node of type u into X0[u]."""
+    n = min(self.X0[u].shape[0], self.cap_nodes[u])
+    self.feat[self.ntypes[u]].gather_into(self.arena.nodes_of(u)[:n], None, self._ctr[u][self.L + 1:self.L + 2],
+                                          self.X0[u][:n])
+    self._k()
+
+  def _loss(self, logits: torch.Tensor, dlogits: torch.Tensor, bias_grad: torch.Tensor):
+    """Forward tail: clear the gradients, then the fused log-softmax / NLL of the seed rows of `logits`, writing
+    `dlogits` and the last layer's bias gradient."""
+    nat, st = self.nat, self.tid[self.seed_type]
+    if self.peer_group is not None:
+      self.peer_group.barrier(1)            # peers finished reading last step's gradients
+      self._k()
+    nat.zero_grads(self.g32, self.loss, self.correct)
+    self._k(1 + nat.softmax_nll(logits, self.C, None, self.labels, self.arena.nodes_of(st), self._ctr[st], self.loss,
+                                dlogits, self.correct, bias_grad, True))
 
   def _forward(self):
     nat, ar = self.nat, self.arena
@@ -289,13 +380,7 @@ class HeteroSageEngine(object):
         self._plan('fwd', l, t).run()
         self._k()
     st = self.tid[self.seed_type]
-    if self.peer_group is not None:
-      self.peer_group.barrier(1)            # peers finished reading last step's gradients
-      self._k()
-    nat.zero_grads(self.g32, self.loss, self.correct)
-    boff, n = self._b_off[(self.L, st)]
-    self._k(1 + nat.softmax_nll(self.Z[self.L][st], self.C, None, self.labels, ar.nodes_of(st), self._ctr[st],
-                                self.loss, self.dPre[self.L][st], self.correct, self.g32[boff:boff + n], True))
+    self._loss(self.Z[self.L][st], self.dPre[self.L][st], self.param(('b', self.L, st), True))
 
   def _backward(self):
     nat, ar = self.nat, self.arena
@@ -320,9 +405,8 @@ class HeteroSageEngine(object):
         nat.add_block_f32(self.dA[l][t], self_col, H, self._ctr[t], nh, self.dH[l - 1][t])
         self._k()
       for s in self.targets[l - 1]:
-        boff, n = self._b_off[(l - 1, s)]
         self._k(nat.relu_bwd_cast(self.dH[l - 1][s], self.Z[l - 1][s], self._ctr[s], nh + 1, self.dPre[l - 1][s],
-                                  self.g32[boff:boff + n], True))
+                                  self.param(('b', l - 1, s), True), True))
 
   def _optimizer(self):
     if self.peer_group is not None:
@@ -423,7 +507,7 @@ class HeteroSageEngine(object):
       self._ids = torch.arange(max(self._n_nodes), dtype=torch.int64, device=dev)
       X = self._infer_input(chunk_rows)
       for l in range(1, L + 1):
-        Z = {t: torch.empty(self._n_nodes[t], self._infer_width(l), dtype=torch.bfloat16, device=dev)
+        Z = {t: torch.empty(self._n_nodes[t], self.Z[l][t].shape[1], dtype=torch.bfloat16, device=dev)
              for t in self.targets[l]}
         self._infer_layer(l, X, Z, chunk_rows)
         X = Z
@@ -442,15 +526,19 @@ class HeteroSageEngine(object):
     """Bytes per chunk row of the call's chunk buffers (sizes the default chunk)."""
     return 2 * max(A.shape[1] for l in range(1, self.L + 1) for A in self.A[l].values())
 
-  def _infer_width(self, l: int) -> int:
-    return self.hidden if l < self.L else self.n_out_pad
-
   def _infer_input(self, chunk_rows: int):
     """Input tables of layer 1 (None: layer 1 reads the feature tables)."""
     return None
 
   def _infer_head(self, X: torch.Tensor) -> torch.Tensor:
+    """Logits from the last layer's output (R-SAGE: the last layer is the classifier)."""
     return X
+
+  def _infer_linear_head(self, X: torch.Tensor) -> torch.Tensor:
+    """The attention engines' `_infer_head`: their Linear head over every seed-type node."""
+    out = torch.empty(X.shape[0], self.n_out_pad, dtype=torch.bfloat16, device=self.device)
+    self._gemm(X, self.param(('head_W',)), self.param(('head_b',)), False, out, 1 + self.tid[self.seed_type])
+    return out
 
   def _gather_chunk(self, t: int, r0: int, r1: int, buf: torch.Tensor) -> torch.Tensor:
     """bf16 feature rows [r0, r1) of type t, gathered from its feature table (any memory tier) into buf."""
@@ -491,7 +579,7 @@ class HeteroSageEngine(object):
           self.feat[self.ntypes[t]].gather_into(self._ids[r0:r1], None, None, blk)
         else:
           blk.copy_(X[t][r0:r1])
-        self._gemm(a, self.W(l, t), self.b(l, t), l < self.L, Z[t][r0:r1], 0)
+        self._gemm(a, self.param(('W', l, t)), self.param(('b', l, t)), l < self.L, Z[t][r0:r1], 0)
 
   def overflow_count(self) -> int:
     return int(self.arena.counters[self._ovf_idx].item())

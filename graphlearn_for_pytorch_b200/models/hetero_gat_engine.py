@@ -50,36 +50,24 @@ class HeteroGatEngine(HeteroSageEngine):
                hidden: int = 512, num_classes: int = 19, heads: int = 4, dropout: float = 0.2, edge_dir: str = 'in',
                lr: float = 1e-3, weight_decay: float = 0.0, seed: int = 0, device: Optional[torch.device] = None,
                use_cuda_graph: bool = True, cap_limit: int = 1 << 21, group=None):
-    self.heads = int(heads)
+    self.heads = self._check_heads(heads, hidden)
     self.dropout = float(dropout)
-    if self.heads < 1 or int(hidden) % self.heads != 0 or (int(hidden) // self.heads) % 8 != 0:
-      raise ValueError(f'heads must divide hidden into head widths that are multiples of 8 (hidden {hidden}, '
-                       f'heads {heads})')
     if not 0.0 <= self.dropout < 1.0:
       raise ValueError(f'dropout must be in [0, 1) (got {dropout})')
     self._training = True
-    super().__init__(graphs, feature_tables, labels, in_dim, num_nodes, seed_type, fanouts, batch_size, hidden,
-                     num_classes, edge_dir, lr, weight_decay, seed, device, use_cuda_graph, cap_limit, group)
+    super().__init__(graphs, feature_tables, labels, in_dim, num_nodes, seed_type, fanouts=fanouts,
+                     batch_size=batch_size, hidden=hidden, num_classes=num_classes, edge_dir=edge_dir, lr=lr,
+                     weight_decay=weight_decay, seed=seed, device=device, use_cuda_graph=use_cuda_graph,
+                     cap_limit=cap_limit, group=group)
 
   # ------------------------------------------------------------------ buffers / parameters
-  def _rows(self, l: int, t: int) -> int:
-    """Rows of type t's layer-l output buffer (l = 0: the gathered input features of every sampled node)."""
-    return max(self._cap_T(l, t), 128)
-
   def _X(self, l: int, t: int) -> torch.Tensor:
     return self.X0[t] if l == 0 else self.Z[l][t]
 
   def _alloc(self):
-    dev, bf, f32 = self.device, torch.bfloat16, torch.float32
+    self._check_attention_schema()
+    z, f32 = self._zeros, torch.float32
     H, nhd = self.hidden, self.heads
-    for t, d in self.dim_in.items():
-      if d % 64 != 0 or not 64 <= d <= 1024:
-        raise ValueError(f'in_dim of node type {t!r} must be a multiple of 64 in [64, 1024] (got {d})')
-    for l in range(1, self.L + 1):
-      for t in self.targets[l]:
-        if not self.in_rel[l][t]:
-          raise ValueError(f'node type {self.ntypes[t]!r} has no incoming relation at layer {l}')
-    z = lambda *s, dt=bf: torch.zeros(*s, dtype=dt, device=dev)   # noqa: E731
     self.X0 = {t: z(self._rows(0, t), self.dim_in[self.ntypes[t]]) for t in self.targets[1]}
     self.Z, self.G, self.dH = [None], [None], [None]
     for l in range(1, self.L + 1):
@@ -123,70 +111,43 @@ class HeteroGatEngine(HeteroSageEngine):
     for l in range(2, self.L + 1):
       for t in self.targets[l - 1]:
         self.dX[t] = z(max(self._rows(l - 1, t), self.dX[t].shape[0] if t in self.dX else 0), H)
-    st = self.tid[self.seed_type]
-    self.logits = z(self._rows(self.L, st), self.n_out_pad)
-    self.dlogits = z(self._rows(self.L, st), self.n_out_pad)
+    self._alloc_head()
 
-  def _init_params(self):
-    """Flat fp32 parameter layout; `param_index[name] = (offset, shape)` with names ('W_src', l, r), ('W_dst', l, r)
-    (only when the two ends have different widths), ('att_src', l, r), ('att_dst', l, r), ('bias', l, r), ('head_W',),
-    ('head_b',).  The biases of the relations into one (layer, type) are contiguous."""
-    H, nhd = self.hidden, self.heads
-    idx, off = {}, 0
-
-    def put(name, *shape):
-      nonlocal off
-      idx[name] = (off, shape)
-      off += math.prod(shape)
-    self._bias_block = {}
+  def _param_layout(self):
+    """Names ('W_src', l, r), ('W_dst', l, r) (only when the two ends have different widths), ('att_src', l, r),
+    ('att_dst', l, r), ('bias', l, r), ('head_W',), ('head_b',).  The biases of the relations into one (layer, type)
+    are contiguous."""
+    H = self.hidden
     for l in range(1, self.L + 1):
       for t in self.targets[l]:
         for r in self.in_rel[l][t]:
           ds = self._width_in(l, self.nt[r])
           dt = self._width_in(l, t)
-          put(('W_src', l, r), H, ds)
+          yield ('W_src', l, r), (H, ds)
           if ds != dt:
-            put(('W_dst', l, r), H, dt)
-          put(('att_src', l, r), H)
-          put(('att_dst', l, r), H)
-        self._bias_block[(l, t)] = (off, len(self.in_rel[l][t]))
+            yield ('W_dst', l, r), (H, dt)
+          yield ('att_src', l, r), (H,)
+          yield ('att_dst', l, r), (H,)
         for r in self.in_rel[l][t]:
-          put(('bias', l, r), H)
-    put(('head_W',), self.n_out_pad, H)
-    put(('head_b',), self.n_out_pad)
-    self.param_index = idx
-    self.p32 = torch.zeros(off, dtype=torch.float32, device=self.device)
-    g = torch.Generator(device='cpu')
-    g.manual_seed(self.seed)
-    C = H // nhd
-    for name, (o, shape) in idx.items():
-      n = math.prod(shape)
-      kind = name[0]
-      if kind in ('W_src', 'W_dst'):
-        a = math.sqrt(6.0 / (shape[0] + shape[1]))                    # glorot on [H, d]
-        v = (torch.rand(*shape, generator=g) * 2 - 1) * a
-      elif kind in ('att_src', 'att_dst'):
-        v = (torch.rand(n, generator=g) * 2 - 1) * math.sqrt(6.0 / (nhd + C))   # glorot on [1, heads, C]
-      elif kind == 'bias':
-        v = torch.zeros(n)
-      else:                                                             # torch.nn.Linear(H, classes) defaults
-        v = (torch.rand(*shape, generator=g) * 2 - 1) / math.sqrt(H)
-        v[self.C:] = 0
-      self.p32[o:o + n].copy_(v.flatten())
-    self._init_optimizer_state()
+          yield ('bias', l, r), (H,)
+    yield ('head_W',), (self.n_out_pad, H)
+    yield ('head_b',), (self.n_out_pad,)
 
-  def param(self, name, grad: bool = False) -> torch.Tensor:
-    """bf16 view of a parameter (grad=True: its fp32 gradient slot)."""
-    o, shape = self.param_index[name]
-    buf = self.g32 if grad else self.p16
-    return buf[o:o + math.prod(shape)].view(*shape)
+  def _param_init(self, name, shape, g: torch.Generator) -> torch.Tensor:
+    H, nhd = self.hidden, self.heads
+    kind = name[0]
+    if kind in ('W_src', 'W_dst'):
+      return (torch.rand(*shape, generator=g) * 2 - 1) * math.sqrt(6.0 / (shape[0] + shape[1]))   # glorot on [H, d]
+    if kind in ('att_src', 'att_dst'):
+      return (torch.rand(*shape, generator=g) * 2 - 1) * math.sqrt(6.0 / (nhd + H // nhd))   # glorot on [1, heads, C]
+    if kind == 'bias':
+      return torch.zeros(shape)
+    v = (torch.rand(*shape, generator=g) * 2 - 1) / math.sqrt(H)       # torch.nn.Linear(H, classes) defaults
+    v[self.C:] = 0
+    return v
 
   def _w_dst(self, l, r, grad=False):
     return self.param(('W_dst', l, r) if ('W_dst', l, r) in self.param_index else ('W_src', l, r), grad)
-
-  def _bias(self, l, t, grad=False):
-    o, n = self._bias_block[(l, t)]
-    return (self.g32 if grad else self.p16)[o:o + n * self.hidden]
 
   # ------------------------------------------------------------------ step pieces
   def _views(self, l, r):
@@ -194,38 +155,29 @@ class HeteroGatEngine(HeteroSageEngine):
     s, t = self.nt[r], self.kt[r]
     return self._rows(l - 1, s), self._rows(l, t), self.Ps[(l, r)], self.Pd[(l, r)]
 
-  def _gat_plan(self, kind: str, l: int = 0, r: int = 0):
+  def _gat_plan(self, kind: str, l: int, r: int):
     key = ('gat', kind, l, r)
     pl = self._plans.get(key)
     if pl is not None:
       return pl
     pl = self.nat.TcGemm(self.device.index)
-    st = self.tid[self.seed_type]
-    if kind.startswith('head'):
-      Zl, cs = self.Z[self.L][st], self._ctr[st]
-      if kind == 'head_fwd':
-        pl.add_forward(Zl, self.param(('head_W',)), self.param(('head_b',)), False, self.logits, cs, 1)
-      else:
-        pl.add_wgrad(self.dlogits, Zl, self.param(('head_W',), True), cs, 1)
-        pl.add_dgrad(self.dlogits, self.param(('head_W',)), self.G[self.L][st], cs, 1)
+    nh = self.L - l + 1
+    s, t = self.nt[r], self.kt[r]
+    ns, ntr, Ps, Pd = self._views(l, r)
+    Xs, Xt = self._X(l - 1, s), self._X(l - 1, t)[:ntr]
+    cs, ct = self._ctr[s], self._ctr[t]
+    if kind == 'proj':
+      pl.add_forward(Xs, self.param(('W_src', l, r)), None, False, Ps, cs, nh + 1)
+      if Pd is not None:
+        pl.add_forward(Xt, self._w_dst(l, r), None, False, Pd, ct, nh)
+    elif kind == 'wgrad':      # a shared weight receives both contributions in the same fp32 slice
+      pl.add_wgrad(self.dPs[r][:ns], Xs, self.param(('W_src', l, r), True), cs, nh + 1)
+      if Pd is not None:
+        pl.add_wgrad(self.dPd[r][:ntr], Xt, self._w_dst(l, r, True), ct, nh)
     else:
-      nh = self.L - l + 1
-      s, t = self.nt[r], self.kt[r]
-      ns, ntr, Ps, Pd = self._views(l, r)
-      Xs, Xt = self._X(l - 1, s), self._X(l - 1, t)[:ntr]
-      cs, ct = self._ctr[s], self._ctr[t]
-      if kind == 'proj':
-        pl.add_forward(Xs, self.param(('W_src', l, r)), None, False, Ps, cs, nh + 1)
-        if Pd is not None:
-          pl.add_forward(Xt, self._w_dst(l, r), None, False, Pd, ct, nh)
-      elif kind == 'wgrad':      # a shared weight receives both contributions in the same fp32 slice
-        pl.add_wgrad(self.dPs[r][:ns], Xs, self.param(('W_src', l, r), True), cs, nh + 1)
-        if Pd is not None:
-          pl.add_wgrad(self.dPd[r][:ntr], Xt, self._w_dst(l, r, True), ct, nh)
-      else:
-        pl.add_dgrad(self.dPs[r][:ns], self.param(('W_src', l, r)), self.dX[s][:ns], cs, nh + 1)
-        if Pd is not None:
-          pl.add_dgrad(self.dPd[r][:ntr], self._w_dst(l, r), self.dX[t][:ntr], ct, nh)
+      pl.add_dgrad(self.dPs[r][:ns], self.param(('W_src', l, r)), self.dX[s][:ns], cs, nh + 1)
+      if Pd is not None:
+        pl.add_dgrad(self.dPd[r][:ntr], self._w_dst(l, r), self.dX[t][:ntr], ct, nh)
     self._plans[key] = pl
     return pl
 
@@ -233,10 +185,7 @@ class HeteroGatEngine(HeteroSageEngine):
     nat, ar, hd = self.nat, self.arena, self.heads
     p = self.dropout if self._training else 0.0
     for t in self.targets[1]:
-      n = min(self.X0[t].shape[0], self.cap_nodes[t])
-      self.feat[self.ntypes[t]].gather_into(ar.nodes_of(t)[:n], None, self._ctr[t][self.L + 1:self.L + 2],
-                                            self.X0[t][:n])
-      self._k()
+      self._gather_input(t)
     for l in range(1, self.L + 1):
       nh = self.L - l + 1
       for t in self.targets[l]:
@@ -254,26 +203,20 @@ class HeteroGatEngine(HeteroSageEngine):
           last = j == len(rels) - 1
           nat.gat_aggregate(Ps, self.as_[r][:ns], self.ad_[r][:ntr], hd, self._ctr[t], nh, ell, ks, ar.deg_of(r),
                             self.alpha[(l, r)], acc=self.acc[t][:ntr] if len(rels) > 1 else None, first=j == 0,
-                            last=last, bias=self._bias(l, t) if last else None, act=l < self.L,
+                            last=last, bias=self._rel_params('bias', l, t) if last else None, act=l < self.L,
                             p=p if l < self.L else 0.0, seed=self.seed, layer=l, step_dev=self.step_dev,
                             Z=self.Z[l][t] if last else None)
           self._k()
-    st = self.tid[self.seed_type]
-    self._gat_plan('head_fwd').run()
+    self._head_plan().run()
     self._k()
-    if self.peer_group is not None:
-      self.peer_group.barrier(1)            # peers finished reading last step's gradients
-      self._k()
-    nat.zero_grads(self.g32, self.loss, self.correct)
-    self._k(1 + nat.softmax_nll(self.logits, self.C, None, self.labels, ar.nodes_of(st), self._ctr[st], self.loss,
-                                self.dlogits, self.correct, self.param(('head_b',), True), True))
+    self._loss(self.logits, self.dlogits, self.param(('head_b',), True))
 
   def _backward(self):
     nat, ar, hd, H = self.nat, self.arena, self.heads, self.hidden
     st = self.tid[self.seed_type]
-    self._gat_plan('head_bwd').run()
+    self._head_plan(self.G[self.L][st]).run()
     self._k()
-    nat.gat_act_bwd(None, None, self.G[self.L][st], self._ctr[st], 1, bias_g=self._bias(self.L, st, True))
+    nat.gat_act_bwd(None, None, self.G[self.L][st], self._ctr[st], 1, bias_g=self._rel_params('bias', self.L, st, True))
     self._k()
     for l in range(self.L, 0, -1):
       nh = self.L - l + 1
@@ -308,15 +251,14 @@ class HeteroGatEngine(HeteroSageEngine):
         for u in self.targets[l - 1]:
           nat.gat_act_bwd(self.dH[l - 1][u], self.Z[l - 1][u], self.G[l - 1][u], self._ctr[u], nh + 1,
                           p=self.dropout, seed=self.seed, layer=l - 1, step_dev=self.step_dev,
-                          bias_g=self._bias(l - 1, u, True))
+                          bias_g=self._rel_params('bias', l - 1, u, True))
           self._k()
 
   # ------------------------------------------------------------------ full-neighbourhood inference
   def _infer_chunk_row_bytes(self) -> int:
     return 2 * max(self.dim_in.values()) + 4 * self.hidden
 
-  def _infer_width(self, l: int) -> int:
-    return self.hidden
+  _infer_head = HeteroSageEngine._infer_linear_head
 
   def _infer_project(self, l: int, X, s: int, W: torch.Tensor, buf: torch.Tensor, chunk_rows: int) -> torch.Tensor:
     """bf16 [N_s, H] projection X_s W^T of every node of type s (layer 1: feature chunks gathered into buf first)."""
@@ -353,13 +295,8 @@ class HeteroGatEngine(HeteroSageEngine):
         for j, (r, Ps, as_, ad) in enumerate(ops):
           last = j == len(ops) - 1
           nat.gat_full_aggregate(self._gh(r), Ps, as_, ad, hd, r0, r1, acc=acc[:r1 - r0] if acc is not None else None,
-                                 first=j == 0, last=last, bias=self._bias(l, t) if last else None, act=l < self.L,
-                                 Z=Z[t][r0:r1] if last else None)
-
-  def _infer_head(self, X: torch.Tensor) -> torch.Tensor:
-    out = torch.empty(X.shape[0], self.n_out_pad, dtype=torch.bfloat16, device=self.device)
-    self._gemm(X, self.param(('head_W',)), self.param(('head_b',)), False, out, 1 + self.tid[self.seed_type])
-    return out
+                                 first=j == 0, last=last, bias=self._rel_params('bias', l, t) if last else None,
+                                 act=l < self.L, Z=Z[t][r0:r1] if last else None)
 
   # ------------------------------------------------------------------ public API
   @torch.no_grad()

@@ -37,7 +37,7 @@ from typing import Dict, Optional, Sequence, Union
 
 import torch
 
-from .hetero_engine import HeteroSageEngine, EdgeType, _round_up
+from .hetero_engine import HeteroSageEngine, EdgeType
 
 MAX_RELATIONS = 8      # incoming relations of one destination type that the attention kernels take
 
@@ -57,32 +57,22 @@ class HeteroHgtEngine(HeteroSageEngine):
                hidden: int = 64, num_classes: int = 349, heads: int = 2, edge_dir: str = 'in', lr: float = 1e-2,
                weight_decay: float = 0.0, seed: int = 0, device: Optional[torch.device] = None,
                use_cuda_graph: bool = True, cap_limit: int = 1 << 21, group=None):
-    self.heads = int(heads)
-    if self.heads < 1 or int(hidden) % self.heads != 0 or (int(hidden) // self.heads) % 8 != 0:
-      raise ValueError(f'heads must divide hidden into head widths that are multiples of 8 (hidden {hidden}, '
-                       f'heads {heads})')
-    super().__init__(graphs, feature_tables, labels, in_dim, num_nodes, seed_type, fanouts, batch_size, hidden,
-                     num_classes, edge_dir, lr, weight_decay, seed, device, use_cuda_graph, cap_limit, group)
+    self.heads = self._check_heads(heads, hidden)
+    super().__init__(graphs, feature_tables, labels, in_dim, num_nodes, seed_type, fanouts=fanouts,
+                     batch_size=batch_size, hidden=hidden, num_classes=num_classes, edge_dir=edge_dir, lr=lr,
+                     weight_decay=weight_decay, seed=seed, device=device, use_cuda_graph=use_cuda_graph,
+                     cap_limit=cap_limit, group=group)
 
   # ------------------------------------------------------------------ buffers / parameters
-  def _rows(self, l: int, t: int) -> int:
-    """Rows of type t's layer-l output buffer (l = 0: the input layer, every sampled node)."""
-    return max(self._cap_T(l, t), 128)
-
   def _alloc(self):
-    dev, bf, f32 = self.device, torch.bfloat16, torch.float32
+    self._check_attention_schema()
+    z, f32 = self._zeros, torch.float32
     H, L = self.hidden, self.L
-    for t, d in self.dim_in.items():
-      if d % 64 != 0 or not 64 <= d <= 1024:
-        raise ValueError(f'in_dim of node type {t!r} must be a multiple of 64 in [64, 1024] (got {d})')
     for l in range(1, L + 1):
       for t in self.targets[l]:
-        if not self.in_rel[l][t]:
-          raise ValueError(f'node type {self.ntypes[t]!r} has no incoming relation at layer {l}')
         if len(self.in_rel[l][t]) > MAX_RELATIONS:
           raise ValueError(f'node type {self.ntypes[t]!r} has {len(self.in_rel[l][t])} incoming relations at layer '
                            f'{l}; the attention kernels take at most {MAX_RELATIONS}')
-    z = lambda *s, dt=bf: torch.zeros(*s, dtype=dt, device=dev)   # noqa: E731
     # types whose K/Q/V layer l computes (message sources and destinations), and the input layer's types
     self.srcs = [None] + [sorted({self.nt[r] for t in self.targets[l] for r in self.in_rel[l][t]})
                           for l in range(1, L + 1)]
@@ -106,10 +96,8 @@ class HeteroHgtEngine(HeteroSageEngine):
         R = len(self.in_rel[l][t])
         self.att_img[(l, t)] = z(R * H, H)
         self.msg_img[(l, t)] = z(H, R * H)
-    st = self.tid[self.seed_type]
-    self.logits = z(self._rows(L, st), self.n_out_pad)
-    self.dlogits = z(self._rows(L, st), self.n_out_pad)
-    self.dZL = z(self._rows(L, st), H)                       # head dgrad: gradient of the last layer's output
+    self._alloc_head()
+    self.dZL = z(self._rows(L, self.tid[self.seed_type]), H)   # head dgrad: gradient of the last layer's output
     # alpha per (layer, relation, hop) and the backward's per-relation scratch (two floats per alpha entry)
     self.alpha, self.dal = {}, {}
     for l in range(1, L + 1):
@@ -139,77 +127,48 @@ class HeteroHgtEngine(HeteroSageEngine):
     self.dKQV = {u: z(n, 3 * H) for u, n in u_rows.items()}
     self.dX = {u: z(n, H) for u, n in u_rows.items()}
 
-  def _init_params(self):
-    """Flat fp32 parameter layout; `param_index[name] = (offset, shape)` with names ('in_W', t), ('in_b', t),
-    ('kqv_W', l, t), ('kqv_b', l, t), ('att', l, r), ('msg', l, r), ('prior', l, r), ('a_W', l, t), ('a_b', l, t),
-    ('skip', l, t), ('head_W',), ('head_b',).  Every parameter starts at a multiple of 8 floats (16-byte aligned bf16
-    shadow); the att and msg blocks of the relations into one (layer, type) are contiguous."""
-    H, nhd, L = self.hidden, self.heads, self.L
+  def _param_layout(self):
+    """Names ('in_W', t), ('in_b', t), ('kqv_W', l, t), ('kqv_b', l, t), ('att', l, r), ('msg', l, r), ('prior', l, r),
+    ('a_W', l, t), ('a_b', l, t), ('skip', l, t), ('head_W',), ('head_b',).  The att and msg blocks of the relations
+    into one (layer, type) are contiguous."""
+    H, nhd = self.hidden, self.heads
     D = H // nhd
-    idx, off = {}, 0
-
-    def put(name, *shape):
-      nonlocal off
-      off = _round_up(off, 8)
-      idx[name] = (off, shape)
-      off += math.prod(shape)
     for u in self.in_types:
-      put(('in_W', u), H, self.dim_in[self.ntypes[u]])
-      put(('in_b', u), H)
-    for l in range(1, L + 1):
+      yield ('in_W', u), (H, self.dim_in[self.ntypes[u]])
+      yield ('in_b', u), (H,)
+    for l in range(1, self.L + 1):
       for u in self.kqv_types[l]:
-        put(('kqv_W', l, u), 3 * H, H)
-        put(('kqv_b', l, u), 3 * H)
+        yield ('kqv_W', l, u), (3 * H, H)
+        yield ('kqv_b', l, u), (3 * H,)
       for t in self.targets[l]:
         for kind in ('att', 'msg'):
           for r in self.in_rel[l][t]:
-            put((kind, l, r), nhd, D, D)
+            yield (kind, l, r), (nhd, D, D)
         for r in self.in_rel[l][t]:
-          put(('prior', l, r), nhd)
-        put(('a_W', l, t), H, H)
-        put(('a_b', l, t), H)
-        put(('skip', l, t), 1)
-    put(('head_W',), self.n_out_pad, H)
-    put(('head_b',), self.n_out_pad)
-    self.param_index = idx
-    self.p32 = torch.zeros(_round_up(off, 8), dtype=torch.float32, device=self.device)
-    g = torch.Generator(device='cpu')
-    g.manual_seed(self.seed)
-    linear_w = {'in_W': 'in_b', 'kqv_W': 'kqv_b', 'a_W': 'a_b', 'head_W': 'head_b'}
-    for name, (o, shape) in idx.items():
-      n = math.prod(shape)
-      kind = name[0]
-      if kind in linear_w or kind in linear_w.values():
-        # torch.nn.Linear defaults: U(-1/sqrt(fan_in), 1/sqrt(fan_in)) for weight and bias
-        fan_in = self.param_index[(next(k for k, v in linear_w.items() if v == kind),) + name[1:]][1][1] \
-            if kind in linear_w.values() else shape[1]
-        v = (torch.rand(*shape, generator=g) * 2 - 1) / math.sqrt(fan_in)
-        if kind in ('head_W', 'head_b'):
-          v[self.C:] = 0
-      elif kind in ('att', 'msg'):
-        v = torch.randn(*shape, generator=g) / math.sqrt(D)
-      else:                                                            # prior, skip
-        v = torch.ones(*shape)
-      self.p32[o:o + n].copy_(v.flatten())
-    self._init_optimizer_state()
+          yield ('prior', l, r), (nhd,)
+        yield ('a_W', l, t), (H, H)
+        yield ('a_b', l, t), (H,)
+        yield ('skip', l, t), (1,)
+    yield ('head_W',), (self.n_out_pad, H)
+    yield ('head_b',), (self.n_out_pad,)
 
-  def param(self, name, grad: bool = False) -> torch.Tensor:
-    """bf16 view of a parameter (grad=True: its fp32 gradient slot)."""
-    o, shape = self.param_index[name]
-    buf = self.g32 if grad else self.p16
-    return buf[o:o + math.prod(shape)].view(*shape)
-
-  def _p32(self, name, grad: bool = False) -> torch.Tensor:
-    o, shape = self.param_index[name]
-    return (self.g32 if grad else self.p32)[o:o + math.prod(shape)]
+  def _param_init(self, name, shape, g: torch.Generator) -> torch.Tensor:
+    kind = name[0]
+    if kind in ('att', 'msg'):
+      return torch.randn(*shape, generator=g) / math.sqrt(self.hidden // self.heads)
+    if kind in ('prior', 'skip'):
+      return torch.ones(*shape)
+    # torch.nn.Linear defaults: U(-1/sqrt(fan_in), 1/sqrt(fan_in)) for weight and bias, fan_in from the weight [out, in]
+    fan_in = self.param_index[(kind[:-1] + 'W',) + name[1:]][1][1]
+    v = (torch.rand(*shape, generator=g) * 2 - 1) / math.sqrt(fan_in)
+    if kind in ('head_W', 'head_b'):
+      v[self.C:] = 0
+    return v
 
   def _blocks(self, kind, l, t, grad=False):
-    """[n_rel, heads, D, D] view of the att or msg blocks of the relations into (l, t) (contiguous by layout)."""
-    rels = self.in_rel[l][t]
-    o, shape = self.param_index[(kind, l, rels[0])]
-    n = math.prod(shape)
-    assert all(self.param_index[(kind, l, r)][0] == o + i * n for i, r in enumerate(rels))
-    return (self.g32 if grad else self.p16)[o:o + n * len(rels)].view(len(rels), *shape)
+    """[n_rel, heads, D, D] view of the att or msg blocks of the relations into (l, t)."""
+    D = self.hidden // self.heads
+    return self._rel_params(kind, l, t, grad).view(-1, self.heads, D, D)
 
   def _rel_view(self, buf, l, t):
     """[rows, n_rel * H] contiguous view of a flat per-type buffer for the relations into (l, t)."""
@@ -217,7 +176,7 @@ class HeteroHgtEngine(HeteroSageEngine):
     return buf[t][:n * w].view(n, w)
 
   # ------------------------------------------------------------------ step pieces
-  def _hgt_plan(self, kind: str, l: int = 0, t: int = 0):
+  def _hgt_plan(self, kind: str, l: int, t: int):
     key = ('hgt', kind, l, t)
     pl = self._plans.get(key)
     if pl is not None:
@@ -256,11 +215,6 @@ class HeteroHgtEngine(HeteroSageEngine):
       elif kind == 'a_bwd':
         pl.add_wgrad(self.dA[t][:n], self.GE[l][t], self.param(('a_W', l, t), True), c, nh)
         pl.add_dgrad(self.dA[t][:n], self.param(('a_W', l, t)), self.dGE[t][:n], c, nh)
-      elif kind == 'head_fwd':
-        pl.add_forward(self.Z[L][t], self.param(('head_W',)), self.param(('head_b',)), False, self.logits, c, 1)
-      elif kind == 'head_bwd':
-        pl.add_wgrad(self.dlogits, self.Z[L][t], self.param(('head_W',), True), c, 1)
-        pl.add_dgrad(self.dlogits, self.param(('head_W',)), self.dZL, c, 1)
       else:
         raise KeyError(kind)
     self._plans[key] = pl
@@ -277,12 +231,11 @@ class HeteroHgtEngine(HeteroSageEngine):
     return kv, prior, list(ells), list(kss), deg, alpha
 
   def _forward(self):
-    nat, ar, L = self.nat, self.arena, self.L
+    nat, L = self.nat, self.L
     for u in self.in_types:
-      n = min(self.X0[u].shape[0], self.cap_nodes[u])
-      self.feat[self.ntypes[u]].gather_into(ar.nodes_of(u)[:n], None, self._ctr[u][L + 1:L + 2], self.X0[u][:n])
+      self._gather_input(u)
       self._hgt_plan('in_fwd', 0, u).run()
-      self._k(2)
+      self._k()
     for l in range(1, L + 1):
       nh = L - l + 1
       for t in self.targets[l]:
@@ -302,20 +255,13 @@ class HeteroHgtEngine(HeteroSageEngine):
         self._hgt_plan('a_fwd', l, t).run()
         nat.hgt_gate(self.A[l][t], self.Z[l - 1][t][:self._rows(l, t)], self.Z[l][t], self._p32(('skip', l, t)), c, nh)
         self._k(6)
-    st = self.tid[self.seed_type]
-    self._hgt_plan('head_fwd', L, st).run()
+    self._head_plan().run()
     self._k()
-    if self.peer_group is not None:
-      self.peer_group.barrier(1)            # peers finished reading last step's gradients
-      self._k()
-    nat.zero_grads(self.g32, self.loss, self.correct)
-    self._k(1 + nat.softmax_nll(self.logits, self.C, None, self.labels, ar.nodes_of(st), self._ctr[st], self.loss,
-                                self.dlogits, self.correct, self.param(('head_b',), True), True))
+    self._loss(self.logits, self.dlogits, self.param(('head_b',), True))
 
   def _backward(self):
     nat, L, H = self.nat, self.L, self.hidden
-    st = self.tid[self.seed_type]
-    self._hgt_plan('head_bwd', L, st).run()
+    self._head_plan(self.dZL).run()
     self._k()
     for l in range(L, 0, -1):
       nh = L - l + 1
@@ -362,8 +308,7 @@ class HeteroHgtEngine(HeteroSageEngine):
     R = max(len(self.in_rel[l][t]) for l in range(1, self.L + 1) for t in self.targets[l])
     return 2 * max(max(self.dim_in.values()), (2 * R + 3) * self.hidden)
 
-  def _infer_width(self, l: int) -> int:
-    return self.hidden
+  _infer_head = HeteroSageEngine._infer_linear_head
 
   def _infer_input(self, chunk_rows: int):
     """Input layer: relu(x W_in^T + b_in) of every node of the input types, from gathered feature chunks."""
@@ -407,8 +352,3 @@ class HeteroHgtEngine(HeteroSageEngine):
         nat.hgt_gelu(AGG[:n], GE[:n], self._rows_dev, 0)
         self._gemm(GE[:n], self.param(('a_W', l, t)), self.param(('a_b', l, t)), False, A[:n], 0)
         nat.hgt_gate(A[:n], X[t][r0:r1], Z[t][r0:r1], self._p32(('skip', l, t)), self._rows_dev, 0)
-
-  def _infer_head(self, X: torch.Tensor) -> torch.Tensor:
-    out = torch.empty(X.shape[0], self.n_out_pad, dtype=torch.bfloat16, device=self.device)
-    self._gemm(X, self.param(('head_W',)), self.param(('head_b',)), False, out, 1 + self.tid[self.seed_type])
-    return out

@@ -48,8 +48,7 @@ def _reference(eng, fb, labels):
   nodes, rows, cols, _, nn, ne = eng.arena.to_coo()
   L, nt, kt = eng.L, eng.nt, eng.kt
   bf = lambda x: x.to(torch.bfloat16).float()
-  W = {k: eng.p16[off:off + n * kk].view(n, kk).float().requires_grad_(True) for k, (off, n, kk) in eng._w_off.items()}
-  B = {k: eng.p16[off:off + n].float().requires_grad_(True) for k, (off, n) in eng._b_off.items()}
+  P = {k: eng.param(k).float().requires_grad_(True) for k in eng.param_index}
   x = {t: fb[eng.ntypes[t]][nodes[t]].float() for t in range(len(eng.ntypes))}
   for l in range(1, L + 1):
     nh = L - l + 1
@@ -66,7 +65,7 @@ def _reference(eng, fb, labels):
         blocks.append(bf(agg / deg.clamp(min=1).unsqueeze(1)))
       blocks.append(x[t][:T])
       A = torch.cat(blocks, 1)
-      z = A @ W[(l, t)].t() + B[(l, t)]
+      z = A @ P[('W', l, t)].t() + P[('b', l, t)]
       out[t] = bf(torch.relu(z)) if l < L else z
     x = out
   st = eng.tid[eng.seed_type]
@@ -75,7 +74,7 @@ def _reference(eng, fb, labels):
   y = labels[nodes[st][:n0]]
   loss = torch.nn.functional.cross_entropy(logits, y)
   loss.backward()
-  return float(loss), {k: w.grad for k, w in W.items()}, {k: b.grad for k, b in B.items()}, (nn, ne)
+  return float(loss), {k: p.grad for k, p in P.items()}, (nn, ne)
 
 
 def _gradient_errors(feat_dim=64, hidden=64, classes=19, batch_seed=0):
@@ -89,17 +88,12 @@ def _gradient_errors(feat_dim=64, hidden=64, classes=19, batch_seed=0):
   eng._backward()
   torch.cuda.synchronize()
   assert eng.overflow_count() == 0
-  ref_loss, ref_grads, ref_bgrads, (nn, ne) = _reference(eng, fb, labels)
+  ref_loss, ref_grads, (nn, ne) = _reference(eng, fb, labels)
   assert sum(sum(v) for v in ne) > 1000                     # the batch really has relations of every kind
   errs = {'loss': abs(float(eng.loss.item()) - ref_loss) / max(1.0, abs(ref_loss))}
-  for k, (off, n, kk) in eng._w_off.items():
-    r = ref_grads[k]
+  for k, r in ref_grads.items():
     if r is not None:
-      errs[f'W{k}'] = float((eng.g32[off:off + n * kk].view(n, kk) - r).abs().max()) / max(float(r.abs().max()), 1e-6)
-  for k, (off, n) in eng._b_off.items():
-    r = ref_bgrads[k]
-    if r is not None:
-      errs[f'b{k}'] = float((eng.g32[off:off + n] - r).abs().max()) / max(float(r.abs().max()), 1e-6)
+      errs[f'{k[0]}{k[1:]}'] = float((eng.param(k, True) - r).abs().max()) / max(float(r.abs().max()), 1e-6)
   return errs
 
 

@@ -134,7 +134,7 @@ def _ref_rsage(eng, data):
         deg = torch.bincount(dst, minlength=n).clamp(min=1).unsqueeze(1).float()
         blocks.append(torch.zeros(n, X[eng.nt[r]].shape[1], device=DEV).index_add_(0, dst, X[eng.nt[r]][src]) / deg)
       A = bf(torch.cat(blocks + [X[t]], 1))
-      z = A @ eng.W(l, t).float().t() + eng.b(l, t).float()
+      z = A @ eng.param(('W', l, t)).float().t() + eng.param(('b', l, t)).float()
       Z[t] = bf(F.relu(z) if l < eng.L else z)
     X = Z
   return X[eng.tid['paper']][:, :eng.C]
