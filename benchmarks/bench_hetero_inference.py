@@ -161,6 +161,8 @@ def main():
   p.add_argument('--warmup', type=int, default=1)
   p.add_argument('--sample', type=int, default=10000)
   p.add_argument('--chunk-rows', type=int, default=None)
+  p.add_argument('--feat-format', default='bf16', choices=['bf16', 'mxfp8'],
+                 help='feature storage of every node type; with mxfp8 the PyTorch arm reads the de-quantised rows')
   args = p.parse_args()
   import graphlearn_for_pytorch_b200 as glt
   from common import synthetic_igbh, synthetic_mag
@@ -179,14 +181,17 @@ def main():
   for et, ei in edges.items():
     graphs[et] = glt.data.Graph(glt.data.Topology(ei.to(dev), layout='CSC', num_nodes=sizes[et[2]]), 'CUDA', 0)
   for t, x in feats.items():
-    fdev[t] = x.to(dev).to(torch.bfloat16)
-    ut = glt.data.UnifiedTensor(0, torch.bfloat16)
-    ut.append_shared_tensor(fdev[t])
+    rows = fdev[t] = x.to(dev).to(torch.bfloat16)
+    if args.feat_format == 'mxfp8':
+      rows = glt.data.quantize_mxfp8_chunked(rows)
+      fdev[t] = glt.data.dequantize_mxfp8(rows, x.shape[1]).to(torch.bfloat16)
+    ut = glt.data.UnifiedTensor(0, rows.dtype)
+    ut.append_shared_tensor(rows)
     keep.append(ut)
     tables[t] = ut._table()
   y = torch.randint(0, classes, (sizes['paper'],), generator=torch.Generator().manual_seed(5)).to(dev)
   kw = dict(fanouts=fan, batch_size=1024, hidden=hidden, num_classes=classes, edge_dir='in', seed=1, device=dev,
-            use_cuda_graph=False)
+            use_cuda_graph=False, feature_format=args.feat_format)
   if args.model == 'rsage':
     eng = HeteroSageEngine(graphs, tables, y, feat_dim, sizes, 'paper', **kw)
   elif args.model == 'rgat':
@@ -228,7 +233,7 @@ def main():
   a, b = out_eng[sample].float(), out_torch[sample].float()
   result = {'metric': f'{args.model} full-neighbourhood inference of every seed-type node (device-timed ms per call, '
                       f'median of {args.calls})',
-            'card': card(), 'model': args.model, 'nodes': sizes,
+            'card': card(), 'model': args.model, 'feature_format': args.feat_format, 'nodes': sizes,
             'edges': {'/'.join(k): int(v.shape[1]) for k, v in edges.items()}, 'feat_dim': feat_dim, 'hidden': hidden,
             'heads': heads if args.model != 'rsage' else None, 'layers': len(fan), 'classes': classes,
             'chunk_rows': args.chunk_rows,

@@ -43,6 +43,9 @@ p.add_argument('--model', default='rsage', choices=['rsage', 'rgat'])
 p.add_argument('--heads', type=int, default=4, help='attention heads of --model rgat')
 p.add_argument('--rounds', type=int, default=1, help='timed windows of --steps steps (ms_per_step is their median)')
 p.add_argument('--cap-limit', type=int, default=1 << 21)
+p.add_argument('--feat-format', default='bf16', choices=['bf16', 'mxfp8'],
+               help='engine path: feature storage of every node type (mxfp8 = e4m3 + UE8M0/32 block scales, '
+                    'de-quantised inside the kernels that read the tables)')
 p.add_argument('--device-gen', action='store_true', help='generate the graph / feature shards on the GPU')
 args = p.parse_args()
 rank, world = int(os.environ.get('RANK', 0)), int(os.environ.get('WORLD_SIZE', 1))
@@ -126,7 +129,7 @@ def emit(ms, extra):
     print(json.dumps(dict({'metric': METRIC, 'value': args.steps * args.batch * world / (ms / 1e3), 'unit': 'samples/s',
                            'n_gpus': world, 'ms_per_step': ms / args.steps, 'steps': args.steps, 'model': args.model,
                            'papers': args.papers, 'feat_dim': args.feat_dim, 'hidden': args.hidden, 'fanout': fan,
-                           'batch': args.batch, 'impl': args.impl,
+                           'batch': args.batch, 'impl': args.impl, 'feature_format': args.feat_format,
                            'ms_per_step_rounds': [m / args.steps for m in ROUND_MS]}, **extra)), flush=True)
 
 
@@ -207,6 +210,11 @@ def run_ours():
   else:
     edges, feats, labels, sizes = igbh_graph()
     feat_shard = lambda nt, lo, hi: feats[nt][lo:hi].to(dev).to(torch.bfloat16)   # noqa: E731
+  if args.feat_format == 'mxfp8':
+    if args.path != 'engine':
+      raise SystemExit('--feat-format mxfp8 is read by the engines (--path engine)')
+    bf16_shard = feat_shard
+    feat_shard = lambda nt, lo, hi: glt.data.quantize_mxfp8_chunked(bf16_shard(nt, lo, hi))   # noqa: E731
   edge_dir = 'in'
   topos = {}
   for et in list(edges):
@@ -221,8 +229,9 @@ def run_ours():
     graphs = {et: glt.data.Graph(t, 'CUDA', local) for et, t in topos.items()}
     fstore, tables = {}, {}
     for nt in sizes:
-      ut = glt.data.UnifiedTensor(local, torch.bfloat16)
-      ut.append_shared_tensor(feat_shard(nt, 0, sizes[nt]))
+      shard = feat_shard(nt, 0, sizes[nt])
+      ut = glt.data.UnifiedTensor(local, shard.dtype)
+      ut.append_shared_tensor(shard)
       fstore[nt], tables[nt] = ut, ut._table()
   del topos
   torch.cuda.empty_cache()
@@ -234,7 +243,7 @@ def run_ours():
 
   if args.path == 'engine':
     kw = dict(fanouts=fan, batch_size=args.batch, hidden=args.hidden, num_classes=args.classes, edge_dir=edge_dir,
-              lr=1e-3, seed=1, device=dev, use_cuda_graph=True, cap_limit=args.cap_limit)
+              lr=1e-3, seed=1, device=dev, use_cuda_graph=True, cap_limit=args.cap_limit, feature_format=args.feat_format)
     if args.model == 'rgat':
       eng = HeteroGatEngine(graphs, tables, y, args.feat_dim, sizes, 'paper', heads=args.heads, **kw)
       path = ('HeteroGatEngine: native grouped hetero sampling arena + per-relation wgmma projections + attention '

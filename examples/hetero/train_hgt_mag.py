@@ -113,6 +113,8 @@ def parse():
   p.add_argument('--zero-copy', action='store_true', help='keep the topology in pinned host memory (reference default)')
   p.add_argument('--mode', choices=['loader', 'engine'], default='loader',
                  help='loader: hetero NeighborLoader + models.HGT under autograd; engine: HeteroHgtEngine (one GPU)')
+  p.add_argument('--feat-format', choices=['bf16', 'mxfp8'], default='bf16',
+                 help='--mode engine: store the feature tables as MXFP8 rows (e4m3 + one scale per 32 elements)')
   p.add_argument('--eval', choices=['sampled', 'full'], default='sampled',
                  help='--mode engine: validation accuracy from sampled batches (evaluate_batch), or validation and test '
                       'accuracy of exact layer-wise full-neighbourhood inference (HeteroHgtEngine.inference)')
@@ -141,17 +143,21 @@ def run_engine(args):
   for et, ei in edges.items():
     topo = glt.data.Topology(ei.to(dev), layout='CSC', num_nodes=sizes[et[2]])
     graphs[et] = glt.data.Graph(topo, 'CUDA', 0)
-  in_dim = {}
+  in_dim, fmt = {}, {}
   for t, x in feats.items():
-    ut = glt.data.UnifiedTensor(0, torch.bfloat16)
-    ut.append_shared_tensor(x.to(dev).to(torch.bfloat16))
+    rows = x.to(dev).to(torch.bfloat16)
+    fmt[t] = 'mxfp8' if args.feat_format == 'mxfp8' and x.shape[1] % 32 == 0 else 'bf16'
+    if fmt[t] == 'mxfp8':
+      rows = glt.data.quantize_mxfp8_chunked(rows)
+    ut = glt.data.UnifiedTensor(0, rows.dtype)
+    ut.append_shared_tensor(rows)
     keep.append(ut)
     tables[t] = ut._table()
     in_dim[t] = x.shape[1]
   y = labels['paper']
   eng = HeteroHgtEngine(graphs, tables, y.to(dev), in_dim, sizes, 'paper', fanouts=[10, 10], batch_size=args.batch,
                         hidden=args.hidden, heads=args.heads, num_classes=int(y.max()) + 1, edge_dir='in', lr=0.01,
-                        device=dev)
+                        device=dev, feature_format=fmt)
   eng.warmup_and_capture()
   print(f'HeteroHgtEngine: {eng.kernels_per_step} kernels per step, one CUDA graph')
   for epoch in range(1, args.epochs + 1):

@@ -137,22 +137,29 @@ def run_engine(rank, world, igbh, a, port):
   log = get_mlperf_logger()
   topos = {et: glt.data.Topology(ei.to(device), layout='CSC', num_nodes=num_nodes[et[2]]) for et, ei in edge_dict.items()}
   keep = []
+  # --feat-format mxfp8: every type whose width is a multiple of 32 is stored as MXFP8 rows (about half the bytes)
+  fmt = {nt: 'mxfp8' if a.feat_format == 'mxfp8' and f.shape[1] % 32 == 0 else 'bf16' for nt, f in feat_dict.items()}
+
+  def shard(nt, rows):
+    rows = rows.to(device).to(torch.bfloat16)
+    return glt.data.quantize_mxfp8_chunked(rows) if fmt[nt] == 'mxfp8' else rows
   if world > 1:
     graphs, bounds, keep = partition_hetero_graph(topos, num_nodes, rank, world, device, 'in')
-    stores = {nt: PartitionedFeature(feat_dict[nt][bounds[nt][rank]:bounds[nt][rank + 1]].to(device).to(torch.bfloat16),
+    stores = {nt: PartitionedFeature(shard(nt, feat_dict[nt][bounds[nt][rank]:bounds[nt][rank + 1]]),
                                      bounds[nt], device) for nt in num_nodes}
     tables = {nt: s.table for nt, s in stores.items()}
   else:
     graphs = {et: glt.data.Graph(t, 'CUDA', rank) for et, t in topos.items()}
     stores, tables = {}, {}
     for nt in num_nodes:
-      ut = glt.data.UnifiedTensor(rank, torch.bfloat16)
-      ut.append_shared_tensor(feat_dict[nt].to(device).to(torch.bfloat16))
+      rows = shard(nt, feat_dict[nt])
+      ut = glt.data.UnifiedTensor(rank, rows.dtype)
+      ut.append_shared_tensor(rows)
       stores[nt], tables[nt] = ut, ut._table()
   in_dim = {nt: (f.shape[1] + 7) // 8 * 8 for nt, f in feat_dict.items()}
   fan = [int(v) for v in a.fan_out.split(',')]
   common = dict(fanouts=fan, batch_size=a.train_batch_size, hidden=a.hidden_channels, num_classes=num_classes,
-                edge_dir='in', lr=a.learning_rate, seed=a.random_seed, device=device)
+                edge_dir='in', lr=a.learning_rate, seed=a.random_seed, device=device, feature_format=fmt)
   if a.model == 'rgat':
     eng = HeteroGatEngine(graphs, tables, label.to(device), in_dim, num_nodes, 'paper', heads=a.num_heads, **common)
   else:
@@ -207,6 +214,8 @@ if __name__ == '__main__':
   ap.add_argument('--use_fp16', action='store_true')
   ap.add_argument('--model', default='rgat', choices=['rgat', 'rsage', 'rgcn'])
   ap.add_argument('--trainer', default='loader', choices=['loader', 'engine'])
+  ap.add_argument('--feat-format', default='bf16', choices=['bf16', 'mxfp8'],
+                  help='--trainer engine: store the feature tables as MXFP8 rows (e4m3 + one scale per 32 elements)')
   ap.add_argument('--fan_out', default='15,10,5')
   ap.add_argument('--train_batch_size', type=int, default=1024)
   ap.add_argument('--val_batch_size', type=int, default=1024)

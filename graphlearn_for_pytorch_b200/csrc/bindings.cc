@@ -684,6 +684,10 @@ struct HeteroArena {
   Tensor ell_of(int64_t r, int64_t h) { return ell[r][h]; }
 };
 
+// Bytes of an MXFP8 row of d elements: d e4m3 bytes, d / 32 scale bytes, zero padding to 16 (data/quantize.py,
+// mxfp8_row_bytes).
+static int64_t mxfp8_row_bytes(int64_t d) { return (d + d / 32 + 15) / 16 * 16; }
+
 // ---------------------------------------------------------------------------
 // RowTableHandle: multi-source row store (UnifiedTensor).
 // ---------------------------------------------------------------------------
@@ -755,6 +759,30 @@ struct RowTableHandle {
     return out;
   }
 
+  bool holds_mxfp8(int64_t d) const {
+    return dtype == torch::kUInt8 && d % 32 == 0 && d >= 32 && d <= 1024 && width == mxfp8_row_bytes(d);
+  }
+
+  // gather_into for MXFP8 rows of d elements (any multiple of 32 up to 1024): out[i, :d] = bf16(dequantised row);
+  // rows past *n_dev and rows with a negative (or unmapped) id are written as zeros; columns >= d are not touched
+  void gather_mxfp8_into(const Tensor& idx, const c10::optional<Tensor>& id2index,
+                         const c10::optional<Tensor>& n_dev, Tensor out, int64_t d) {
+    c10::cuda::CUDAGuard guard(device);
+    TORCH_CHECK(d % 32 == 0 && d >= 32 && d <= 1024, "gather_mxfp8_into: d must be a multiple of 32 in [32, 1024]");
+    TORCH_CHECK(holds_mxfp8(d), "gather_mxfp8_into: the table must hold uint8 rows of mxfp8_row_bytes(d) bytes");
+    TORCH_CHECK(idx.is_cuda() && idx.scalar_type() == torch::kInt64 && idx.is_contiguous(),
+                "gather_mxfp8_into: idx must be a contiguous int64 CUDA tensor");
+    TORCH_CHECK(out.is_cuda() && out.scalar_type() == torch::kBFloat16 && out.dim() == 2 && out.stride(1) == 1 &&
+                out.size(0) >= idx.numel() && out.size(1) >= d && out.stride(0) % 8 == 0 &&
+                reinterpret_cast<uintptr_t>(out.data_ptr()) % 16 == 0,
+                "gather_mxfp8_into: destination must be bf16 [>= rows, >= d] with unit inner stride and 16-byte aligned rows");
+    const int64_t* map = (id2index.has_value() && id2index->defined()) ? id2index->data_ptr<int64_t>() : nullptr;
+    const int32_t* nd = (n_dev.has_value() && n_dev->defined()) ? n_dev->data_ptr<int32_t>() : nullptr;
+    launch_gather_mxfp8_rows(tbl, idx.data_ptr<int64_t>(), map, idx.numel(), nd, static_cast<int>(d), out.data_ptr(),
+                             out.stride(0) * 2, cur_stream(), map ? id2index->numel() : 0);
+    check_cuda_err("gather_mxfp8_into");
+  }
+
   // static-shape gather into a caller-provided buffer with a device-side count
   void gather_into(const Tensor& idx, const c10::optional<Tensor>& id2index,
                    const c10::optional<Tensor>& n_dev, Tensor out) {
@@ -797,9 +825,10 @@ static SageAggArgs make_agg(RowTableHandle* feat, const c10::optional<Tensor>& n
     TORCH_CHECK(feat != nullptr && nodes.has_value(), "layer-1 aggregation needs a feature table + nodes");
     TORCH_CHECK(feat->dtype == torch::kBFloat16 || feat->dtype == torch::kUInt8,
                 "engine features must be bf16 rows or MXFP8 (uint8) rows");
-    TORCH_CHECK(feat->dtype == torch::kBFloat16 ? feat->width == d : feat->width == d + 16,
-                "feature width mismatch (MXFP8 rows are d + 16 bytes)");
+    TORCH_CHECK(feat->dtype == torch::kBFloat16 ? feat->width == d : feat->holds_mxfp8(d),
+                "feature width mismatch (bf16 rows are d wide; MXFP8 rows are mxfp8_row_bytes(d) bytes, d a multiple of 32 in [32, 1024])");
     a.feat = feat->tbl;
+    a.feat_fp8 = feat->dtype == torch::kUInt8 ? 1 : 0;
     a.nodes = nodes->data_ptr<int64_t>();
   }
   TORCH_CHECK(d % 8 == 0, "feature width must be a multiple of 8");
@@ -820,8 +849,6 @@ static void sage_aggregate(RowTableHandle* feat, const c10::optional<Tensor>& no
   c10::cuda::CUDAGuard guard(out.device());
   check_sage_width(d, "sage_aggregate: d must be a multiple of 8 in [8, 1024]");
   TORCH_CHECK(out.scalar_type() == torch::kBFloat16 && out.is_contiguous() && out.size(1) == 2 * d);
-  TORCH_CHECK(feat == nullptr || (src_local.has_value() && src_local->defined()) || feat->dtype == torch::kBFloat16,
-              "the unfused aggregation kernel reads bf16 rows; MXFP8 tables go through sage_fused");
   SageAggArgs a = make_agg(feat, nodes, src_local, d, counters, n_hops_targets, out.size(0), ell, ks,
                            deg, out.data_ptr());
   launch_sage_aggregate(a, cur_stream());
@@ -911,8 +938,8 @@ static void sage_full_aggregate(GraphHandle* graph, RowTableHandle* feat, const 
     TORCH_CHECK(feat != nullptr, "sage_full_aggregate: needs a feature table or a src table");
     TORCH_CHECK(feat->dtype == torch::kBFloat16 || feat->dtype == torch::kUInt8,
                 "engine features must be bf16 rows or MXFP8 (uint8) rows");
-    TORCH_CHECK(feat->dtype == torch::kBFloat16 ? feat->width == d : (feat->width == d + 16 && d == 128),
-                "feature width mismatch (MXFP8 rows are d + 16 bytes, d = 128)");
+    TORCH_CHECK(feat->dtype == torch::kBFloat16 ? feat->width == d : feat->holds_mxfp8(d),
+                "feature width mismatch (bf16 rows are d wide; MXFP8 rows are mxfp8_row_bytes(d) bytes, d a multiple of 32 in [32, 1024])");
     a.feat = feat->tbl;
     a.feat_fp8 = feat->dtype == torch::kUInt8 ? 1 : 0;
   }
@@ -2092,11 +2119,13 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def("append", &RowTableHandle::append, py::arg("part"), py::arg("remote") = false)
       .def("num_rows", &RowTableHandle::num_rows)
       .def_readonly("width", &RowTableHandle::width)
+      .def_property_readonly("is_uint8", [](const RowTableHandle& t) { return t.dtype == torch::kUInt8; })
       .def_property_readonly("num_parts", [](const RowTableHandle& t) { return t.tbl.num_parts; })
       .def("gather", &RowTableHandle::gather, py::arg("idx"), py::arg("id2index") = py::none(),
            py::arg("out_width") = 0)
       .def("gather_into", &RowTableHandle::gather_into)
       .def("gather_mxfp8", &RowTableHandle::gather_mxfp8)
+      .def("gather_mxfp8_into", &RowTableHandle::gather_mxfp8_into)
       .def("all_local", &RowTableHandle::all_local);
 
   // ---- GraphSAGE engine ----

@@ -122,11 +122,9 @@ __device__ __forceinline__ uint32_t ld_nc_u32(const void* p) {
   return r;
 }
 
-// MXFP8 (OCP microscaling: e4m3 elements, one UE8M0 power-of-two scale per 32 elements).  `v` holds 16 consecutive
-// elements of a row starting at element gl * 16, `scales` the row's first four block-scale bytes; the block of this
-// lane's elements is gl >> 1.  acc[0..16) += dequantised values.
-__device__ __forceinline__ void mxfp8x16_accum(const uint4& v, uint32_t scales, int gl, float* acc) {
-  const float s = __uint_as_float(((scales >> (8 * (gl >> 1))) & 0xFFu) << 23);   // UE8M0 byte b -> 2^(b - 127)
+// MXFP8 (OCP microscaling: e4m3 elements, one UE8M0 power-of-two scale per 32 elements; a scale byte b is 2^(b - 127)).
+// acc[0..16) += the 16 consecutive elements in `v` times their block's scale s.
+__device__ __forceinline__ void mxfp8x16_accum_scaled(const uint4& v, float s, float* acc) {
   const uint32_t w[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
@@ -139,6 +137,26 @@ __device__ __forceinline__ void mxfp8x16_accum(const uint4& v, uint32_t scales, 
       acc[i * 4 + h * 2 + 1] += f2.y * s;
     }
   }
+}
+
+// d = 128 rows: `v` holds the elements starting at element gl * 16, `scales` the row's four block-scale bytes; the
+// block of this lane's elements is gl >> 1.
+__device__ __forceinline__ void mxfp8x16_accum(const uint4& v, uint32_t scales, int gl, float* acc) {
+  mxfp8x16_accum_scaled(v, __uint_as_float(((scales >> (8 * (gl >> 1))) & 0xFFu) << 23), acc);
+}
+
+// Rows of any width d (a multiple of 32): `row` points at an MXFP8 row, c is the 16-element vector
+// index (elements [16c, 16c + 16), block c >> 1).  The block's scale byte sits at row + d + (c >> 1) and is fetched
+// once per vector.  mxfp8_scale_at and mxfp8x16_accum_scaled are the two halves, for callers that issue the loads
+// of several rows before they accumulate.
+__device__ __forceinline__ float mxfp8_scale_at(const uint8_t* row, int d, int c) {
+  uint32_t b;
+  asm volatile("ld.global.nc.L1::no_allocate.u8 %0, [%1];" : "=r"(b) : "l"(row + d + (c >> 1)));
+  return __uint_as_float(b << 23);
+}
+
+__device__ __forceinline__ void mxfp8x16_accum_at(const uint8_t* row, int d, int c, float* acc) {
+  mxfp8x16_accum_scaled(ld_nc_v4(row + c * 16), mxfp8_scale_at(row, d, c), acc);
 }
 
 __device__ __forceinline__ void bf16x8_accum(const uint4& v, float* acc) {

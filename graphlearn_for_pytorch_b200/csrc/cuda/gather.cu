@@ -133,6 +133,60 @@ __global__ void __launch_bounds__(256) k_gather_mxfp8(RowTable t, const int64_t*
   }
 }
 
+// k_gather_vec for MXFP8 rows of d elements (d / 16 vectors of 16 e4m3 elements): the same id -> (id2index) -> shard
+// pointer chase with R rows in flight per lane group, but every 16-byte load comes with its block's scale byte and
+// is stored as two 16-byte vectors of bf16.  Rows past the device count and negative ids are written as zeros.
+template <int LPR, int R>
+__global__ void __launch_bounds__(256) k_gather_mxfp8_vec(RowTable t, const int64_t* idx, const int64_t* id2index,
+                                                          int64_t n, const int32_t* n_dev, int d, uint8_t* out,
+                                                          int64_t out_row_bytes, int64_t map_len) {
+  constexpr int RPW = 32 / LPR;
+  const int lane = threadIdx.x & 31;
+  const int gl = lane % LPR;
+  const int gw = lane / LPR;
+  const int64_t n_valid = n_dev ? min(static_cast<int64_t>(*n_dev), n) : n;
+  const int nvec = d >> 4;
+  const int64_t wpb = blockDim.x >> 5;
+  for (int64_t base = (blockIdx.x * wpb + (threadIdx.x >> 5)) * (RPW * R); base < n;
+       base += static_cast<int64_t>(gridDim.x) * wpb * (RPW * R)) {
+    int64_t row[R];
+#pragma unroll
+    for (int k = 0; k < R; ++k) {
+      const int64_t r = base + k * RPW + gw;
+      row[k] = (r < n_valid) ? idx[r] : -1;
+    }
+    if (id2index) {
+#pragma unroll
+      for (int k = 0; k < R; ++k)
+        if (row[k] >= 0) row[k] = (map_len <= 0 || row[k] < map_len) ? id2index[row[k]] : -1;
+    }
+    const uint8_t* src[R];
+#pragma unroll
+    for (int k = 0; k < R; ++k) src[k] = row[k] >= 0 ? row_ptr(t, row[k]) : nullptr;
+    for (int c = gl; c < nvec; c += LPR) {
+      uint4 v[R];
+      float sc[R];
+#pragma unroll
+      for (int k = 0; k < R; ++k) {
+        v[k] = src[k] ? ld_nc_v4(src[k] + c * 16) : make_uint4(0, 0, 0, 0);
+        sc[k] = src[k] ? mxfp8_scale_at(src[k], d, c) : 0.f;
+      }
+#pragma unroll
+      for (int k = 0; k < R; ++k) {
+        const int64_t r = base + k * RPW + gw;
+        if (r >= n) continue;
+        float x[16];
+#pragma unroll
+        for (int i = 0; i < 16; ++i) x[i] = 0.f;
+        mxfp8x16_accum_scaled(v[k], sc[k], x);
+        uint4* o = reinterpret_cast<uint4*>(out + r * out_row_bytes) + 2 * c;
+        o[0] = pack_bf16x8(x, 1.f);
+        o[1] = pack_bf16x8(x + 8, 1.f);
+      }
+    }
+  }
+}
+
 }  // namespace
 
 void launch_gather_rows(RowTable t, const int64_t* idx, const int64_t* id2index, int64_t n,
@@ -208,6 +262,31 @@ void launch_gather_mxfp8(RowTable t, const int64_t* idx, int64_t n, int d, void*
   int64_t blocks = (n + 31) / 32;
   if (blocks > 132 * 16) blocks = 132 * 16;
   k_gather_mxfp8<<<static_cast<int>(blocks), 256, 0, s>>>(t, idx, n, d, reinterpret_cast<__nv_bfloat16*>(out));
+}
+
+void launch_gather_mxfp8_rows(RowTable t, const int64_t* idx, const int64_t* id2index, int64_t n, const int32_t* n_dev,
+                              int d, void* out, int64_t out_row_bytes, cudaStream_t s, int64_t id2index_len) {
+  if (n <= 0) return;
+  uint8_t* o = reinterpret_cast<uint8_t*>(out);
+  const int nvec = d / 16;
+  // launch shapes as in launch_gather_rows: small lookups one row per group, large ones four rows in flight
+#define GLT_LAUNCH_MXFP8(LPR)                                                                                 \
+  do {                                                                                                        \
+    if (n >= static_cast<int64_t>(132) * 2 * 8 * (32 / LPR) * 4)                                              \
+      k_gather_mxfp8_vec<LPR, 4><<<grid_for(n, 8 * (32 / LPR) * 4), 256, 0, s>>>(t, idx, id2index, n, n_dev,  \
+                                                                                  d, o, out_row_bytes,        \
+                                                                                  id2index_len);              \
+    else                                                                                                      \
+      k_gather_mxfp8_vec<LPR, 1><<<grid_for(n, 8 * (32 / LPR)), 256, 0, s>>>(t, idx, id2index, n, n_dev, d,   \
+                                                                              o, out_row_bytes,               \
+                                                                              id2index_len);                  \
+  } while (0)
+  if (nvec <= 2) GLT_LAUNCH_MXFP8(2);
+  else if (nvec <= 4) GLT_LAUNCH_MXFP8(4);
+  else if (nvec <= 8) GLT_LAUNCH_MXFP8(8);
+  else if (nvec <= 16) GLT_LAUNCH_MXFP8(16);
+  else GLT_LAUNCH_MXFP8(32);
+#undef GLT_LAUNCH_MXFP8
 }
 
 }  // namespace glt

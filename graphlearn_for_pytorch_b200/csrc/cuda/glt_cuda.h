@@ -157,8 +157,12 @@ void launch_gather_i64(RowTable t, const int64_t* idx, int64_t n, const int32_t*
                        int64_t* out, cudaStream_t s);
 // copy `nbytes` (multiple of 16) from local memory to an NVSwitch multicast address
 void launch_multimem_copy(const void* src, void* mc_dst, int64_t nbytes, cudaStream_t s);
-// out[i, 0..d) (bf16) = dequantised MXFP8 row idx[i] of `t` (rows of d + 16 bytes, see data/quantize.py)
+// out[i, 0..d) (bf16) = dequantised MXFP8 row idx[i] of `t` (see data/quantize.py), d a multiple of 128
 void launch_gather_mxfp8(RowTable t, const int64_t* idx, int64_t n, int d, void* out, cudaStream_t s);
+// launch_gather_rows for MXFP8 rows of any d that is a multiple of 32 up to 1024: the same idx / id2index / n_dev
+// contract, de-quantised into bf16 rows of pitch out_row_bytes (a multiple of 16; `out` 16-byte aligned)
+void launch_gather_mxfp8_rows(RowTable t, const int64_t* idx, const int64_t* id2index, int64_t n, const int32_t* n_dev,
+                              int d, void* out, int64_t out_row_bytes, cudaStream_t s, int64_t id2index_len = 0);
 
 // ---- sage.cu (GraphSAGE engine kernels) ---------------------------------------
 struct SageAggArgs {
@@ -181,6 +185,7 @@ struct SageAggArgs {
   int out_ld;                   // row pitch of `out` in elements
   int mean_col;                 // first column of this relation's mean block
   int self_col;                 // first column of the self block, -1 = do not write it
+  int feat_fp8;                 // 1: `feat` rows are MXFP8 (data/quantize.py), d a multiple of 32; src_local is always bf16
 };
 void launch_sage_aggregate(const SageAggArgs& a, cudaStream_t s);
 
@@ -192,7 +197,8 @@ void launch_sage_aggregate(const SageAggArgs& a, cudaStream_t s);
 //   mean only (combine = 0, mean_only = 1): out[r - r0, :d] = bf16(mean_u x_u), nothing else is written (one relation's
 //                                           column block of a heterogeneous layer's wider A operand)
 // Sources: the dense bf16 table `src` (row u at src + u * src_ld, ids outside [0, n_src) read as zero rows), or,
-// when src == nullptr, the feature table `feat` (bf16 rows of d elements, or MXFP8 rows with feat_fp8 = 1, d = 128).
+// when src == nullptr, the feature table `feat` (bf16 rows of d elements, or MXFP8 rows with feat_fp8 = 1, d a multiple
+// of 32).
 struct SageFullAggArgs {
   GraphTable g;
   RowTable feat;

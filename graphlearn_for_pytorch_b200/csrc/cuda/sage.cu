@@ -33,8 +33,10 @@ __device__ __forceinline__ const uint8_t* src_row(const SageAggArgs& a, int s) {
   return row_ptr(a.feat, a.nodes[s]);
 }
 
-// LPR lanes cooperate on one target row; each lane owns VPL 16-byte vectors.
-template <int LPR, int VPL>
+// LPR lanes cooperate on one target row; each lane owns VPL 16-byte vectors: 8 bf16 elements, or (FP8: the feature
+// table holds MXFP8 rows) 16 e4m3 elements that are de-quantised as they are accumulated.  Either way the mean is
+// summed in fp32 in ELL slot order, rounded once and written as bf16; the FP8 self block is bf16(de-quantised row).
+template <int LPR, int VPL, bool FP8 = false>
 __global__ void __launch_bounds__(256) k_sage_aggregate(SageAggArgs a) {
   pdl_enter();
   constexpr int RPW = 32 / LPR;
@@ -44,15 +46,16 @@ __global__ void __launch_bounds__(256) k_sage_aggregate(SageAggArgs a) {
   const unsigned gmask = (LPR == 32) ? 0xffffffffu : (((1u << LPR) - 1u) << (gw * LPR));
   const int T = min(a.cum[a.n_hops_targets], a.cap_targets);
   const int wpb = blockDim.x >> 5;
-  const int nvec = a.d >> 3;
+  constexpr int EPV = FP8 ? 16 : 8;
+  const int nvec = a.d / EPV;
   for (int base = (blockIdx.x * wpb + (threadIdx.x >> 5)) * RPW; base < T; base += gridDim.x * wpb * RPW) {
     const int t = base + gw;
     const bool valid = t < T;
-    float acc[VPL][8];
+    float acc[VPL][EPV];
 #pragma unroll
     for (int v = 0; v < VPL; ++v)
 #pragma unroll
-      for (int i = 0; i < 8; ++i) acc[v][i] = 0.f;
+      for (int i = 0; i < EPV; ++i) acc[v][i] = 0.f;
     int dg = 0, k = 0;
     const int32_t* ell = nullptr;
     if (valid) {
@@ -75,7 +78,10 @@ __global__ void __launch_bounds__(256) k_sage_aggregate(SageAggArgs a) {
 #pragma unroll
         for (int v = 0; v < VPL; ++v) {
           const int c = v * LPR + gl;
-          if (c < nvec) bf16x8_accum(ld_nc_v4(p + c * 16), acc[v]);
+          if (c < nvec) {
+            if (FP8) mxfp8x16_accum_at(p, a.d, c, acc[v]);
+            else bf16x8_accum(ld_nc_v4(p + c * 16), acc[v]);
+          }
         }
       }
     }
@@ -89,10 +95,26 @@ __global__ void __launch_bounds__(256) k_sage_aggregate(SageAggArgs a) {
 #pragma unroll
     for (int v = 0; v < VPL; ++v) {
       const int c = v * LPR + gl;
-      if (c < nvec) {
+      if (c >= nvec) continue;
+      if (FP8) {
+        uint4* om = reinterpret_cast<uint4*>(o + mcol * 2) + 2 * c;
+        om[0] = pack_bf16x8(acc[v], inv);
+        om[1] = pack_bf16x8(acc[v] + 8, inv);
+      } else {
         reinterpret_cast<uint4*>(o + mcol * 2)[c] = pack_bf16x8(acc[v], inv);
         if (scol >= 0)
           reinterpret_cast<uint4*>(o + scol * 2)[c] = self ? ld_nc_v4(self + c * 16) : make_uint4(0, 0, 0, 0);
+      }
+    }
+    if (FP8 && scol >= 0) {   // after the means, so that the accumulators are dead
+      for (int c = gl; c < nvec; c += LPR) {
+        float x[16];
+#pragma unroll
+        for (int i = 0; i < 16; ++i) x[i] = 0.f;
+        if (self) mxfp8x16_accum_at(self, a.d, c, x);
+        uint4* os = reinterpret_cast<uint4*>(o + scol * 2) + 2 * c;
+        os[0] = pack_bf16x8(x, 1.f);
+        os[1] = pack_bf16x8(x + 8, 1.f);
       }
     }
   }
@@ -414,6 +436,20 @@ int set_pdl(int on) {
 }
 
 void launch_sage_aggregate(const SageAggArgs& a, cudaStream_t s) {
+  if (a.feat_fp8) {
+    // MXFP8 layer-1 source: d / 16 vectors of 16 elements; <32, 2> holds a 1024-wide row in 32 accumulators per lane
+    const int nvec = a.d / 16;
+#define GLT_LAUNCH_AGG_FP8(LPR, VPL)                                                                             \
+  launch_k(k_sage_aggregate<LPR, VPL, true>, dim3(grid_for(a.cap_targets, 8 * (32 / LPR))), dim3(256), 0, s, a)
+    if (nvec <= 2) GLT_LAUNCH_AGG_FP8(2, 1);
+    else if (nvec <= 4) GLT_LAUNCH_AGG_FP8(4, 1);
+    else if (nvec <= 8) GLT_LAUNCH_AGG_FP8(8, 1);
+    else if (nvec <= 16) GLT_LAUNCH_AGG_FP8(16, 1);
+    else if (nvec <= 32) GLT_LAUNCH_AGG_FP8(32, 1);
+    else GLT_LAUNCH_AGG_FP8(32, 2);
+#undef GLT_LAUNCH_AGG_FP8
+    return;
+  }
   // (a variant keeping 4 neighbour rows in flight per lane group before accumulating made the step slower and was
   // removed: the rows are L2-resident activations)
   GLT_DISPATCH_WIDTH(a.d, {

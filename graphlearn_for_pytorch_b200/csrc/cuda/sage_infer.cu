@@ -35,7 +35,7 @@ struct FullAgg {
   __device__ static void accumulate(const SageFullAggArgs& a, int part, int64_t start, int deg, int first, int stride,
                                     int gl, unsigned gmask, float (&acc)[VPL][EPV]) {
     const int n = first < deg ? (deg - first + stride - 1) / stride : 0;
-    const int nvec = a.d >> 3;
+    const int nvec = a.d / EPV;
     for (int i0 = 0; i0 < n; i0 += LPR) {
       const uint8_t* mine = nullptr;
       if (i0 + gl < n)
@@ -45,37 +45,33 @@ struct FullAgg {
       for (int jj = 0; jj < cnt; jj += R) {
         const uint8_t* p[R];
         uint4 raw[R][VPL];
-        uint32_t sc[R];
+        float sc[R][VPL];   // FP8: the block scale of each vector
 #pragma unroll
         for (int u = 0; u < R; ++u) {
           p[u] = reinterpret_cast<const uint8_t*>(
               __shfl_sync(gmask, reinterpret_cast<unsigned long long>(mine), jj + u, LPR));
           if (jj + u >= cnt) p[u] = nullptr;
-          sc[u] = 0u;
 #pragma unroll
-          for (int v = 0; v < VPL; ++v) raw[u][v] = make_uint4(0, 0, 0, 0);
+          for (int v = 0; v < VPL; ++v) { raw[u][v] = make_uint4(0, 0, 0, 0); sc[u][v] = 0.f; }
         }
 #pragma unroll
         for (int u = 0; u < R; ++u) {
           if (p[u] == nullptr) continue;
-          if (FP8) {
-            // MXFP8 rows (d == 128): d e4m3 bytes, then the d/32 UE8M0 block scales
-            raw[u][0] = ld_nc_v4(p[u] + gl * 16);
-            sc[u] = ld_nc_u32(p[u] + a.d);
-          } else {
 #pragma unroll
-            for (int v = 0; v < VPL; ++v)
-              if (v * LPR + gl < nvec) raw[u][v] = ld_nc_v4(p[u] + (v * LPR + gl) * 16);
+          for (int v = 0; v < VPL; ++v) {
+            const int c = v * LPR + gl;
+            if (c >= nvec) continue;
+            raw[u][v] = ld_nc_v4(p[u] + c * 16);
+            if (FP8) sc[u][v] = mxfp8_scale_at(p[u], a.d, c);   // MXFP8 rows: d e4m3 bytes, then d/32 UE8M0 scales
           }
         }
 #pragma unroll
         for (int u = 0; u < R; ++u) {
           if (p[u] == nullptr) continue;
-          if (FP8) {
-            mxfp8x16_accum(raw[u][0], sc[u], gl, acc[0]);
-          } else {
 #pragma unroll
-            for (int v = 0; v < VPL; ++v) bf16x8_accum(raw[u][v], acc[v]);
+          for (int v = 0; v < VPL; ++v) {
+            if (FP8) mxfp8x16_accum_scaled(raw[u][v], sc[u][v], acc[v]);
+            else bf16x8_accum(raw[u][v], acc[v]);
           }
         }
       }
@@ -87,16 +83,21 @@ struct FullAgg {
     const float inv = deg > 0 ? 1.f / static_cast<float>(deg) : 0.f;
     uint8_t* o = reinterpret_cast<uint8_t*>(a.out) + (r - a.r0) * a.out_ld * 2;
     if (FP8) {
-      float self[16];
+      const uint8_t* sp = a.mean_only ? nullptr : row_ptr(a.feat, r);
 #pragma unroll
-      for (int i = 0; i < 16; ++i) self[i] = 0.f;
-      const uint8_t* sp = row_ptr(a.feat, r);
-      if (sp) mxfp8x16_accum(ld_nc_v4(sp + gl * 16), ld_nc_u32(sp + a.d), gl, self);
-      reinterpret_cast<uint4*>(o)[gl * 2] = pack_bf16x8(acc[0], inv);
-      reinterpret_cast<uint4*>(o)[gl * 2 + 1] = pack_bf16x8(acc[0] + 8, inv);
-      if (a.mean_only) return;
-      reinterpret_cast<uint4*>(o + a.d * 2)[gl * 2] = pack_bf16x8(self, 1.f);
-      reinterpret_cast<uint4*>(o + a.d * 2)[gl * 2 + 1] = pack_bf16x8(self + 8, 1.f);
+      for (int v = 0; v < VPL; ++v) {
+        const int c = v * LPR + gl;
+        if (c >= a.d / EPV) continue;
+        reinterpret_cast<uint4*>(o)[c * 2] = pack_bf16x8(acc[v], inv);
+        reinterpret_cast<uint4*>(o)[c * 2 + 1] = pack_bf16x8(acc[v] + 8, inv);
+        if (a.mean_only) continue;
+        float self[16];
+#pragma unroll
+        for (int i = 0; i < 16; ++i) self[i] = 0.f;
+        if (sp) mxfp8x16_accum_at(sp, a.d, c, self);
+        reinterpret_cast<uint4*>(o + a.d * 2)[c * 2] = pack_bf16x8(self, 1.f);
+        reinterpret_cast<uint4*>(o + a.d * 2)[c * 2 + 1] = pack_bf16x8(self + 8, 1.f);
+      }
       return;
     }
     const int nvec = a.d >> 3;
@@ -213,7 +214,16 @@ void launch_full(const SageFullAggArgs& a, cudaStream_t s) {
 
 void launch_sage_full_aggregate(const SageFullAggArgs& a, cudaStream_t s) {
   if (a.r1 <= a.r0) return;
-  if (a.feat_fp8) { launch_full<8, 1, true>(a, s); return; }
+  if (a.feat_fp8) {   // d / 16 vectors of 16 e4m3 elements; d = 128 is <8, 1, true>
+    const int nvec = a.d / 16;
+    if (nvec <= 2) launch_full<2, 1, true>(a, s);
+    else if (nvec <= 4) launch_full<4, 1, true>(a, s);
+    else if (nvec <= 8) launch_full<8, 1, true>(a, s);
+    else if (nvec <= 16) launch_full<16, 1, true>(a, s);
+    else if (nvec <= 32) launch_full<32, 1, true>(a, s);
+    else launch_full<32, 2, true>(a, s);
+    return;
+  }
   const int nvec = a.d / 8;
   if (nvec <= 4) launch_full<4, 1, false>(a, s);
   else if (nvec <= 8) launch_full<8, 1, false>(a, s);

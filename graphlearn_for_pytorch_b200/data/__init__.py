@@ -9,7 +9,7 @@ from .vineyard_utils import (vineyard_to_csr, load_vertex_feature_from_vineyard,
                              get_fid_from_gid, get_frag_vertex_offset, get_frag_vertex_num, VineyardPartitionBook,
                              VineyardGid2Lid, v6d_id_select, v6d_id_filter, write_arrow_fragments,
                              register_fragment_backend)
-from .quantize import quantize_mxfp8, dequantize_mxfp8, mxfp8_row_bytes
+from .quantize import quantize_mxfp8, quantize_mxfp8_chunked, dequantize_mxfp8, mxfp8_row_bytes
 # names the reference's `data` namespace re-exports from its helpers (python/data/__init__.py star imports)
 from ..partition.partition_book import PartitionBook
 from ..utils import convert_to_tensor, coo_to_csc, coo_to_csr, ptr2ind, share_memory, squeeze

@@ -6,8 +6,18 @@ tables, NVLink), so halving the row size is worth more than any kernel tweak: a 
 
     [ d bytes e4m3 | d/32 bytes UE8M0 scales | zero padding to a multiple of 16 bytes ]
 
-(d = 128: 144 bytes instead of 256).  The fused layer-1 kernel (csrc/cuda/sage_tc.cu, `FP8` loader) and
-`RowTableHandle.gather_mxfp8` de-quantise in registers; everything downstream still sees bf16 / fp32.
+(d = 128: 144 bytes instead of 256; d = 1024: 1056 instead of 2048).  The rows are de-quantised in registers by
+every kernel that reads a feature table, at any d that is a multiple of 32 up to 1024 unless noted:
+
+  k_sage_aggregate            layer-1 neighbour mean of the sampled batch (csrc/cuda/sage.cu): GraphSageEngine's
+                              unfused layer 1 and the heterogeneous engines' per-relation column blocks
+  k_sage_fused3               fused layer-1 gather + GEMM of GraphSageEngine (csrc/cuda/sage_tc.cu), d = 128 only
+  k_gather_mxfp8_vec          `RowTableHandle.gather_mxfp8_into`: rows into a bf16 column block, device-side count
+                              (the engines' self blocks and the attention engines' layer-1 inputs)
+  k_gather_mxfp8              `RowTableHandle.gather_mxfp8`: a fresh dense bf16 [n, d], d a multiple of 128
+  k_sage_full_aggregate       exact full-neighbourhood inference of every engine (csrc/cuda/sage_infer.cu)
+
+Everything downstream still sees bf16 / fp32.
 """
 import torch
 
@@ -43,3 +53,11 @@ def dequantize_mxfp8(rows: torch.Tensor, d: int) -> torch.Tensor:
   e = rows[:, d:d + d // BLOCK].float() - 127.0
   return (q * torch.exp2(e).unsqueeze(2)).view(n, d)
 
+
+def quantize_mxfp8_chunked(x: torch.Tensor, rows: int = 1 << 20) -> torch.Tensor:
+  """`quantize_mxfp8(x)` computed `rows` rows at a time, so that the fp32 temporaries of the quantiser never cover the
+  whole table (a 1024-wide table of 10^7 rows would need 40 GB of them)."""
+  n = x.shape[0]
+  if n <= rows:
+    return quantize_mxfp8(x)
+  return torch.cat([quantize_mxfp8(x[b0:min(n, b0 + rows)]) for b0 in range(0, n, rows)])

@@ -26,6 +26,7 @@ from typing import Dict, List, Optional, Sequence, Tuple, Union
 
 import torch
 
+from ..data.quantize import mxfp8_row_bytes
 from ..ops import require_native
 
 EdgeType = Tuple[str, str, str]
@@ -35,12 +36,39 @@ def _round_up(x, m):
   return (x + m - 1) // m * m
 
 
+def resolve_feature_formats(feature_format, dim_in: Dict[str, int], feature_tables: Dict[str, object]) -> Dict[str, str]:
+  """{node type: 'bf16' | 'mxfp8'} from the engines' `feature_format` argument (one format for every type, or a dict
+  whose missing types are bf16), checked against each type's width and table: an MXFP8 type needs a width that is a
+  multiple of 32 and a uint8 table of `mxfp8_row_bytes(width)`-byte rows (`data.quantize_mxfp8`); a bf16 type must not
+  be handed a uint8 table.  Raises ValueError."""
+  fmt = {}
+  for t, d in dim_in.items():
+    f = feature_format.get(t, 'bf16') if isinstance(feature_format, dict) else feature_format
+    if f not in ('bf16', 'mxfp8'):
+      raise ValueError(f"feature_format of node type {t!r} must be 'bf16' or 'mxfp8' (got {f!r})")
+    tbl = feature_tables[t]
+    if f == 'mxfp8':
+      if d % 32 != 0:
+        raise ValueError(f'MXFP8 features of node type {t!r}: in_dim must be a multiple of 32 (got {d})')
+      if not tbl.is_uint8 or tbl.width != mxfp8_row_bytes(d):
+        raise ValueError(f'MXFP8 features of node type {t!r}: the table must hold uint8 rows of '
+                         f'mxfp8_row_bytes({d}) = {mxfp8_row_bytes(d)} bytes (data.quantize_mxfp8)')
+    elif tbl.is_uint8:
+      raise ValueError(f"node type {t!r} has a uint8 feature table but feature_format 'bf16'; pass "
+                       f"feature_format='mxfp8' (or a dict naming this type) for data.quantize_mxfp8 rows")
+    fmt[t] = f
+  return fmt
+
+
 class HeteroSageEngine(object):
   """Args:
     graphs: {(src, rel, dst): data.Graph} device graphs (single- or multi-shard), CSC by dst for edge_dir='in',
       CSR by src for edge_dir='out'.
-    feature_tables: {node type: native RowTableHandle of bf16 rows indexed by global id} (`UnifiedTensor._table()`,
-      `PartitionedFeature.table`).
+    feature_tables: {node type: native RowTableHandle of rows indexed by global id} (`UnifiedTensor._table()`,
+      `PartitionedFeature.table`): bf16 rows, or `data.quantize_mxfp8` rows for the types `feature_format` names.
+    feature_format: 'bf16', 'mxfp8', or {node type: format} (types left out are bf16; small tables rarely justify
+      quantising).  MXFP8 rows are de-quantised inside the layer-1 aggregation, the gathers and the inference
+      aggregation; every buffer downstream is bf16 as before.  An MXFP8 type needs an in_dim that is a multiple of 32.
     labels: int64 [num_nodes[seed_type]].
     in_dim: feature width (int or {type: int}), a multiple of 8 up to 1024.  The layer-1 operand of each destination
       type (its incoming relations' source widths plus its own) must be a multiple of 64 wide.
@@ -58,7 +86,8 @@ class HeteroSageEngine(object):
                fanouts: Union[Sequence[int], Dict[EdgeType, Sequence[int]]] = (15, 10, 5), batch_size: int = 1024,
                hidden: int = 512, num_classes: int = 19, edge_dir: str = 'in', lr: float = 1e-3,
                weight_decay: float = 0.0, seed: int = 0, device: Optional[torch.device] = None,
-               use_cuda_graph: bool = True, cap_limit: int = 1 << 21, group=None):
+               use_cuda_graph: bool = True, cap_limit: int = 1 << 21, group=None,
+               feature_format: Union[str, Dict[str, str]] = 'bf16'):
     self.nat = require_native()
     self.edge_types = [tuple(e) for e in graphs]
     self.graphs = graphs
@@ -100,6 +129,7 @@ class HeteroSageEngine(object):
     if self.C < 1:
       raise ValueError(f'num_classes must be >= 1 (got {self.C})')
     self.feat = feature_tables
+    self.feature_format = resolve_feature_formats(feature_format, self.dim_in, feature_tables)
     self.labels = labels.to(dev)
     # types that can appear at hop h (static reachability over the schema)
     hop_types = [{self.tid[seed_type]}]
@@ -333,11 +363,19 @@ class HeteroSageEngine(object):
       self._plans[key] = pl
     return pl
 
+  def _gather_feat(self, t: int, ids: torch.Tensor, n_dev: Optional[torch.Tensor], out: torch.Tensor):
+    """out[i, :in_dim] = bf16 feature row ids[i] of type t (MXFP8 tables are de-quantised); rows past the device count
+    `n_dev` are zeros.  One launch."""
+    name = self.ntypes[t]
+    if self.feature_format[name] == 'mxfp8':
+      self.feat[name].gather_mxfp8_into(ids, None, n_dev, out, self.dim_in[name])
+    else:
+      self.feat[name].gather_into(ids, None, n_dev, out)
+
   def _gather_input(self, u: int):
     """Layer-1 input of the attention engines: the feature rows of every sampled node of type u into X0[u]."""
     n = min(self.X0[u].shape[0], self.cap_nodes[u])
-    self.feat[self.ntypes[u]].gather_into(self.arena.nodes_of(u)[:n], None, self._ctr[u][self.L + 1:self.L + 2],
-                                          self.X0[u][:n])
+    self._gather_feat(u, self.arena.nodes_of(u)[:n], self._ctr[u][self.L + 1:self.L + 2], self.X0[u][:n])
     self._k()
 
   def _loss(self, logits: torch.Tensor, dlogits: torch.Tensor, bias_grad: torch.Tensor):
@@ -373,7 +411,7 @@ class HeteroSageEngine(object):
         blk = A[:, self_col:self_col + d]
         if l == 1:
           n = min(A.shape[0], self.cap_nodes[t])
-          self.feat[self.ntypes[t]].gather_into(ar.nodes_of(t)[:n], None, self._ctr[t][nh:nh + 1], blk)
+          self._gather_feat(t, ar.nodes_of(t)[:n], self._ctr[t][nh:nh + 1], blk)
         else:
           blk.copy_(self.Z[l - 1][t][:A.shape[0]])
         self._k()
@@ -544,7 +582,7 @@ class HeteroSageEngine(object):
     """bf16 feature rows [r0, r1) of type t, gathered from its feature table (any memory tier) into buf."""
     d = self.dim_in[self.ntypes[t]]
     x = buf[:(r1 - r0) * d].view(r1 - r0, d)
-    self.feat[self.ntypes[t]].gather_into(self._ids[r0:r1], None, None, x)
+    self._gather_feat(t, self._ids[r0:r1], None, x)
     return x
 
   def _gemm(self, A, W, b, relu, out, idx):
@@ -576,7 +614,7 @@ class HeteroSageEngine(object):
                                     mean_only=True)
         blk = a[:, self_col:K]
         if l == 1:
-          self.feat[self.ntypes[t]].gather_into(self._ids[r0:r1], None, None, blk)
+          self._gather_feat(t, self._ids[r0:r1], None, blk)
         else:
           blk.copy_(X[t][r0:r1])
         self._gemm(a, self.param(('W', l, t)), self.param(('b', l, t)), l < self.L, Z[t][r0:r1], 0)

@@ -49,7 +49,8 @@ class HeteroGatEngine(HeteroSageEngine):
                fanouts: Union[Sequence[int], Dict[EdgeType, Sequence[int]]] = (15, 10, 5), batch_size: int = 1024,
                hidden: int = 512, num_classes: int = 19, heads: int = 4, dropout: float = 0.2, edge_dir: str = 'in',
                lr: float = 1e-3, weight_decay: float = 0.0, seed: int = 0, device: Optional[torch.device] = None,
-               use_cuda_graph: bool = True, cap_limit: int = 1 << 21, group=None):
+               use_cuda_graph: bool = True, cap_limit: int = 1 << 21, group=None,
+               feature_format: Union[str, Dict[str, str]] = 'bf16'):
     self.heads = self._check_heads(heads, hidden)
     self.dropout = float(dropout)
     if not 0.0 <= self.dropout < 1.0:
@@ -58,7 +59,7 @@ class HeteroGatEngine(HeteroSageEngine):
     super().__init__(graphs, feature_tables, labels, in_dim, num_nodes, seed_type, fanouts=fanouts,
                      batch_size=batch_size, hidden=hidden, num_classes=num_classes, edge_dir=edge_dir, lr=lr,
                      weight_decay=weight_decay, seed=seed, device=device, use_cuda_graph=use_cuda_graph,
-                     cap_limit=cap_limit, group=group)
+                     cap_limit=cap_limit, group=group, feature_format=feature_format)
 
   # ------------------------------------------------------------------ buffers / parameters
   def _X(self, l: int, t: int) -> torch.Tensor:

@@ -23,6 +23,7 @@ from ..utils.tracing import nvtx_range
 import torch.nn as nn
 import torch.nn.functional as F
 
+from ..data.quantize import mxfp8_row_bytes
 from ..ops import require_native
 
 
@@ -128,12 +129,17 @@ class GraphSageEngine(object):
     # mask keyed by (seed, layer, optimizer step, element); backward rescales inside sage_gather_bwd.
     assert 0.0 <= float(dropout) < 1.0
     self.dropout = float(dropout)
-    # 'mxfp8': `feature_table` holds data.quantize_mxfp8 rows (uint8, in_dim + 16 bytes); the fused layer-1 kernel
-    # de-quantises in its loaders (half the gather bytes), so the fused path is mandatory for that format
+    # 'mxfp8': `feature_table` holds data.quantize_mxfp8 rows (uint8, mxfp8_row_bytes(in_dim) bytes, in_dim a multiple
+    # of 32), de-quantised inside whichever kernel reads them (half the gather bytes).  Layer 1 runs the fused kernel
+    # where its MXFP8 loader applies (in_dim 128 and a fused-capable shape and table), otherwise sage_aggregate + GEMM.
     assert feature_format in ('bf16', 'mxfp8')
     self.feature_format = feature_format
     if feature_format == 'mxfp8':
-      assert int(in_dim) == 128, 'MXFP8 features: in_dim must be 128'
+      if int(in_dim) % 32 != 0:
+        raise ValueError(f'MXFP8 features: in_dim must be a multiple of 32 (got {in_dim})')
+      if not feature_table.is_uint8 or feature_table.width != mxfp8_row_bytes(int(in_dim)):
+        raise ValueError(f'MXFP8 features: the table must hold uint8 rows of mxfp8_row_bytes({in_dim}) = '
+                         f'{mxfp8_row_bytes(int(in_dim))} bytes (data.quantize_mxfp8)')
       use_fused = True
     self.pipeline = bool(pipeline)
     self.deterministic_sampling = bool(deterministic_sampling)
@@ -193,19 +199,23 @@ class GraphSageEngine(object):
       self._health_host = torch.zeros(2, dtype=torch.int32).pin_memory()
       self._autotune_fused = (use_fused == 'auto')
       # layer 1 also needs a feature table that the fused kernel's 32-bit row handles can address
-      self.fused_ok = [False] + [bool(use_fused and self.nat.sage_fused_supported(
-          self.dims_in[l - 1], self.dims_out[l - 1], self.feat if l == 1 else None)) for l in range(1, self.L + 1)]
+      self.fused_ok = [False] + [bool(use_fused and self._fused_shape(l, self.dims_in[l - 1], self.dims_out[l - 1]))
+                                 for l in range(1, self.L + 1)]
       bf = torch.bfloat16
       self.w_packed = [None] + [torch.zeros(self.dims_out[l - 1] * 2 * self.dims_in[l - 1], dtype=bf, device=dev)
                                 if self.fused_ok[l] else None for l in range(1, self.L + 1)]
       self._repack()
       self._resolve_preagg()
-      if self.feature_format == 'mxfp8' and not self.fused_ok[1]:
-        raise RuntimeError('MXFP8 features need the fused layer-1 kernel (in_dim 128, hidden multiple of 32, <= 256, '
-                           'at most 16 feature parts of fewer than 2^28 rows each)')
     self._graph_fb = None
     self._graph_opt = None
     self._graph_full = None
+
+  def _fused_shape(self, l: int, d: int, n_out: int) -> bool:
+    """Can the fused layer kernel run layer l (input width d, output width n_out)?  Its MXFP8 loader is written for
+    128-wide rows."""
+    if l == 1 and self.feature_format == 'mxfp8' and d != 128:
+      return False
+    return bool(self.nat.sage_fused_supported(d, n_out, self.feat if l == 1 else None))
 
   def _check_widths(self, use_fused):
     """Rejects, at construction, widths that a kernel of the step cannot run (instead of failing at the first step or
@@ -228,8 +238,7 @@ class GraphSageEngine(object):
     if self.hidden % 64 != 0:
       dims_in = [self.in_dim] + [self.hidden] * (self.L - 1)
       for l in range(1, self.L):          # hidden layers (the last layer's output is padded to 64 columns)
-        fused = use_fused != 'auto' and bool(use_fused) and \
-            bool(self.nat.sage_fused_supported(dims_in[l - 1], self.hidden, self.feat if l == 1 else None))
+        fused = use_fused != 'auto' and bool(use_fused) and self._fused_shape(l, dims_in[l - 1], self.hidden)
         if not fused:
           raise ValueError(f'hidden = {self.hidden}: layer {l} runs the unfused forward GEMM, whose output width must '
                            f'be a multiple of 64')

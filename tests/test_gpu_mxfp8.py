@@ -1,0 +1,496 @@
+"""MXFP8 feature tables (data/quantize.py) through every kernel that reads a feature table and through the engines.
+
+The oracle: a de-quantised MXFP8 value (an e4m3 number times a power of two) is exactly a bf16 value, so a bf16 table
+holding `dequantize_mxfp8(q, d)` is an exact twin of the MXFP8 table `q`.  Kernels are checked against float64 over
+the de-quantised rows (and bit for bit where they only convert); engines on MXFP8 tables are checked against the same
+engine on the twin tables, whose kernels have their own float64 tests.
+"""
+import pytest
+import torch
+
+import graphlearn_for_pytorch_b200 as glt
+from graphlearn_for_pytorch_b200.data import dequantize_mxfp8, mxfp8_row_bytes, quantize_mxfp8
+from graphlearn_for_pytorch_b200.models import GraphSageEngine, HeteroGatEngine, HeteroHgtEngine, HeteroSageEngine
+from helpers import bf16_ulp, bound_ratio
+
+pytestmark = pytest.mark.gpu
+DEV = torch.device('cuda', 0)
+SENTINEL = 7.0
+EPS32 = 2.0 ** -23
+# both sides of every lane-group boundary of the MXFP8 dispatch (16 columns = one 16-byte vector of e4m3)
+WIDTHS = [32, 64, 96, 128, 160, 256, 480, 512, 992, 1024]
+
+
+def _quantised(n, d, seed):
+  """(q uint8 [n, row bytes], twin bf16 [n, d]) on the host; blocks of very different magnitude, one all-zero row."""
+  g = torch.Generator().manual_seed(seed)
+  x = torch.randn(n, d, generator=g) * torch.exp2(torch.randint(-6, 7, (n, d // 32), generator=g).float()).repeat_interleave(32, 1)
+  x[n // 2] = 0
+  q = quantize_mxfp8(x)
+  xd = dequantize_mxfp8(q, d)
+  twin = xd.to(torch.bfloat16)
+  assert torch.equal(twin.float(), xd), 'de-quantised MXFP8 values are bf16 values'
+  return q, twin
+
+
+_KEEP = []        # the UnifiedTensors behind the tables handed out by _table
+
+
+def _table(rows, split=False):
+  """RowTableHandle over `rows` (uint8 or bf16, host); split: first part in HBM, the rest in pinned host memory."""
+  ut = glt.data.UnifiedTensor(0, rows.dtype)
+  if split:
+    ut.append_shared_tensor(rows[:rows.shape[0] // 3].to(DEV))
+    ut.append_cpu_tensor(rows[rows.shape[0] // 3:].clone())
+  else:
+    ut.append_shared_tensor(rows.to(DEV))
+  _KEEP.append(ut)
+  return ut._table()
+
+
+# --------------------------------------------------------------------------- gather_mxfp8_into
+@pytest.mark.parametrize('d', WIDTHS)
+def test_gather_mxfp8_into_is_bit_exact(native, d):
+  N = 3000
+  q, twin = _quantised(N, d, seed=d)
+  twin = twin.to(DEV)
+  zero = torch.zeros(1, d, dtype=torch.bfloat16, device=DEV)
+  ref_rows = torch.cat([twin, zero])                      # row N = the zero row of invalid ids
+  g = torch.Generator().manual_seed(d + 1)
+  for split in (False, True):
+    tbl = _table(q, split)
+    # small and large launch shape (the latter keeps four rows in flight per lane group), with negative ids
+    for n in (777, 140001):
+      ids = torch.randint(0, N, (n,), generator=g)
+      ids[::13] = -1
+      out = torch.full((n, d), SENTINEL, dtype=torch.bfloat16, device=DEV)
+      tbl.gather_mxfp8_into(ids.to(DEV), None, None, out, d)
+      torch.cuda.synchronize()
+      assert torch.equal(out, ref_rows[torch.where(ids < 0, N, ids).to(DEV)]), (d, split, n)
+    # a column block of a wider buffer, a device count below n: tail rows are zeros, other columns untouched
+    n, n_valid, col = 500, 463, 16
+    ids = torch.randint(0, N, (n,), generator=g).to(DEV)
+    buf = torch.full((n + 5, d + 48), SENTINEL, dtype=torch.bfloat16, device=DEV)
+    tbl.gather_mxfp8_into(ids, None, torch.tensor([n_valid], dtype=torch.int32, device=DEV), buf[:, col:col + d], d)
+    torch.cuda.synchronize()
+    assert torch.equal(buf[:n_valid, col:col + d], twin[ids[:n_valid]])
+    assert bool((buf[n_valid:n, col:col + d] == 0).all()) and bool((buf[n:] == SENTINEL).all())
+    assert bool((buf[:, :col] == SENTINEL).all()) and bool((buf[:, col + d:] == SENTINEL).all())
+    # id2index: ids beyond the map and ids it maps to -1 give zero rows
+    M = 4000
+    id2index = torch.full((M,), -1, dtype=torch.int64)
+    id2index[torch.randperm(M, generator=g)[:N]] = torch.arange(N)
+    ids = torch.randint(0, M + 500, (n,), generator=g)
+    out = torch.full((n, d), SENTINEL, dtype=torch.bfloat16, device=DEV)
+    tbl.gather_mxfp8_into(ids.to(DEV), id2index.to(DEV), None, out, d)
+    torch.cuda.synchronize()
+    mapped = torch.where(ids < M, id2index[ids.clamp(max=M - 1)], torch.full_like(ids, -1))
+    assert int((mapped < 0).sum()) > 0
+    assert torch.equal(out, ref_rows[torch.where(mapped < 0, N, mapped).to(DEV)])
+
+
+# --------------------------------------------------------------------------- sage_aggregate / sage_aggregate_block
+HOPS = [(3, 512), (50, 7), (400, 3)]          # (rows, k): a hub hop, then two ordinary hops
+
+
+def _structure(n_src, seed):
+  """Per-hop ELL blocks over sources [0, n_src): the first rows of each hop have degree 0, 1 and k; slots past a row's
+  degree hold valid ids that must not be read; some slots inside the degree hold -1 (a neighbour the sampler dropped:
+  it adds nothing but still counts in the mean's divisor)."""
+  g = torch.Generator().manual_seed(seed)
+  cum, degs, ells = [0], [], []
+  for rows, k in HOPS:
+    deg = torch.randint(0, k + 1, (rows,), generator=g)
+    deg[:3] = torch.tensor([0, 1, k])
+    ell = torch.randint(0, n_src, (rows, k), generator=g)
+    ell[torch.rand(rows, k, generator=g) < 0.05] = -1
+    ells.append(ell.to(torch.int32))
+    degs.append(deg.to(torch.int32))
+    cum.append(cum[-1] + rows)
+  return cum, torch.cat(degs), ells
+
+
+def _edges(cum, deg, ells, T):
+  tg, sr = [], []
+  for h, (rows, k) in enumerate(HOPS):
+    n = max(0, min(T, cum[h + 1]) - cum[h])
+    if n == 0:
+      continue
+    e = ells[h][:n].long()
+    m = (torch.arange(k).unsqueeze(0) < deg[cum[h]:cum[h] + n].long().unsqueeze(1)) & (e >= 0)
+    tg.append((torch.arange(n).unsqueeze(1) + cum[h]).expand(n, k)[m])
+    sr.append(e[m])
+  return torch.cat(tg).to(DEV), torch.cat(sr).to(DEV)
+
+
+def _counters(cum, total=None):
+  c = torch.zeros(16, dtype=torch.int32)
+  c[:len(cum)] = torch.tensor(cum, dtype=torch.int32)
+  if total is not None:
+    c[len(cum) - 1] = total
+  return c.to(DEV)
+
+
+@pytest.mark.parametrize('block', [False, True])
+@pytest.mark.parametrize('d', WIDTHS)
+def test_sage_aggregate_on_mxfp8_matches_fp64_mean_and_the_bf16_twin(native, d, block):
+  n_src = 600
+  cum, deg, ells = _structure(n_src, seed=d)
+  ell, ks, deg_d = [e.flatten().to(DEV) for e in ells], [k for _, k in HOPS], deg.to(DEV)
+  n_glob = n_src + 97
+  q, twin = _quantised(n_glob, d, seed=d + 1)
+  nodes = torch.randperm(n_glob, generator=torch.Generator().manual_seed(d + 2))[:n_src].to(DEV)
+  feat8, feat16 = _table(q, split=True), _table(twin, split=True)
+  X = twin.to(DEV)[nodes]
+  Xd = X.double()
+  for cap, total in ((cum[-1] + 37, None), (cum[-1] - 20, cum[-1] + 1000)):   # spare rows; counters above the capacity
+    ctr = _counters(cum, total)
+    T = min(cum[-1] if total is None else total, cap)
+    ld, mcol = (2 * d + 24, 16) if block else (2 * d, 0)
+    outs = []
+    for feat in (feat8, feat16):
+      out = torch.full((cap, ld), SENTINEL, dtype=torch.bfloat16, device=DEV)
+      if block:
+        native.sage_aggregate_block(feat, nodes, None, d, ctr, 3, ell, ks, deg_d, out, mcol)
+      else:
+        native.sage_aggregate(feat, nodes, None, d, ctr, 3, ell, ks, deg_d, out)
+      outs.append(out)
+    torch.cuda.synchronize()
+    out, out16 = outs
+    tg, sr = _edges(cum, deg, ells, T)
+    s = torch.zeros(T, d, dtype=torch.float64, device=DEV).index_add_(0, tg, Xd[sr])
+    a = torch.zeros(T, d, dtype=torch.float64, device=DEV).index_add_(0, tg, Xd[sr].abs())
+    dg = deg[:T].to(DEV).double().unsqueeze(1)
+    ref = s / dg.clamp(min=1)
+    bound = torch.where(dg > 0, bf16_ulp(ref) + (dg + 2) * EPS32 * a / dg.clamp(min=1), torch.zeros_like(ref))
+    r = bound_ratio(out[:T, mcol:mcol + d], ref, bound)
+    assert r <= 1.0, (d, block, cap, r)
+    assert bound_ratio(out[:T, mcol:mcol + d], out16[:T, mcol:mcol + d].double(), bf16_ulp(ref)) <= 1.0
+    if not block:
+      assert torch.equal(out[:T, d:], X[:T]), 'self half must be the de-quantised row, bit for bit'
+    else:
+      assert bool((out[:, :mcol] == SENTINEL).all()) and bool((out[:, mcol + d:] == SENTINEL).all())
+    assert bool((out[T:] == SENTINEL).all()), 'rows at and above T must not be written'
+
+
+# --------------------------------------------------------------------------- sage_full_aggregate
+def _csr_graph(n_dst, n_src, seed, hub_deg=600):
+  """CSR rows 0..3 of degree 0, 1, 40 and hub_deg (above the 256 of the whole-CTA path, with repeated ids), the rest
+  random <= 12; the last 20 rows are isolated."""
+  g = torch.Generator().manual_seed(seed)
+  deg = torch.randint(0, 13, (n_dst,), generator=g)
+  deg[:4] = torch.tensor([0, 1, 40, hub_deg])
+  deg[-20:] = 0
+  dst = torch.repeat_interleave(torch.arange(n_dst), deg)
+  src = torch.randint(0, n_src, (int(deg.sum()),), generator=g)
+  topo = glt.data.Topology(torch.stack([src, dst]).to(DEV), layout='CSC', num_nodes=n_dst)
+  graph = glt.data.Graph(topo, 'CUDA', 0)
+  graph.lazy_init()
+  graph._keep = topo
+  indptr = topo.indptr.to(DEV)
+  d_ = torch.repeat_interleave(torch.arange(n_dst, device=DEV), indptr[1:] - indptr[:-1])
+  return graph, indptr, d_, topo.indices.to(DEV).long()
+
+
+@pytest.mark.parametrize('mean_only', [False, True])
+@pytest.mark.parametrize('d', WIDTHS)
+def test_sage_full_aggregate_on_mxfp8_matches_fp64_and_is_chunk_invariant(native, d, mean_only):
+  n_dst, n_src = 300, 700
+  graph, indptr, dst, src = _csr_graph(n_dst, n_src, seed=d)
+  q, twin = _quantised(n_src, d, seed=d + 5)
+  feat = _table(q, split=True)
+  Xd = twin.to(DEV).double()
+  W = d if mean_only else 2 * d
+
+  def run(chunk):
+    out = torch.full((n_dst, W + 8), SENTINEL, dtype=torch.bfloat16, device=DEV)
+    for r0 in range(0, n_dst, chunk):
+      r1 = min(n_dst, r0 + chunk)
+      native.sage_full_aggregate(graph.graph_handler, feat, None, 0, 0, d, r0, r1, False, None, False, out[r0:r1],
+                                 mean_only=mean_only)
+    torch.cuda.synchronize()
+    return out
+
+  out = run(n_dst)
+  assert torch.equal(out, run(n_dst)) and torch.equal(out, run(77)), 'bitwise repeatable and chunk invariant'
+  deg = (indptr[1:] - indptr[:-1]).double().unsqueeze(1)
+  s = torch.zeros(n_dst, d, dtype=torch.float64, device=DEV).index_add_(0, dst, Xd[src])
+  a = torch.zeros(n_dst, d, dtype=torch.float64, device=DEV).index_add_(0, dst, Xd[src].abs())
+  ref = s / deg.clamp(min=1)
+  bound = torch.where(deg > 0, bf16_ulp(ref) + (deg + 2) * EPS32 * a / deg.clamp(min=1), torch.zeros_like(ref))
+  assert bound_ratio(out[:, :d], ref, bound) <= 1.0
+  assert bool((out[:, W:] == SENTINEL).all())
+  if not mean_only:
+    assert torch.equal(out[:, d:2 * d], twin.to(DEV)[:n_dst]), 'self half must be the de-quantised row, bit for bit'
+  if d == 128:
+    # rows up to 256 neighbours: a sequential fp32 sum in CSR order, times the fp32 1/deg, rounded once
+    ptr = indptr.tolist()
+    X32 = twin.to(DEV).float()
+    for r in range(n_dst):
+      n = ptr[r + 1] - ptr[r]
+      if n == 0 or n > 256:
+        continue
+      acc = torch.zeros(d, device=DEV)
+      for u in src[ptr[r]:ptr[r + 1]].tolist():
+        acc = acc + X32[u]
+      inv = torch.tensor(1.0, device=DEV) / torch.tensor(float(n), device=DEV)
+      assert torch.equal(out[r, :d], (acc * inv).to(torch.bfloat16)), r
+
+
+# --------------------------------------------------------------------------- rejections
+def test_bindings_reject_wrong_widths_with_one_message(native):
+  q, twin = _quantised(64, 128, seed=0)
+  tbl = _table(q)
+  ids = torch.arange(8, device=DEV)
+  out = torch.zeros(8, 128, dtype=torch.bfloat16, device=DEV)
+  with pytest.raises(RuntimeError, match='multiple of 32'):
+    tbl.gather_mxfp8_into(ids, None, None, torch.zeros(8, 112, dtype=torch.bfloat16, device=DEV), 112)
+  with pytest.raises(RuntimeError, match='mxfp8_row_bytes'):
+    tbl.gather_mxfp8_into(ids, None, None, torch.zeros(8, 256, dtype=torch.bfloat16, device=DEV), 256)
+  with pytest.raises(RuntimeError, match='mxfp8_row_bytes'):
+    _table(twin).gather_mxfp8_into(ids, None, None, out, 128)
+  with pytest.raises(RuntimeError, match='destination must be bf16'):
+    tbl.gather_mxfp8_into(ids, None, None, out[:, :96], 128)
+  ctr = _counters([0, 8])
+  ell, deg = torch.zeros(8 * 2, dtype=torch.int32, device=DEV), torch.ones(8, dtype=torch.int32, device=DEV)
+  with pytest.raises(RuntimeError, match='feature width mismatch'):
+    native.sage_aggregate(tbl, ids, None, 256, ctr, 1, [ell], [2], deg, torch.zeros(8, 512, dtype=torch.bfloat16, device=DEV))
+  with pytest.raises(RuntimeError, match='feature width mismatch'):
+    native.sage_aggregate_block(tbl, ids, None, 96, ctr, 1, [ell], [2], deg,
+                                torch.zeros(8, 192, dtype=torch.bfloat16, device=DEV), 0)
+  graph, _, _, _ = _csr_graph(40, 64, seed=1, hub_deg=5)
+  with pytest.raises(RuntimeError, match='feature width mismatch'):
+    native.sage_full_aggregate(graph.graph_handler, tbl, None, 0, 0, 64, 0, 40, False, None, False,
+                               torch.zeros(40, 128, dtype=torch.bfloat16, device=DEV), mean_only=False)
+
+
+# --------------------------------------------------------------------------- heterogeneous engines
+SIZES = {'paper': 2000, 'author': 1000, 'inst': 100, 'fos': 150}
+DIMS = {'paper': 1024, 'author': 256, 'inst': 64, 'fos': 128}        # IGBH-like: wide papers, narrow small types
+FORMATS = {'paper': 'mxfp8', 'author': 'mxfp8', 'fos': 'mxfp8'}       # 'inst' stays bf16
+CLASSES = 8
+ENGINES = {'rsage': HeteroSageEngine, 'rgat': HeteroGatEngine, 'hgt': HeteroHgtEngine}
+
+
+def _hetero_edges(seed=0, max_deg=6):
+  """Every type has an incoming relation; unique edges with in-degree <= max_deg, so that a fan-out of max_deg takes
+  every neighbour and two engines with the same seed sample the same batch."""
+  g = torch.Generator().manual_seed(seed)
+
+  def rnd(s, t, m):
+    ei = torch.stack([torch.randint(0, SIZES[s], (m,), generator=g), torch.randint(0, SIZES[t], (m,), generator=g)])
+    ei = torch.unique(ei[:, ~((ei[0] == ei[1]) & (s == t))], dim=1)
+    ei = ei[:, torch.argsort(ei[1], stable=True)]
+    first = torch.searchsorted(ei[1].contiguous(), ei[1].contiguous())
+    return ei[:, (torch.arange(ei.shape[1]) - first) < max_deg]
+  writes, topic = rnd('author', 'paper', 5000), rnd('fos', 'paper', 3000)
+  return {('paper', 'cites', 'paper'): rnd('paper', 'paper', 7000),
+          ('author', 'writes', 'paper'): writes,
+          ('paper', 'rev_writes', 'author'): rnd('paper', 'author', 3000),
+          ('inst', 'employs', 'author'): rnd('inst', 'author', 1500),
+          ('author', 'affiliated_with', 'inst'): rnd('author', 'inst', 500),
+          ('fos', 'topic', 'paper'): topic,
+          ('paper', 'rev_topic', 'fos'): rnd('paper', 'fos', 600)}
+
+
+class _Hetero:
+  """Graphs, learnable labels, and per type the MXFP8 table (types of FORMATS) and its exact bf16 twin table."""
+
+  def __init__(self, split_host=False):
+    self.graphs = {}
+    for et, ei in _hetero_edges().items():
+      self.graphs[et] = glt.data.Graph(glt.data.Topology(ei.to(DEV), layout='CSC', num_nodes=SIZES[et[2]]), 'CUDA', 0)
+    g = torch.Generator().manual_seed(5)
+    self.t8, self.t16 = {}, {}
+    for t in SIZES:
+      x = torch.randn(SIZES[t], DIMS[t], generator=g)
+      if t in FORMATS:
+        q, twin = quantize_mxfp8(x), None
+        twin = dequantize_mxfp8(q, DIMS[t]).to(torch.bfloat16)
+        self.t8[t], self.t16[t] = _table(q, split_host), _table(twin, split_host)
+      else:
+        self.t8[t] = self.t16[t] = _table(x.to(torch.bfloat16), split_host)
+      if t == 'paper':
+        self.labels = (twin.float() @ torch.randn(DIMS[t], CLASSES, generator=g)).argmax(1).to(DEV)
+
+  def engine(self, kind, mxfp8, use_graph=False, fan=(6, 6, 6), **kw):
+    args = dict(fanouts=list(fan), batch_size=128, hidden=128, num_classes=CLASSES, edge_dir='in', lr=5e-3, seed=1,
+                device=DEV, use_cuda_graph=use_graph)
+    if kind != 'rsage':
+      args['heads'] = 4
+    if kind == 'rgat':
+      args['dropout'] = 0.0        # its mask is keyed by local row, which two runs of one batch assign differently
+    args.update(kw)
+    eng = ENGINES[kind](self.graphs, self.t8 if mxfp8 else self.t16, self.labels, dict(DIMS), dict(SIZES), 'paper',
+                        feature_format=dict(FORMATS) if mxfp8 else 'bf16', **args)
+    eng._keep = self
+    return eng
+
+
+@pytest.fixture(scope='module')
+def hetero():
+  return _Hetero(split_host=True)
+
+
+def _by_global_id(eng, t, buf, n_hops):
+  """Rows of a per-type batch buffer in ascending global-id order (local ids are assigned in arrival order)."""
+  n = int(eng._ctr[t][n_hops].item())
+  ids = eng.arena.nodes_of(t)[:n]
+  o = torch.argsort(ids)
+  return ids[o], buf[:n][o]
+
+
+def _grad_close(ga, gb):
+  """Two runs of one step differ by the arrival order of fp32 atomics (split-K weight gradients, column sums)."""
+  tol = 2e-2 * float(gb.abs().max()) + 1e-7
+  assert float((ga - gb).abs().max()) <= tol, (float((ga - gb).abs().max()), tol)
+
+
+@pytest.mark.parametrize('kind', list(ENGINES))
+def test_hetero_engine_step_on_mxfp8_matches_the_bf16_twin(native, hetero, kind):
+  e8, e16 = hetero.engine(kind, True), hetero.engine(kind, False)
+  assert e8.feature_format == {'paper': 'mxfp8', 'author': 'mxfp8', 'fos': 'mxfp8', 'inst': 'bf16'}
+  assert torch.equal(e8.p32, e16.p32)
+  seeds = torch.randperm(SIZES['paper'], generator=torch.Generator().manual_seed(3))[:128].to(DEV)
+  l8, l16 = float(e8.train_step(seeds).item()), float(e16.train_step(seeds).item())
+  torch.cuda.synchronize()
+  for t in range(len(e8.ntypes)):
+    if kind == 'rsage':
+      if t not in e8.targets[1]:
+        continue
+      (i8, a8), (i16, a16) = _by_global_id(e8, t, e8.A[1][t], e8.L), _by_global_id(e16, t, e16.A[1][t], e16.L)
+      assert torch.equal(i8, i16) and i8.numel() > 0
+      assert bound_ratio(a8, a16.double(), bf16_ulp(a16.double())) <= 1.0, e8.ntypes[t]
+    elif t in e8.X0:
+      (i8, x8), (i16, x16) = _by_global_id(e8, t, e8.X0[t], e8.L + 1), _by_global_id(e16, t, e16.X0[t], e16.L + 1)
+      assert torch.equal(i8, i16) and i8.numel() > 0
+      assert torch.equal(x8, x16), e8.ntypes[t]
+  assert abs(l8 - l16) <= 1e-3 * max(1.0, abs(l16)), (l8, l16)
+  for name in e8.param_index:                     # every weight and bias gradient
+    _grad_close(e8._p32(name, True), e16._p32(name, True))
+
+
+@pytest.mark.parametrize('kind', list(ENGINES))
+def test_hetero_engine_on_mxfp8_replays_its_eager_step_with_the_same_launch_count(native, hetero, kind):
+  eng = hetero.engine(kind, True, use_graph=True)
+  eng.warmup_and_capture(n_eager=1)
+  assert eng._graph is not None
+  twin = hetero.engine(kind, False)
+  twin.warmup_and_capture(n_eager=1)
+  assert eng.kernels_per_step == twin.kernels_per_step > 0
+  seeds = torch.randperm(SIZES['paper'], generator=torch.Generator().manual_seed(4))[:128].to(DEV)
+  saved = eng.state_dict()
+  graph, eng._graph = eng._graph, None
+  l_eager = float(eng.train_step(seeds).item())
+  g_eager = eng.g32.clone()
+  eng.load_state_dict(saved)
+  eng._graph = graph
+  l_graph = float(eng.train_step(seeds).item())
+  assert abs(l_graph - l_eager) <= 1e-3 * max(1.0, abs(l_eager)), (l_graph, l_eager)
+  _grad_close(eng.g32, g_eager)
+  loss, correct, n = eng.evaluate_batch(seeds)
+  assert n == 128 and 0 <= correct <= n and loss == loss
+  eng.close()
+
+
+@pytest.mark.parametrize('kind', list(ENGINES))
+def test_hetero_inference_on_mxfp8_matches_the_twin_and_is_chunk_invariant(native, hetero, kind):
+  e8, e16 = hetero.engine(kind, True), hetero.engine(kind, False)
+  a = e8.inference()
+  assert a.shape == (SIZES['paper'], CLASSES)
+  assert torch.equal(a, e8.inference()) and torch.equal(a, e8.inference(chunk_rows=333))
+  b = e16.inference()
+  torch.testing.assert_close(a.float(), b.float(), rtol=2e-2, atol=2e-2)
+  assert float((a.float().argmax(1) == b.float().argmax(1)).float().mean()) >= 0.99
+
+
+@pytest.mark.parametrize('kind', list(ENGINES))
+def test_hetero_engine_learns_on_mxfp8_like_on_bf16(native, hetero, kind):
+  accs = {}
+  for name, mx in (('mxfp8', True), ('bf16', False)):
+    eng = hetero.engine(kind, mx, use_graph=True, fan=(4, 3, 2), lr=5e-3 if kind == 'hgt' else 1e-2)
+    eng.warmup_and_capture(n_eager=1)
+    g = torch.Generator().manual_seed(0)
+    for _ in range(400 if kind == 'hgt' else 200):
+      eng.train_step(torch.randperm(SIZES['paper'], generator=g)[:128].to(DEV))
+    correct = total = 0
+    for i in range(8):
+      _, c, n = eng.evaluate_batch(torch.arange(i * 128, (i + 1) * 128, device=DEV))
+      correct, total = correct + c, total + n
+    accs[name] = correct / total
+    eng.close()
+  print(kind, accs)
+  assert accs['bf16'] > 1.5 / CLASSES and accs['mxfp8'] > accs['bf16'] - 0.08, accs
+
+
+def test_hetero_engine_rejects_mismatched_formats(native, hetero):
+  with pytest.raises(ValueError, match='uint8 feature table'):
+    ENGINES['rsage'](hetero.graphs, hetero.t8, hetero.labels, dict(DIMS), dict(SIZES), 'paper', device=DEV)
+  with pytest.raises(ValueError, match='mxfp8_row_bytes'):
+    ENGINES['rsage'](hetero.graphs, hetero.t16, hetero.labels, dict(DIMS), dict(SIZES), 'paper', device=DEV,
+                     feature_format='mxfp8')
+  with pytest.raises(ValueError, match="'bf16' or 'mxfp8'"):
+    ENGINES['rgat'](hetero.graphs, hetero.t16, hetero.labels, dict(DIMS), dict(SIZES), 'paper', device=DEV,
+                    feature_format={'paper': 'fp8'})
+
+
+# --------------------------------------------------------------------------- GraphSageEngine
+def _homo(in_dim, hidden, seed=0):
+  from graphlearn_for_pytorch_b200.utils.synthetic import rmat_edges
+  N = 6000
+  ei = rmat_edges(N, 30000, seed=seed, device=DEV)
+  ei = torch.cat([ei, ei.flip(0)], 1)
+  graph = glt.data.Graph(glt.data.Topology(ei, layout='CSR', num_nodes=N), 'CUDA', 0)
+  g = torch.Generator().manual_seed(seed + 1)
+  q = quantize_mxfp8(torch.randn(N, in_dim, generator=g))
+  twin = dequantize_mxfp8(q, in_dim).to(torch.bfloat16)
+  labels = torch.randint(0, 10, (N,), generator=g).to(DEV)
+
+  def make(mxfp8, **kw):
+    args = dict(fanouts=[4, 3], batch_size=128, hidden=hidden, num_classes=10, device=DEV, seed=2,
+                use_cuda_graph=False, deterministic_sampling=True)
+    args.update(kw)
+    eng = GraphSageEngine(graph, _table(q if mxfp8 else twin), labels, in_dim=in_dim, num_nodes=N,
+                          feature_format='mxfp8' if mxfp8 else 'bf16', **args)
+    eng._keep = graph
+    return eng
+  return make, N
+
+
+@pytest.mark.parametrize('in_dim,hidden', [(256, 128), (128, 512), (96, 64)])
+def test_graphsage_engine_on_mxfp8_runs_layer_1_unfused_where_the_fused_kernel_cannot(native, in_dim, hidden):
+  make, N = _homo(in_dim, hidden)
+  seeds = torch.randperm(N, generator=torch.Generator().manual_seed(1))[:128].to(DEV)
+  for pipeline in (False, True):
+    e8, e16 = make(True, pipeline=pipeline), make(False, pipeline=pipeline)
+    assert not e8.fused_ok[1] and e8.preaggregate == pipeline
+    if not pipeline:                          # identical parameters: the logits differ by bf16 roundings at most
+      a, b = e8.inference(), e16.inference()
+      assert torch.equal(a, e8.inference(chunk_rows=1001))
+      torch.testing.assert_close(a.float(), b.float(), rtol=3e-2, atol=3e-2)
+    if pipeline:
+      e8.warmup_and_capture(n_eager=1)
+      e16.warmup_and_capture(n_eager=1)
+    assert e8.kernels_per_step == e16.kernels_per_step
+    # (a pipelined engine samples and pre-aggregates the batch in its first call and trains it in flush())
+    l8, l16 = [float((e.flush() if e.train_step(seeds) is None else e.loss).item()) for e in (e8, e16)]
+    torch.cuda.synchronize()
+    assert abs(l8 - l16) <= 1e-3 * max(1.0, abs(l16)), (pipeline, l8, l16)
+    if not pipeline:
+      T = int(e8.arena.counters[e8.L].item())
+      assert T == int(e16.arena.counters[e16.L].item()) and torch.equal(e8.arena.nodes[:T], e16.arena.nodes[:T])
+      assert bound_ratio(e8.A[1][:T], e16.A[1][:T].double(), bf16_ulp(e16.A[1][:T].double())) <= 1.0
+      _grad_close(e8.g32, e16.g32)
+      e8.regrow(1.2)
+      assert torch.isfinite(e8.train_step(seeds)).all()
+
+
+def test_graphsage_engine_on_mxfp8_keeps_the_fused_layer_at_128_by_256(native):
+  make, N = _homo(128, 256)
+  eng = make(True)
+  assert eng.fused_ok[1] and not eng.preaggregate
+  assert torch.isfinite(eng.train_step(torch.arange(128, device=DEV))).all()
+  with pytest.raises(ValueError, match='multiple of 32'):
+    GraphSageEngine(None, eng.feat, eng.labels, in_dim=72, num_nodes=N, feature_format='mxfp8')
+  with pytest.raises(ValueError, match='mxfp8_row_bytes'):
+    GraphSageEngine(None, eng.feat, eng.labels, in_dim=256, num_nodes=N, feature_format='mxfp8')
