@@ -807,10 +807,19 @@ static void fill_ell(const std::vector<Tensor>& ell, const std::vector<int64_t>&
   for (size_t i = 0; i < ell.size(); ++i) { out_ell[i] = ell[i].data_ptr<int32_t>(); out_k[i] = ks[i]; }
 }
 
-// The aggregation / scatter kernels cover at most 128 16-byte vectors per row (csrc/cuda/sage.cu, GLT_DISPATCH_WIDTH).
+// The aggregation / scatter kernels cover at most 128 16-byte vectors per row, i.e. 1024 bf16 columns (the lane-group
+// dispatch, dispatch_lanes in csrc/cuda/launch_utils.h).
 // `msg` is one string: a TORCH_CHECK message assembled from several arguments crashes this extension when thrown.
 static void check_sage_width(int64_t d, const char* msg) {
   TORCH_CHECK(d % 8 == 0 && d >= 8 && d <= 1024, msg);
+}
+
+// A layer-1 feature table of width d: bf16 rows d wide, or MXFP8 rows of mxfp8_row_bytes(d) bytes.
+static void check_feature_table(const RowTableHandle* feat, int64_t d) {
+  TORCH_CHECK(feat->dtype == torch::kBFloat16 || feat->dtype == torch::kUInt8,
+              "engine features must be bf16 rows or MXFP8 (uint8) rows");
+  TORCH_CHECK(feat->dtype == torch::kBFloat16 ? feat->width == d : feat->holds_mxfp8(d),
+              "feature width mismatch (bf16 rows are d wide; MXFP8 rows are mxfp8_row_bytes(d) bytes, d a multiple of 32 in [32, 1024])");
 }
 
 static SageAggArgs make_agg(RowTableHandle* feat, const c10::optional<Tensor>& nodes,
@@ -823,10 +832,7 @@ static SageAggArgs make_agg(RowTableHandle* feat, const c10::optional<Tensor>& n
     a.src_local = src_local->data_ptr();
   } else {
     TORCH_CHECK(feat != nullptr && nodes.has_value(), "layer-1 aggregation needs a feature table + nodes");
-    TORCH_CHECK(feat->dtype == torch::kBFloat16 || feat->dtype == torch::kUInt8,
-                "engine features must be bf16 rows or MXFP8 (uint8) rows");
-    TORCH_CHECK(feat->dtype == torch::kBFloat16 ? feat->width == d : feat->holds_mxfp8(d),
-                "feature width mismatch (bf16 rows are d wide; MXFP8 rows are mxfp8_row_bytes(d) bytes, d a multiple of 32 in [32, 1024])");
+    check_feature_table(feat, d);
     a.feat = feat->tbl;
     a.feat_fp8 = feat->dtype == torch::kUInt8 ? 1 : 0;
     a.nodes = nodes->data_ptr<int64_t>();
@@ -936,10 +942,7 @@ static void sage_full_aggregate(GraphHandle* graph, RowTableHandle* feat, const 
   } else {
     TORCH_CHECK(!combine, "sage_full_aggregate: combine reads a dense src table");
     TORCH_CHECK(feat != nullptr, "sage_full_aggregate: needs a feature table or a src table");
-    TORCH_CHECK(feat->dtype == torch::kBFloat16 || feat->dtype == torch::kUInt8,
-                "engine features must be bf16 rows or MXFP8 (uint8) rows");
-    TORCH_CHECK(feat->dtype == torch::kBFloat16 ? feat->width == d : feat->holds_mxfp8(d),
-                "feature width mismatch (bf16 rows are d wide; MXFP8 rows are mxfp8_row_bytes(d) bytes, d a multiple of 32 in [32, 1024])");
+    check_feature_table(feat, d);
     a.feat = feat->tbl;
     a.feat_fp8 = feat->dtype == torch::kUInt8 ? 1 : 0;
   }
@@ -1026,8 +1029,9 @@ static int64_t relu_bwd_cast(const Tensor& dH, const Tensor& Z, const Tensor& co
 }
 
 // ---- relational GAT (cuda/gat.cu) -------------------------------------------------------------------------------
-// H = heads * C must be a multiple of 64 in [64, 1024] with C a multiple of 8 (one 16-byte vector never straddles two
-// heads).  Messages are single strings (see check_sage_width).
+// H = heads * C must be a multiple of 64 in [64, 1024] (the lane-group dispatch covers 1024 columns, see
+// check_sage_width) with C a multiple of 8 (one 16-byte vector never straddles two heads).  Messages are single
+// strings (see check_sage_width).
 static void check_gat_width(int64_t H, int64_t heads) {
   TORCH_CHECK(H % 64 == 0 && H >= 64 && H <= 1024 && heads >= 1 && H % heads == 0 && (H / heads) % 8 == 0,
               "gat: H must be a multiple of 64 in [64, 1024] and heads must divide H into head widths C with C % 8 == 0");

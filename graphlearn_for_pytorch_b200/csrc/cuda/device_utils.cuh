@@ -187,4 +187,45 @@ __device__ __forceinline__ const uint8_t* row_ptr(const RowTable& t, int64_t row
   return nullptr;
 }
 
+// Target row t of a sampled batch -> (hop, row inside that hop's ELL block), from the cumulative per-hop counters
+// cum[0..n_hops].
+struct HopLoc { int hop; int row; };
+
+__device__ __forceinline__ HopLoc locate_hop(const int32_t* cum, int n_hops, int t) {
+  HopLoc l; l.hop = 0; l.row = t;
+#pragma unroll 1
+  for (int h = 0; h < n_hops; ++h) {
+    const int b = cum[h], e = cum[h + 1];
+    if (t >= b && t < e) { l.hop = h; l.row = t - b; break; }
+  }
+  return l;
+}
+
+// Source row s of a GraphSAGE aggregation: the dense bf16 activation of the previous layer, or the feature table row of
+// batch node s (layer 1).
+__device__ __forceinline__ const uint8_t* src_row(const SageAggArgs& a, int s) {
+  if (a.src_local) return reinterpret_cast<const uint8_t*>(a.src_local) + static_cast<int64_t>(s) * a.d * 2;
+  return row_ptr(a.feat, a.nodes[s]);
+}
+
+// dst[0..8) += v[0..8) as two 16-byte vector atomics (red.global.add.v4.f32; dst 16-byte aligned).
+__device__ __forceinline__ void red_add8(float* dst, const float* v) {
+  atomicAdd(reinterpret_cast<float4*>(dst), make_float4(v[0], v[1], v[2], v[3]));
+  atomicAdd(reinterpret_cast<float4*>(dst + 4), make_float4(v[4], v[5], v[6], v[7]));
+}
+
+__device__ __forceinline__ float leaky(float x, float slope) { return x > 0.f ? x : x * slope; }
+
+// Random bits of 16-byte vector i (8 bf16 elements) of a dropout mask: a pure function of (seed, layer, optimizer
+// step, i), so a replayed step draws the same mask and a backward can regenerate it.  Element q is kept when 16-bit
+// half (q & 1) of word q >> 1 is >= the caller's threshold.
+__device__ __forceinline__ U4 dropout_bits(uint64_t seed, int layer, uint32_t step, int64_t i) {
+  U4 c;
+  c.x = static_cast<uint32_t>(i);
+  c.y = static_cast<uint32_t>(i >> 32);
+  c.z = step;
+  c.w = 0xD509u + static_cast<uint32_t>(layer);
+  return philox4x32_10(static_cast<uint32_t>(seed), static_cast<uint32_t>(seed >> 32), c);
+}
+
 }  // namespace glt

@@ -20,30 +20,12 @@ namespace glt {
 
 namespace {
 
-struct GatHopLoc { int hop; int row; };
-
-__device__ __forceinline__ GatHopLoc gat_locate(const int32_t* cum, int n_hops, int t) {
-  GatHopLoc l; l.hop = 0; l.row = t;
-#pragma unroll 1
-  for (int h = 0; h < n_hops; ++h) {
-    const int b = cum[h], e = cum[h + 1];
-    if (t >= b && t < e) { l.hop = h; l.row = t - b; break; }
-  }
-  return l;
-}
-
-__device__ __forceinline__ float leaky(float x, float slope) { return x > 0.f ? x : x * slope; }
-
-// keep bits of the 8 elements of 16-byte vector i of a dropout mask: the key of k_dropout_bf16 (sage.cu), so a
-// mask regenerated here equals the one `dropout_bf16` draws for the same (seed, layer, step) and row pitch
+// keep bits of the 8 elements of 16-byte vector i of a dropout mask, drawn from dropout_bits as in k_dropout_bf16
+// (sage.cu), so a mask regenerated here equals the one `dropout_bf16` draws for the same (seed, layer, step) and row
+// pitch
 __device__ __forceinline__ unsigned dropout_keep8(uint64_t seed, int layer, uint32_t step, int64_t i,
                                                   uint32_t thresh16) {
-  U4 c;
-  c.x = static_cast<uint32_t>(i);
-  c.y = static_cast<uint32_t>(i >> 32);
-  c.z = step;
-  c.w = 0xD509u + static_cast<uint32_t>(layer);
-  const U4 r = philox4x32_10(static_cast<uint32_t>(seed), static_cast<uint32_t>(seed >> 32), c);
+  const U4 r = dropout_bits(seed, layer, step, i);
   const uint32_t rr[4] = {r.x, r.y, r.z, r.w};
   unsigned m = 0;
 #pragma unroll
@@ -60,11 +42,6 @@ __device__ __forceinline__ void load_f32x8(const float* p, float* v) {
 __device__ __forceinline__ void store_f32x8(float* p, const float* v) {
   reinterpret_cast<float4*>(p)[0] = make_float4(v[0], v[1], v[2], v[3]);
   reinterpret_cast<float4*>(p)[1] = make_float4(v[4], v[5], v[6], v[7]);
-}
-
-__device__ __forceinline__ void red_add8(float* dst, const float* v) {
-  atomicAdd(reinterpret_cast<float4*>(dst), make_float4(v[0], v[1], v[2], v[3]));
-  atomicAdd(reinterpret_cast<float4*>(dst + 4), make_float4(v[4], v[5], v[6], v[7]));
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -120,7 +97,7 @@ __global__ void __launch_bounds__(256) k_gat_aggregate(GatAggArgs a) {
   for (int base = (blockIdx.x * wpb + (threadIdx.x >> 5)) * RPW; base < T; base += gridDim.x * wpb * RPW) {
     const int t = base + gw;
     if (t >= T) continue;                       // whole lane groups leave together
-    const GatHopLoc l = gat_locate(a.cum, a.n_hops_targets, t);
+    const HopLoc l = locate_hop(a.cum, a.n_hops_targets, t);
     const int dg = a.deg[t];
     const int k = a.k[l.hop];
     const int32_t* ell = a.ell[l.hop] + static_cast<int64_t>(l.row) * k;
@@ -223,7 +200,7 @@ __global__ void __launch_bounds__(256) k_gat_backward(GatBwdArgs a) {
   for (int base = (blockIdx.x * wpb + warp) * RPW; base < T; base += gridDim.x * wpb * RPW) {
     const int t = base + gw;
     if (t >= T) continue;
-    const GatHopLoc l = gat_locate(a.cum, a.n_hops_targets, t);
+    const HopLoc l = locate_hop(a.cum, a.n_hops_targets, t);
     const int dg = a.deg[t];
     const int k = a.k[l.hop];
     const int32_t* ell = a.ell[l.hop] + static_cast<int64_t>(l.row) * k;
@@ -407,40 +384,25 @@ __global__ void __launch_bounds__(256) k_gat_act_bwd(GatActBwdArgs a) {
   }
 }
 
-inline int gat_grid(int64_t items, int per_block, int max_blocks = 132 * 16) {
-  int64_t b = (items + per_block - 1) / per_block;
-  if (b < 1) b = 1;
-  if (b > max_blocks) b = max_blocks;
-  return static_cast<int>(b);
-}
-
 }  // namespace
-
-// lane-group shape from the row width H (a multiple of 64 in [64, 1024]: 8 .. 128 vectors)
-#define GLT_GAT_DISPATCH(H, ...)                                              \
-  do {                                                                        \
-    const int nvec_ = (H) / 8;                                                \
-    if (nvec_ <= 8) { constexpr int LPR = 8, VPL = 1; __VA_ARGS__; }          \
-    else if (nvec_ <= 16) { constexpr int LPR = 16, VPL = 1; __VA_ARGS__; }   \
-    else if (nvec_ <= 32) { constexpr int LPR = 32, VPL = 1; __VA_ARGS__; }   \
-    else if (nvec_ <= 64) { constexpr int LPR = 32, VPL = 2; __VA_ARGS__; }   \
-    else { constexpr int LPR = 32, VPL = 4; __VA_ARGS__; }                    \
-  } while (0)
 
 void launch_gat_scores(const GatScoreArgs& a, cudaStream_t s) {
   const int64_t n = (static_cast<int64_t>(a.cap[0]) + a.cap[1]) * a.heads;
-  launch_k(k_gat_scores, dim3(gat_grid(n, 256)), dim3(256), 0, s, a);
+  launch_k(k_gat_scores, dim3(grid_for(n, 256)), dim3(256), 0, s, a);
 }
 
+// lane-group shape from the row width H (a multiple of 64 in [64, 1024]: 8 .. 128 vectors)
 void launch_gat_aggregate(const GatAggArgs& a, cudaStream_t s) {
-  GLT_GAT_DISPATCH(a.H, {
-    launch_k(k_gat_aggregate<LPR, VPL>, dim3(gat_grid(a.cap_targets, 8 * (32 / LPR))), dim3(256), 0, s, a);
+  dispatch_lanes<8, 4>(a.H / 8, [&](auto lpr, auto vpl) {
+    constexpr int LPR = decltype(lpr)::value, VPL = decltype(vpl)::value;
+    launch_k(k_gat_aggregate<LPR, VPL>, dim3(grid_for(a.cap_targets, 8 * (32 / LPR))), dim3(256), 0, s, a);
   });
 }
 
 void launch_gat_backward(const GatBwdArgs& a, cudaStream_t s) {
-  GLT_GAT_DISPATCH(a.H, {
-    launch_k(k_gat_backward<LPR, VPL>, dim3(gat_grid(a.cap_targets, 8 * (32 / LPR))), dim3(256), 0, s, a);
+  dispatch_lanes<8, 4>(a.H / 8, [&](auto lpr, auto vpl) {
+    constexpr int LPR = decltype(lpr)::value, VPL = decltype(vpl)::value;
+    launch_k(k_gat_backward<LPR, VPL>, dim3(grid_for(a.cap_targets, 8 * (32 / LPR))), dim3(256), 0, s, a);
   });
 }
 
@@ -448,12 +410,12 @@ void launch_gat_score_bwd(const GatScoreBwdArgs& a, cudaStream_t s) {
   const int rpb = 256 / (a.H / 8);
   int cap = a.seg[0].cap;
   if (a.seg[1].P) cap = cap > a.seg[1].cap ? cap : a.seg[1].cap;
-  launch_k(k_gat_score_bwd, dim3(gat_grid(cap, rpb * 4, 132 * 4), a.seg[1].P ? 2 : 1), dim3(256), 0, s, a);
+  launch_k(k_gat_score_bwd, dim3(grid_for(cap, rpb * 4, 132 * 4), a.seg[1].P ? 2 : 1), dim3(256), 0, s, a);
 }
 
 void launch_gat_act_bwd(const GatActBwdArgs& a, cudaStream_t s) {
   const int rpb = 256 / (a.d / 8);
-  launch_k(k_gat_act_bwd, dim3(gat_grid(a.cap, rpb * 4, 132 * 4)), dim3(256), 0, s, a);
+  launch_k(k_gat_act_bwd, dim3(grid_for(a.cap, rpb * 4, 132 * 4)), dim3(256), 0, s, a);
 }
 
 }  // namespace glt

@@ -8,6 +8,7 @@
 // rows are narrow, every lane keeps up to four loads in flight, and the row
 // count can stay on the device (n_dev) so the launch is CUDA-graph capturable.
 #include "device_utils.cuh"
+#include "launch_utils.h"
 
 namespace glt {
 
@@ -81,27 +82,6 @@ __global__ void __launch_bounds__(256) k_gather_scalar(RowTable t, const int64_t
     const T* s = reinterpret_cast<const T*>(src);
     for (int c = lane; c < nel; c += 32) dst[c] = src ? s[c] : T(0);
   }
-}
-
-__global__ void k_gather_i64(RowTable t, const int64_t* idx, int64_t n, const int32_t* n_dev,
-                             int64_t* out) {
-  const int64_t n_valid = n_dev ? min(static_cast<int64_t>(*n_dev), n) : n;
-  for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < n;
-       i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
-    int64_t v = -1;
-    if (i < n_valid && idx[i] >= 0) {
-      const uint8_t* p = row_ptr(t, idx[i]);
-      if (p) v = *reinterpret_cast<const int64_t*>(p);
-    }
-    out[i] = v;
-  }
-}
-
-inline int grid_for(int64_t items, int per_block, int max_blocks = 132 * 16) {
-  int64_t b = (items + per_block - 1) / per_block;
-  if (b < 1) b = 1;
-  if (b > max_blocks) b = max_blocks;
-  return static_cast<int>(b);
 }
 
 // 8 lanes per row, 16 e4m3 elements per lane and iteration (d multiple of 128 keeps every lane busy)
@@ -198,26 +178,17 @@ void launch_gather_rows(RowTable t, const int64_t* idx, const int64_t* id2index,
                  (reinterpret_cast<uintptr_t>(out) % 16 == 0);
   for (int p = 0; p < t.num_parts; ++p) aligned &= (reinterpret_cast<uintptr_t>(t.base[p]) % 16 == 0);
   if (aligned) {
-    const int nvec = static_cast<int>(t.row_bytes / 16);
-  // small lookups spread one row per group over as many SMs as possible; large ones keep four rows
-  // in flight per group
-#define GLT_LAUNCH_VEC(LPR)                                                                            \
-  do {                                                                                                 \
-    if (n >= static_cast<int64_t>(132) * 2 * 8 * (32 / LPR) * 4)                                       \
-      k_gather_vec<LPR, 4><<<grid_for(n, 8 * (32 / LPR) * 4), 256, 0, s>>>(t, idx, id2index, n, n_dev, \
-                                                                            o, out_row_bytes,          \
-                                                                            id2index_len);             \
-    else                                                                                               \
-      k_gather_vec<LPR, 1><<<grid_for(n, 8 * (32 / LPR)), 256, 0, s>>>(t, idx, id2index, n, n_dev, o,  \
-                                                                        out_row_bytes, id2index_len);  \
-  } while (0)
-    if (nvec <= 1) GLT_LAUNCH_VEC(1);
-    else if (nvec <= 2) GLT_LAUNCH_VEC(2);
-    else if (nvec <= 4) GLT_LAUNCH_VEC(4);
-    else if (nvec <= 8) GLT_LAUNCH_VEC(8);
-    else if (nvec <= 16) GLT_LAUNCH_VEC(16);
-    else GLT_LAUNCH_VEC(32);
-#undef GLT_LAUNCH_VEC
+    // small lookups spread one row per group over as many SMs as possible; large ones keep four rows
+    // in flight per group
+    dispatch_lanes<1, 1>(static_cast<int>(t.row_bytes / 16), [&](auto lpr, auto) {
+      constexpr int LPR = decltype(lpr)::value;
+      if (n >= static_cast<int64_t>(132) * 2 * 8 * (32 / LPR) * 4)
+        k_gather_vec<LPR, 4><<<grid_for(n, 8 * (32 / LPR) * 4), 256, 0, s>>>(t, idx, id2index, n, n_dev, o,
+                                                                              out_row_bytes, id2index_len);
+      else
+        k_gather_vec<LPR, 1><<<grid_for(n, 8 * (32 / LPR)), 256, 0, s>>>(t, idx, id2index, n, n_dev, o,
+                                                                          out_row_bytes, id2index_len);
+    });
     return;
   }
   const int g = grid_for(n, 8);
@@ -251,12 +222,6 @@ void launch_multimem_copy(const void* src, void* mc_dst, int64_t nbytes, cudaStr
                                                            reinterpret_cast<uint4*>(mc_dst), n16);
 }
 
-void launch_gather_i64(RowTable t, const int64_t* idx, int64_t n, const int32_t* n_dev,
-                       int64_t* out, cudaStream_t s) {
-  if (n <= 0) return;
-  k_gather_i64<<<grid_for(n, 256), 256, 0, s>>>(t, idx, n, n_dev, out);
-}
-
 void launch_gather_mxfp8(RowTable t, const int64_t* idx, int64_t n, int d, void* out, cudaStream_t s) {
   if (n <= 0) return;
   int64_t blocks = (n + 31) / 32;
@@ -268,25 +233,16 @@ void launch_gather_mxfp8_rows(RowTable t, const int64_t* idx, const int64_t* id2
                               int d, void* out, int64_t out_row_bytes, cudaStream_t s, int64_t id2index_len) {
   if (n <= 0) return;
   uint8_t* o = reinterpret_cast<uint8_t*>(out);
-  const int nvec = d / 16;
   // launch shapes as in launch_gather_rows: small lookups one row per group, large ones four rows in flight
-#define GLT_LAUNCH_MXFP8(LPR)                                                                                 \
-  do {                                                                                                        \
-    if (n >= static_cast<int64_t>(132) * 2 * 8 * (32 / LPR) * 4)                                              \
-      k_gather_mxfp8_vec<LPR, 4><<<grid_for(n, 8 * (32 / LPR) * 4), 256, 0, s>>>(t, idx, id2index, n, n_dev,  \
-                                                                                  d, o, out_row_bytes,        \
-                                                                                  id2index_len);              \
-    else                                                                                                      \
-      k_gather_mxfp8_vec<LPR, 1><<<grid_for(n, 8 * (32 / LPR)), 256, 0, s>>>(t, idx, id2index, n, n_dev, d,   \
-                                                                              o, out_row_bytes,               \
-                                                                              id2index_len);                  \
-  } while (0)
-  if (nvec <= 2) GLT_LAUNCH_MXFP8(2);
-  else if (nvec <= 4) GLT_LAUNCH_MXFP8(4);
-  else if (nvec <= 8) GLT_LAUNCH_MXFP8(8);
-  else if (nvec <= 16) GLT_LAUNCH_MXFP8(16);
-  else GLT_LAUNCH_MXFP8(32);
-#undef GLT_LAUNCH_MXFP8
+  dispatch_lanes<2, 1>(d / 16, [&](auto lpr, auto) {
+    constexpr int LPR = decltype(lpr)::value;
+    if (n >= static_cast<int64_t>(132) * 2 * 8 * (32 / LPR) * 4)
+      k_gather_mxfp8_vec<LPR, 4><<<grid_for(n, 8 * (32 / LPR) * 4), 256, 0, s>>>(t, idx, id2index, n, n_dev, d, o,
+                                                                                  out_row_bytes, id2index_len);
+    else
+      k_gather_mxfp8_vec<LPR, 1><<<grid_for(n, 8 * (32 / LPR)), 256, 0, s>>>(t, idx, id2index, n, n_dev, d, o,
+                                                                              out_row_bytes, id2index_len);
+  });
 }
 
 }  // namespace glt

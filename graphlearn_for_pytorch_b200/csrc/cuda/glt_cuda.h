@@ -153,8 +153,6 @@ void launch_nbr_prob(GraphTable g, GraphTable nbr_g, const float* last, const fl
 void launch_gather_rows(RowTable t, const int64_t* idx, const int64_t* id2index, int64_t n,
                         const int32_t* n_dev, void* out, int64_t out_row_bytes, cudaStream_t s,
                         int64_t id2index_len = 0);
-void launch_gather_i64(RowTable t, const int64_t* idx, int64_t n, const int32_t* n_dev,
-                       int64_t* out, cudaStream_t s);
 // copy `nbytes` (multiple of 16) from local memory to an NVSwitch multicast address
 void launch_multimem_copy(const void* src, void* mc_dst, int64_t nbytes, cudaStream_t s);
 // out[i, 0..d) (bf16) = dequantised MXFP8 row idx[i] of `t` (see data/quantize.py), d a multiple of 128
@@ -313,7 +311,6 @@ void launch_zero_rows(float* p, const int32_t* cum, int n_hops, int cap, int d, 
 void launch_adam(float* p, const float* g, float* m, float* v, void* p_bf16, int64_t n, float lr,
                  float b1, float b2, float eps, float wd, int32_t* step_dev, float gscale,
                  cudaStream_t s);
-void launch_bf16_to_f32(const void* src, float* dst, int64_t n, cudaStream_t s);
 
 // ---- link.cu (link-prediction step: in-graph negatives + fused edge loss) --------
 // pos: int64 [2, B] positive pairs (-1 = padding).  Writes seeds [2P], P = (1 + k) B: seeds[p] = source and

@@ -5,6 +5,7 @@
 // (distributed/dist_neighbor_sampler.py:411-413 non-strict local negatives,
 // :555-571 broadcasts whole node sets over RPC).
 #include "device_utils.cuh"
+#include "launch_utils.h"
 
 namespace glt {
 
@@ -144,13 +145,6 @@ __global__ void k_nbr_prob(GraphTable g, GraphTable ng, const float* last, const
     for (int off = 16; off > 0; off >>= 1) acc *= __shfl_xor_sync(0xffffffffu, acc, off);
     if (lane == 0) cur[v] = 1.f - (1.f - last[v]) * acc;
   }
-}
-
-inline int grid_for(int64_t items, int per_block, int max_blocks = 132 * 16) {
-  int64_t b = (items + per_block - 1) / per_block;
-  if (b < 1) b = 1;
-  if (b > max_blocks) b = max_blocks;
-  return static_cast<int>(b);
 }
 
 }  // namespace

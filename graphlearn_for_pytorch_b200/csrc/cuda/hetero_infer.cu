@@ -20,8 +20,6 @@ namespace {
 
 constexpr int kThreads = 256;
 
-__device__ __forceinline__ float leaky_f(float x, float slope) { return x > 0.f ? x : x * slope; }
-
 // ------------------------------------------------------------------------------------------------------ R-GAT
 // Scores are per node (as, ad), so both passes over a row read scalars; only pass 2 reads the projection rows.
 //   pass 1  m = max_j e_ij,h                       (order-free: a max is exact)
@@ -47,7 +45,7 @@ struct GatFull {
 #pragma unroll
       for (int v = 0; v < VPL; ++v) {
         const int c = v * LPR + gl;
-        if (c < nvec) m[v] = fmaxf(m[v], leaky_f(a.as[u * a.heads + c / cv] + ad[v], 0.2f));
+        if (c < nvec) m[v] = fmaxf(m[v], leaky(a.as[u * a.heads + c / cv] + ad[v], 0.2f));
       }
     }
   }
@@ -64,7 +62,7 @@ struct GatFull {
       for (int v = 0; v < VPL; ++v) {
         const int c = v * LPR + gl;
         if (c < nvec) {
-          const float w = expf(leaky_f(a.as[u * a.heads + c / cv] + ad[v], 0.2f) - m[v]);
+          const float w = expf(leaky(a.as[u * a.heads + c / cv] + ad[v], 0.2f) - m[v]);
           s[v] += w;
           float x[8] = {0, 0, 0, 0, 0, 0, 0, 0};
           bf16x8_accum(ld_nc_v4(p + c * 16), x);
@@ -103,7 +101,7 @@ struct GatFull {
         bf16x8_accum(reinterpret_cast<const uint4*>(a.bias)[(b * a.H + c * 8) >> 3], o);
       if (a.act) {
 #pragma unroll
-        for (int q = 0; q < 8; ++q) o[q] = leaky_f(o[q], 0.01f);
+        for (int q = 0; q < 8; ++q) o[q] = leaky(o[q], 0.01f);
       }
       reinterpret_cast<uint4*>(a.z)[e >> 3] = pack_bf16x8(o, 1.f);
     }
@@ -459,19 +457,10 @@ __global__ void __launch_bounds__(kThreads, 2) k_hgt_full_attention(HgtFullAttnA
 }  // namespace
 
 // lane-group shape from the row width H (a multiple of 64 in [64, 1024]: 8 .. 128 vectors)
-#define GLT_HETERO_INFER_DISPATCH(H, ...)                                     \
-  do {                                                                        \
-    const int nvec_ = (H) / 8;                                                \
-    if (nvec_ <= 8) { constexpr int LPR = 8, VPL = 1; __VA_ARGS__; }          \
-    else if (nvec_ <= 16) { constexpr int LPR = 16, VPL = 1; __VA_ARGS__; }   \
-    else if (nvec_ <= 32) { constexpr int LPR = 32, VPL = 1; __VA_ARGS__; }   \
-    else if (nvec_ <= 64) { constexpr int LPR = 32, VPL = 2; __VA_ARGS__; }   \
-    else { constexpr int LPR = 32, VPL = 4; __VA_ARGS__; }                    \
-  } while (0)
-
 void launch_gat_full_aggregate(const GatFullAggArgs& a, cudaStream_t s) {
   if (a.r1 <= a.r0) return;
-  GLT_HETERO_INFER_DISPATCH(a.H, {
+  dispatch_lanes<8, 4>(a.H / 8, [&](auto lpr, auto vpl) {
+    constexpr int LPR = decltype(lpr)::value, VPL = decltype(vpl)::value;
     constexpr int G = kThreads / LPR;
     const int64_t blocks = (a.r1 - a.r0 + G - 1) / G;
     const size_t smem = sizeof(float) * G * (a.H + a.H / 8);
@@ -483,7 +472,8 @@ void launch_gat_full_aggregate(const GatFullAggArgs& a, cudaStream_t s) {
 
 void launch_hgt_full_attention(const HgtFullAttnArgs& a, cudaStream_t s) {
   if (a.r1 <= a.r0) return;
-  GLT_HETERO_INFER_DISPATCH(a.H, {
+  dispatch_lanes<8, 4>(a.H / 8, [&](auto lpr, auto vpl) {
+    constexpr int LPR = decltype(lpr)::value, VPL = decltype(vpl)::value;
     constexpr int G = kThreads / LPR;
     const int64_t blocks = (a.r1 - a.r0 + G - 1) / G;
     const size_t smem = sizeof(float) * G * (LPR * VPL + 3 * a.heads + a.H);   // up to 48 KB (H = 1024, D = 8)

@@ -20,23 +20,6 @@ namespace glt {
 
 namespace {
 
-struct HgtHopLoc { int hop; int row; };
-
-__device__ __forceinline__ HgtHopLoc hgt_locate(const int32_t* cum, int n_hops, int t) {
-  HgtHopLoc l; l.hop = 0; l.row = t;
-#pragma unroll 1
-  for (int h = 0; h < n_hops; ++h) {
-    const int b = cum[h], e = cum[h + 1];
-    if (t >= b && t < e) { l.hop = h; l.row = t - b; break; }
-  }
-  return l;
-}
-
-__device__ __forceinline__ void hgt_red_add8(float* dst, const float* v) {
-  atomicAdd(reinterpret_cast<float4*>(dst), make_float4(v[0], v[1], v[2], v[3]));
-  atomicAdd(reinterpret_cast<float4*>(dst + 4), make_float4(v[4], v[5], v[6], v[7]));
-}
-
 __device__ __forceinline__ float gelu_f(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752f)); }
 
 __device__ __forceinline__ float gelu_grad(float x) {
@@ -44,13 +27,6 @@ __device__ __forceinline__ float gelu_grad(float x) {
 }
 
 __device__ __forceinline__ float sigmoid_f(float x) { return 1.f / (1.f + expf(-x)); }
-
-inline int hgt_grid(int64_t items, int per_block, int max_blocks = 132 * 16) {
-  int64_t b = (items + per_block - 1) / per_block;
-  if (b < 1) b = 1;
-  if (b > max_blocks) b = max_blocks;
-  return static_cast<int>(b);
-}
 
 // ---------------------------------------------------------------------------------------------------------------
 // LPR lanes per target row; a lane owns VPL 16-byte vectors (columns c * 8 .. c * 8 + 7, c = v * LPR + lane) of an
@@ -77,7 +53,7 @@ __global__ void __launch_bounds__(256) k_hgt_attention(HgtAttnArgs a) {
   for (int base = (blockIdx.x * wpb + warp) * RPW; base < T; base += gridDim.x * wpb * RPW) {
     const int t = base + gw;
     if (t >= T) continue;                       // whole lane groups leave together
-    const HgtHopLoc l = hgt_locate(a.cum, a.n_hops_targets, t);
+    const HopLoc l = locate_hop(a.cum, a.n_hops_targets, t);
     float mx[VPL];
 #pragma unroll
     for (int q = 0; q < VPL; ++q) mx[q] = -INFINITY;
@@ -231,7 +207,7 @@ __global__ void __launch_bounds__(256) k_hgt_attention_bwd(HgtAttnBwdArgs a) {
   for (int base = (blockIdx.x * wpb + warp) * RPW; base < T; base += gridDim.x * wpb * RPW) {
     const int t = base + gw;
     if (t >= T) continue;
-    const HgtHopLoc l = hgt_locate(a.cum, a.n_hops_targets, t);
+    const HopLoc l = locate_hop(a.cum, a.n_hops_targets, t);
     float ssum[VPL];
 #pragma unroll
     for (int q = 0; q < VPL; ++q) ssum[q] = 0.f;
@@ -277,7 +253,7 @@ __global__ void __launch_bounds__(256) k_hgt_attention_bwd(HgtAttnBwdArgs a) {
             float z[8];
 #pragma unroll
             for (int e = 0; e < 8; ++e) z[e] = w * g[v][e];
-            hgt_red_add8(dkv + s * ldg + a.H + c * 8, z);
+            red_add8(dkv + s * ldg + a.H + c * 8, z);
           }
         }
         __syncwarp(gmask);
@@ -350,7 +326,7 @@ __global__ void __launch_bounds__(256) k_hgt_attention_bwd(HgtAttnBwdArgs a) {
             bf16x8_accum(ld_nc_v4(p + c * 16), x);
 #pragma unroll
             for (int e = 0; e < 8; ++e) { acc[v][e] = fmaf(w, x[e], acc[v][e]); z[e] = w * qv[v][e]; }
-            hgt_red_add8(dkv + s * ldg + c * 8, z);
+            red_add8(dkv + s * ldg + c * 8, z);
           }
         }
       }
@@ -556,49 +532,41 @@ __global__ void __launch_bounds__(256) k_hgt_kqv_cast(HgtKqvCastArgs a) {
 }  // namespace
 
 // lane-group shape from the row width H (a multiple of 64 in [64, 1024]: 8 .. 128 vectors)
-#define GLT_HGT_DISPATCH(H, ...)                                              \
-  do {                                                                        \
-    const int nvec_ = (H) / 8;                                                \
-    if (nvec_ <= 8) { constexpr int LPR = 8, VPL = 1; __VA_ARGS__; }          \
-    else if (nvec_ <= 16) { constexpr int LPR = 16, VPL = 1; __VA_ARGS__; }   \
-    else if (nvec_ <= 32) { constexpr int LPR = 32, VPL = 1; __VA_ARGS__; }   \
-    else if (nvec_ <= 64) { constexpr int LPR = 32, VPL = 2; __VA_ARGS__; }   \
-    else { constexpr int LPR = 32, VPL = 4; __VA_ARGS__; }                    \
-  } while (0)
-
 void launch_hgt_attention(const HgtAttnArgs& a, cudaStream_t s) {
-  GLT_HGT_DISPATCH(a.H, {
-    launch_k(k_hgt_attention<LPR, VPL>, dim3(hgt_grid(a.cap_targets, 8 * (32 / LPR))), dim3(256), 0, s, a);
+  dispatch_lanes<8, 4>(a.H / 8, [&](auto lpr, auto vpl) {
+    constexpr int LPR = decltype(lpr)::value, VPL = decltype(vpl)::value;
+    launch_k(k_hgt_attention<LPR, VPL>, dim3(grid_for(a.cap_targets, 8 * (32 / LPR))), dim3(256), 0, s, a);
   });
 }
 
 void launch_hgt_attention_bwd(const HgtAttnBwdArgs& a, cudaStream_t s) {
-  GLT_HGT_DISPATCH(a.H, {
-    launch_k(k_hgt_attention_bwd<LPR, VPL>, dim3(hgt_grid(a.cap_targets, 8 * (32 / LPR))), dim3(256), 0, s, a);
+  dispatch_lanes<8, 4>(a.H / 8, [&](auto lpr, auto vpl) {
+    constexpr int LPR = decltype(lpr)::value, VPL = decltype(vpl)::value;
+    launch_k(k_hgt_attention_bwd<LPR, VPL>, dim3(grid_for(a.cap_targets, 8 * (32 / LPR))), dim3(256), 0, s, a);
   });
 }
 
 void launch_hgt_gelu(const void* X, void* Y, const int32_t* cum, int n_hops, int cap, int d, const void* dY,
                      cudaStream_t s) {
-  launch_k(k_hgt_gelu, dim3(hgt_grid(static_cast<int64_t>(cap) * (d / 8), 256, 132 * 8)), dim3(256), 0, s,
+  launch_k(k_hgt_gelu, dim3(grid_for(static_cast<int64_t>(cap) * (d / 8), 256, 132 * 8)), dim3(256), 0, s,
            reinterpret_cast<const __nv_bfloat16*>(X), reinterpret_cast<__nv_bfloat16*>(Y), cum, n_hops, cap, d,
            reinterpret_cast<const __nv_bfloat16*>(dY));
 }
 
 void launch_hgt_gate(const HgtGateArgs& a, cudaStream_t s) {
-  launch_k(k_hgt_gate, dim3(hgt_grid(static_cast<int64_t>(a.cap) * (a.d / 8), 256, 132 * 8)), dim3(256), 0, s, a);
+  launch_k(k_hgt_gate, dim3(grid_for(static_cast<int64_t>(a.cap) * (a.d / 8), 256, 132 * 8)), dim3(256), 0, s, a);
 }
 
 void launch_hgt_blocks(const HgtBlockArgs& a, cudaStream_t s) {
   const int64_t H = static_cast<int64_t>(a.heads) * a.D;
-  launch_k(k_hgt_blocks, dim3(hgt_grid(a.n_rel * H * H, 256, 132 * 8)), dim3(256), 0, s, a);
+  launch_k(k_hgt_blocks, dim3(grid_for(a.n_rel * H * H, 256, 132 * 8)), dim3(256), 0, s, a);
 }
 
 void launch_hgt_kqv_cast(const HgtKqvCastArgs& a, cudaStream_t s) {
   const int nvec = 3 * (a.H / 8);
   const int cw = nvec < 128 ? nvec : 128;
   const int rpb = 256 / cw;
-  launch_k(k_hgt_kqv_cast, dim3(hgt_grid(a.cap, rpb * 4, 132 * 4), (nvec + 127) / 128), dim3(256), 0, s, a);
+  launch_k(k_hgt_kqv_cast, dim3(grid_for(a.cap, rpb * 4, 132 * 4), (nvec + 127) / 128), dim3(256), 0, s, a);
 }
 
 }  // namespace glt

@@ -132,13 +132,6 @@ __global__ void __launch_bounds__(256) k_link_bce(const __nv_bfloat16* Z, int ld
   }
 }
 
-inline int grid_for(int64_t items, int per_block, int max_blocks = 132 * 16) {
-  int64_t b = (items + per_block - 1) / per_block;
-  if (b < 1) b = 1;
-  if (b > max_blocks) b = max_blocks;
-  return static_cast<int>(b);
-}
-
 }  // namespace
 
 void launch_link_seeds(GraphTable g, const int64_t* pos, int B, int k, int64_t num_nodes, uint64_t seed,
@@ -150,16 +143,11 @@ void launch_link_seeds(GraphTable g, const int64_t* pos, int B, int k, int64_t n
 void launch_link_bce(const void* Z, int ld, int C, const int32_t* seed_local, int P, int B, const int32_t* n_pairs,
                      float* loss, int32_t* correct, float* dZ, cudaStream_t s) {
   const __nv_bfloat16* z = reinterpret_cast<const __nv_bfloat16*>(Z);
-  const int nvec = C / 8;
-#define GLT_LINK_BCE(LPR, VPL)                                                                              \
-  launch_k(k_link_bce<LPR, VPL>, dim3(grid_for(P, 8 * (32 / LPR))), dim3(256), 0, s, z, ld, C, seed_local, P, B, \
-           n_pairs, loss, correct, dZ)
-  if (nvec <= 4) GLT_LINK_BCE(4, 1);
-  else if (nvec <= 8) GLT_LINK_BCE(8, 1);
-  else if (nvec <= 16) GLT_LINK_BCE(16, 1);
-  else if (nvec <= 32) GLT_LINK_BCE(32, 1);
-  else GLT_LINK_BCE(32, 2);
-#undef GLT_LINK_BCE
+  dispatch_lanes<4, 2>(C / 8, [&](auto lpr, auto vpl) {
+    constexpr int LPR = decltype(lpr)::value, VPL = decltype(vpl)::value;
+    launch_k(k_link_bce<LPR, VPL>, dim3(grid_for(P, 8 * (32 / LPR))), dim3(256), 0, s, z, ld, C, seed_local, P, B,
+             n_pairs, loss, correct, dZ);
+  });
 }
 
 }  // namespace glt

@@ -16,23 +16,6 @@ namespace glt {
 
 namespace {
 
-struct HopLoc { int hop; int row; };
-
-__device__ __forceinline__ HopLoc locate(const int32_t* cum, int n_hops, int t) {
-  HopLoc l; l.hop = 0; l.row = t;
-#pragma unroll 1
-  for (int h = 0; h < n_hops; ++h) {
-    const int b = cum[h], e = cum[h + 1];
-    if (t >= b && t < e) { l.hop = h; l.row = t - b; break; }
-  }
-  return l;
-}
-
-__device__ __forceinline__ const uint8_t* src_row(const SageAggArgs& a, int s) {
-  if (a.src_local) return reinterpret_cast<const uint8_t*>(a.src_local) + static_cast<int64_t>(s) * a.d * 2;
-  return row_ptr(a.feat, a.nodes[s]);
-}
-
 // LPR lanes cooperate on one target row; each lane owns VPL 16-byte vectors: 8 bf16 elements, or (FP8: the feature
 // table holds MXFP8 rows) 16 e4m3 elements that are de-quantised as they are accumulated.  Either way the mean is
 // summed in fp32 in ELL slot order, rounded once and written as bf16; the FP8 self block is bf16(de-quantised row).
@@ -59,7 +42,7 @@ __global__ void __launch_bounds__(256) k_sage_aggregate(SageAggArgs a) {
     int dg = 0, k = 0;
     const int32_t* ell = nullptr;
     if (valid) {
-      const HopLoc l = locate(a.cum, a.n_hops_targets, t);
+      const HopLoc l = locate_hop(a.cum, a.n_hops_targets, t);
       dg = a.deg[t];
       k = a.k[l.hop];
       ell = a.ell[l.hop] + static_cast<int64_t>(l.row) * k;
@@ -120,11 +103,6 @@ __global__ void __launch_bounds__(256) k_sage_aggregate(SageAggArgs a) {
   }
 }
 
-__device__ __forceinline__ void atomic_add8(float* dst, const float* v) {
-  atomicAdd(reinterpret_cast<float4*>(dst), make_float4(v[0], v[1], v[2], v[3]));
-  atomicAdd(reinterpret_cast<float4*>(dst + 4), make_float4(v[4], v[5], v[6], v[7]));
-}
-
 // 8 blocks per SM: every width variant stays at <= 32 registers, i.e. 64 resident warps to cover the atomics' latency
 template <int LPR, int VPL>
 __global__ void __launch_bounds__(256, 8) k_sage_scatter_bwd(SageScatterArgs a) {
@@ -139,7 +117,7 @@ __global__ void __launch_bounds__(256, 8) k_sage_scatter_bwd(SageScatterArgs a) 
   for (int base = (blockIdx.x * wpb + (threadIdx.x >> 5)) * RPW; base < T; base += gridDim.x * wpb * RPW) {
     const int t = base + gw;
     if (t >= T) continue;
-    const HopLoc l = locate(a.cum, a.n_hops_targets, t);
+    const HopLoc l = locate_hop(a.cum, a.n_hops_targets, t);
     const int dg = a.deg[t];
     const int k = a.k[l.hop];
     const int32_t* ell = a.ell[l.hop] + static_cast<int64_t>(l.row) * k;
@@ -157,7 +135,7 @@ __global__ void __launch_bounds__(256, 8) k_sage_scatter_bwd(SageScatterArgs a) 
       for (int i = 0; i < 8; ++i) gn[i] *= inv;
       for (int j = 0; j < dg; ++j) {
         const int s = ell[j];
-        if (s >= 0) atomic_add8(a.dH + static_cast<int64_t>(s) * a.d + c * 8, gn);
+        if (s >= 0) red_add8(a.dH + static_cast<int64_t>(s) * a.d + c * 8, gn);
       }
     }
   }
@@ -398,36 +376,12 @@ __global__ void k_zero_rows(float* p, const int32_t* cum, int n_hops, int cap, i
     reinterpret_cast<float4*>(p)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
 }
 
-__global__ void k_bf16_to_f32(const __nv_bfloat16* s, float* d, int64_t n) {
-  for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < n;
-       i += static_cast<int64_t>(gridDim.x) * blockDim.x)
-    d[i] = __bfloat162float(s[i]);
-}
-
-inline int grid_for(int64_t items, int per_block, int max_blocks = 132 * 16) {
-  int64_t b = (items + per_block - 1) / per_block;
-  if (b < 1) b = 1;
-  if (b > max_blocks) b = max_blocks;
-  return static_cast<int>(b);
-}
-
 }  // namespace
 
 int& pdl_flag() {
   static int flag = 1;
   return flag;
 }
-
-#define GLT_DISPATCH_WIDTH(D, ...)                                            \
-  do {                                                                        \
-    const int nvec_ = (D) / 8;                                                \
-    if (nvec_ <= 4) { constexpr int LPR = 4, VPL = 1; __VA_ARGS__; }          \
-    else if (nvec_ <= 8) { constexpr int LPR = 8, VPL = 1; __VA_ARGS__; }     \
-    else if (nvec_ <= 16) { constexpr int LPR = 16, VPL = 1; __VA_ARGS__; }   \
-    else if (nvec_ <= 32) { constexpr int LPR = 32, VPL = 1; __VA_ARGS__; }   \
-    else if (nvec_ <= 64) { constexpr int LPR = 32, VPL = 2; __VA_ARGS__; }   \
-    else { constexpr int LPR = 32, VPL = 4; __VA_ARGS__; }                    \
-  } while (0)
 
 int set_pdl(int on) {
   const int old = pdl_flag();
@@ -438,27 +392,23 @@ int set_pdl(int on) {
 void launch_sage_aggregate(const SageAggArgs& a, cudaStream_t s) {
   if (a.feat_fp8) {
     // MXFP8 layer-1 source: d / 16 vectors of 16 elements; <32, 2> holds a 1024-wide row in 32 accumulators per lane
-    const int nvec = a.d / 16;
-#define GLT_LAUNCH_AGG_FP8(LPR, VPL)                                                                             \
-  launch_k(k_sage_aggregate<LPR, VPL, true>, dim3(grid_for(a.cap_targets, 8 * (32 / LPR))), dim3(256), 0, s, a)
-    if (nvec <= 2) GLT_LAUNCH_AGG_FP8(2, 1);
-    else if (nvec <= 4) GLT_LAUNCH_AGG_FP8(4, 1);
-    else if (nvec <= 8) GLT_LAUNCH_AGG_FP8(8, 1);
-    else if (nvec <= 16) GLT_LAUNCH_AGG_FP8(16, 1);
-    else if (nvec <= 32) GLT_LAUNCH_AGG_FP8(32, 1);
-    else GLT_LAUNCH_AGG_FP8(32, 2);
-#undef GLT_LAUNCH_AGG_FP8
+    dispatch_lanes<2, 2>(a.d / 16, [&](auto lpr, auto vpl) {
+      constexpr int LPR = decltype(lpr)::value, VPL = decltype(vpl)::value;
+      launch_k(k_sage_aggregate<LPR, VPL, true>, dim3(grid_for(a.cap_targets, 8 * (32 / LPR))), dim3(256), 0, s, a);
+    });
     return;
   }
   // (a variant keeping 4 neighbour rows in flight per lane group before accumulating made the step slower and was
   // removed: the rows are L2-resident activations)
-  GLT_DISPATCH_WIDTH(a.d, {
+  dispatch_lanes<4, 4>(a.d / 8, [&](auto lpr, auto vpl) {
+    constexpr int LPR = decltype(lpr)::value, VPL = decltype(vpl)::value;
     launch_k(k_sage_aggregate<LPR, VPL>, dim3(grid_for(a.cap_targets, 8 * (32 / LPR))), dim3(256), 0, s, a);
   });
 }
 
 void launch_sage_scatter_bwd(const SageScatterArgs& a, cudaStream_t s) {
-  GLT_DISPATCH_WIDTH(a.d, {
+  dispatch_lanes<4, 4>(a.d / 8, [&](auto lpr, auto vpl) {
+    constexpr int LPR = decltype(lpr)::value, VPL = decltype(vpl)::value;
     launch_k(k_sage_scatter_bwd<LPR, VPL>, dim3(grid_for(a.cap_targets, 8 * (32 / LPR))), dim3(256), 0, s, a);
   });
 }
@@ -475,12 +425,7 @@ __global__ void __launch_bounds__(256) k_dropout_bf16(__nv_bfloat16* Z, const in
   const uint32_t step = step_dev ? static_cast<uint32_t>(*step_dev) : 0u;
   for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < n8;
        i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
-    U4 c;
-    c.x = static_cast<uint32_t>(i);
-    c.y = static_cast<uint32_t>(i >> 32);
-    c.z = step;
-    c.w = 0xD509u + static_cast<uint32_t>(layer);
-    const U4 r = philox4x32_10(static_cast<uint32_t>(seed), static_cast<uint32_t>(seed >> 32), c);
+    const U4 r = dropout_bits(seed, layer, step, i);
     const uint32_t rr[4] = {r.x, r.y, r.z, r.w};
     uint4 v = *reinterpret_cast<const uint4*>(Z + i * 8);
     float z[8];
@@ -572,10 +517,6 @@ void launch_zero_grads(float* g, int64_t n, float* loss, int32_t* correct, cudaS
 
 void launch_zero_rows(float* p, const int32_t* cum, int n_hops, int cap, int d, cudaStream_t s) {
   launch_k(k_zero_rows, dim3(grid_for(static_cast<int64_t>(cap) * d / 4, 256 * 4)), dim3(256), 0, s, p, cum, n_hops, cap, d);
-}
-
-void launch_bf16_to_f32(const void* src, float* dst, int64_t n, cudaStream_t s) {
-  k_bf16_to_f32<<<grid_for(n, 256), 256, 0, s>>>(reinterpret_cast<const __nv_bfloat16*>(src), dst, n);
 }
 
 }  // namespace glt

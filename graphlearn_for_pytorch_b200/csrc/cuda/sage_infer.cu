@@ -215,22 +215,14 @@ void launch_full(const SageFullAggArgs& a, cudaStream_t s) {
 void launch_sage_full_aggregate(const SageFullAggArgs& a, cudaStream_t s) {
   if (a.r1 <= a.r0) return;
   if (a.feat_fp8) {   // d / 16 vectors of 16 e4m3 elements; d = 128 is <8, 1, true>
-    const int nvec = a.d / 16;
-    if (nvec <= 2) launch_full<2, 1, true>(a, s);
-    else if (nvec <= 4) launch_full<4, 1, true>(a, s);
-    else if (nvec <= 8) launch_full<8, 1, true>(a, s);
-    else if (nvec <= 16) launch_full<16, 1, true>(a, s);
-    else if (nvec <= 32) launch_full<32, 1, true>(a, s);
-    else launch_full<32, 2, true>(a, s);
+    dispatch_lanes<2, 2>(a.d / 16, [&](auto lpr, auto vpl) {
+      launch_full<decltype(lpr)::value, decltype(vpl)::value, true>(a, s);
+    });
     return;
   }
-  const int nvec = a.d / 8;
-  if (nvec <= 4) launch_full<4, 1, false>(a, s);
-  else if (nvec <= 8) launch_full<8, 1, false>(a, s);
-  else if (nvec <= 16) launch_full<16, 1, false>(a, s);
-  else if (nvec <= 32) launch_full<32, 1, false>(a, s);
-  else if (nvec <= 64) launch_full<32, 2, false>(a, s);
-  else launch_full<32, 4, false>(a, s);
+  dispatch_lanes<4, 4>(a.d / 8, [&](auto lpr, auto vpl) {
+    launch_full<decltype(lpr)::value, decltype(vpl)::value, false>(a, s);
+  });
 }
 
 }  // namespace glt

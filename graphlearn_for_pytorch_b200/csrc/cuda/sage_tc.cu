@@ -28,22 +28,6 @@ constexpr int kChunkBytes = 128;                    // 64 bf16 = one SWIZZLE_128
 constexpr int kAChunkTile = kTileM * kChunkBytes;   // 16 KB per K-chunk of an A tile
 constexpr int kMmaStageBytes = 16 * 128;            // per-warp epilogue staging: 16 rows x 64 bf16
 
-struct HopLoc2 { int hop; int row; };
-__device__ __forceinline__ HopLoc2 locate2(const int32_t* cum, int n_hops, int t) {
-  HopLoc2 l; l.hop = 0; l.row = t;
-#pragma unroll 1
-  for (int h = 0; h < n_hops; ++h) {
-    const int b = cum[h], e = cum[h + 1];
-    if (t >= b && t < e) { l.hop = h; l.row = t - b; break; }
-  }
-  return l;
-}
-
-__device__ __forceinline__ const uint8_t* src_row2(const SageAggArgs& a, int s) {
-  if (a.src_local) return reinterpret_cast<const uint8_t*>(a.src_local) + static_cast<int64_t>(s) * a.d * 2;
-  return row_ptr(a.feat, a.nodes[s]);
-}
-
 // One warpgroup's work on half h (rows 64 h .. 64 h + 63) of a 128-row tile:
 // Z[row0 + 64 h ...] = act([mean | self] . W^T + b).  It runs in blocks of 64 columns (wgmma.m64n64k16;
 // m64n32k16 for a 32-column tail) so that the accumulator takes 32 registers per thread in CTAs of up to 768
@@ -285,13 +269,13 @@ __global__ void __launch_bounds__(kThreads3, 1) k_sage_fused3(SageFusedArgs f) {
             for (int jj = 0; jj < NF; ++jj) mxfp8x16_accum(v[jj], sc[jj], gl, acc);
           }
           if (dg > kKP) {  // rows wider than the table (fan-out > 15): chase the rest here
-            const HopLoc2 l = locate2(a.cum, a.n_hops_targets, t);
+            const HopLoc l = locate_hop(a.cum, a.n_hops_targets, t);
             const int32_t* ellrow = a.ell[l.hop] + static_cast<int64_t>(l.row) * a.k[l.hop];
 #pragma unroll 1
             for (int j = kKP; j < dg; ++j) {
               const int sidx = __ldg(ellrow + j);
               if (sidx < 0) continue;
-              const uint8_t* p = src_row2(a, sidx);
+              const uint8_t* p = src_row(a, sidx);
               mxfp8x16_accum(ld_nc_v4(p + gl * 16), ld_nc_u32(p + a.d), gl, acc);
             }
           }
@@ -363,13 +347,13 @@ __global__ void __launch_bounds__(kThreads3, 1) k_sage_fused3(SageFusedArgs f) {
             for (int c = 0; c < NC; ++c) bf16x8_accum(v[jj][c], acc[c]);
         }
         if (dg > kKP) {  // rows wider than the table (fan-out > 15): chase the rest here
-          const HopLoc2 l = locate2(a.cum, a.n_hops_targets, t);
+          const HopLoc l = locate_hop(a.cum, a.n_hops_targets, t);
           const int32_t* ellrow = a.ell[l.hop] + static_cast<int64_t>(l.row) * a.k[l.hop];
 #pragma unroll 1
           for (int j = kKP; j < dg; ++j) {
             const int sidx = __ldg(ellrow + j);
             if (sidx < 0) continue;
-            const uint8_t* p = src_row2(a, sidx);
+            const uint8_t* p = src_row(a, sidx);
 #pragma unroll
             for (int c = 0; c < NC; ++c) bf16x8_accum(ld_nc_v4(p + c * kChunkBytes + gl * 16), acc[c]);
           }
@@ -416,7 +400,7 @@ __global__ void __launch_bounds__(kThreads3, 1) k_sage_fused3(SageFusedArgs f) {
       const int32_t* ellp = nullptr;
       int64_t self_gid = -1;
       if (t < T) {
-        const HopLoc2 l = locate2(a.cum, a.n_hops_targets, t);
+        const HopLoc l = locate_hop(a.cum, a.n_hops_targets, t);
         kk = min(a.k[l.hop], kKP);
         ellp = a.ell[l.hop] + static_cast<int64_t>(l.row) * a.k[l.hop];
         dg = __ldg(a.deg + t);

@@ -489,13 +489,6 @@ __global__ void k_table_lookup(HashTable t, const int64_t* keys, int64_t n, int3
   }
 }
 
-inline int grid_for(int64_t work_items, int per_block, int max_blocks = 132 * 16) {
-  int64_t b = (work_items + per_block - 1) / per_block;
-  if (b < 1) b = 1;
-  if (b > max_blocks) b = max_blocks;
-  return static_cast<int>(b);
-}
-
 }  // namespace
 
 void launch_table_clear(HashTable t, cudaStream_t s) {

@@ -187,13 +187,6 @@ __global__ void k_tr_meta(TransposeArgs a) {
   }
 }
 
-inline int grid_for(int64_t items, int per_block, int max_blocks = 132 * 16) {
-  int64_t b = (items + per_block - 1) / per_block;
-  if (b < 1) b = 1;
-  if (b > max_blocks) b = max_blocks;
-  return static_cast<int>(b);
-}
-
 // ------------------------------------------------------------------------------------------
 // Gather-style backward of the mean aggregation:
 //   dPre[s] = relu'(Z[s]) * gscale * (dA_self[s] + sum_{t in in(s)} dA_mean[t] / deg[t])       (+ bias column sums)
@@ -548,20 +541,10 @@ void launch_build_transpose(const TransposeArgs& a, cudaStream_t s) {
   if (a.meta) k_tr_meta<<<grid_for(a.cap_nodes, 256, 132 * 4), 256, 0, s>>>(a);
 }
 
-#define GLT_DISPATCH_WIDTH_T(D, ...)                                          \
-  do {                                                                        \
-    const int nvec_ = (D) / 8;                                                \
-    if (nvec_ <= 4) { constexpr int LPR = 4, VPL = 1; __VA_ARGS__; }          \
-    else if (nvec_ <= 8) { constexpr int LPR = 8, VPL = 1; __VA_ARGS__; }     \
-    else if (nvec_ <= 16) { constexpr int LPR = 16, VPL = 1; __VA_ARGS__; }   \
-    else if (nvec_ <= 32) { constexpr int LPR = 32, VPL = 1; __VA_ARGS__; }   \
-    else if (nvec_ <= 64) { constexpr int LPR = 32, VPL = 2; __VA_ARGS__; }   \
-    else { constexpr int LPR = 32, VPL = 4; __VA_ARGS__; }                    \
-  } while (0)
-
 void launch_sage_gather_bwd(const SageGatherBwdArgs& a, cudaStream_t s) {
   if (a.colsum && !a.colsum_prezeroed) cudaMemsetAsync(a.colsum, 0, sizeof(float) * a.d, s);
-  GLT_DISPATCH_WIDTH_T(a.d, {
+  dispatch_lanes<4, 4>(a.d / 8, [&](auto lpr, auto vpl) {
+    constexpr int LPR = decltype(lpr)::value, VPL = decltype(vpl)::value;
     constexpr int TEAM = (LPR == 32) ? 4 : (LPR == 16 ? 2 : 1);
     launch_k(k_sage_gather_bwd<LPR, VPL>, dim3(grid_for(a.cap_src, 8 * 32 / TEAM, 132 * 8)), dim3(256),
              sizeof(float) * a.d * 8, s, a);
