@@ -10,6 +10,10 @@
 #include <pybind11/stl.h>
 #include <torch/extension.h>
 
+#include <cstdarg>
+#include <cstdio>
+#include <type_traits>
+
 #include "cpu/cpu_ops.h"
 #include "cpu/sample_queue.h"
 #include "cuda/glt_cuda.h"
@@ -21,9 +25,21 @@ namespace glt {
 
 static cudaStream_t cur_stream() { return at::cuda::getCurrentCUDAStream().stream(); }
 
+// Every TORCH_CHECK in this extension takes at most one message argument: a message assembled from several arguments
+// crashes the process when it is thrown instead of raising.  A message that carries values is formatted first.
+static std::string fmt(const char* f, ...) __attribute__((format(printf, 1, 2)));
+static std::string fmt(const char* f, ...) {
+  char buf[512];
+  va_list ap;
+  va_start(ap, f);
+  std::vsnprintf(buf, sizeof(buf), f, ap);
+  va_end(ap);
+  return buf;
+}
+
 static void check_cuda_err(const char* what) {
   cudaError_t e = cudaGetLastError();
-  TORCH_CHECK(e == cudaSuccess, what, ": ", cudaGetErrorString(e));
+  TORCH_CHECK(e == cudaSuccess, fmt("%s: %s", what, cudaGetErrorString(e)));
 }
 
 static const void* dev_ptr(const Tensor& t) {
@@ -31,6 +47,47 @@ static const void* dev_ptr(const Tensor& t) {
   // directly dereferenceable from a kernel under UVA.
   TORCH_CHECK(t.is_cuda() || t.is_pinned(), "tensor must be CUDA or pinned host memory");
   return t.data_ptr();
+}
+
+// Argument checks of the engine operands.  Unlike graph shards and row-table parts (dev_ptr), an operand must live on
+// the device the binding launches on, the one its CUDAGuard made current.
+static bool has(const c10::optional<Tensor>& t) { return t.has_value() && t->defined(); }
+
+template <typename T = void>
+static T* opt_ptr(const c10::optional<Tensor>& t) {
+  if constexpr (std::is_void_v<T>) return has(t) ? t->data_ptr() : nullptr;
+  else return has(t) ? t->data_ptr<T>() : nullptr;
+}
+
+static bool on_dev(const Tensor& t) { return t.is_cuda() && t.get_device() == c10::cuda::current_device(); }
+static bool aligned16(const Tensor& t) { return reinterpret_cast<uintptr_t>(t.data_ptr()) % 16 == 0; }
+
+// contiguous [rows, w], 16-byte aligned
+static void check_rows(const Tensor& t, c10::ScalarType dt, int64_t w, const char* msg) {
+  TORCH_CHECK(on_dev(t) && t.scalar_type() == dt && t.dim() == 2 && t.size(1) == w && t.is_contiguous() &&
+              aligned16(t), msg);
+}
+
+// 2-D view with unit inner stride and 16-byte aligned rows whose columns [col, col + w) lie inside the row
+static void check_block(const Tensor& t, c10::ScalarType dt, int64_t col, int64_t w, const char* msg) {
+  TORCH_CHECK(on_dev(t) && t.scalar_type() == dt && t.dim() == 2 && t.stride(1) == 1 &&
+              t.stride(0) * t.element_size() % 16 == 0 && aligned16(t) && col >= 0 &&
+              col * t.element_size() % 16 == 0 && col + w <= t.size(1), msg);
+}
+
+// contiguous [n], 16-byte aligned
+static void check_vec(const Tensor& t, c10::ScalarType dt, int64_t n, const char* msg) {
+  TORCH_CHECK(on_dev(t) && t.scalar_type() == dt && t.numel() == n && t.is_contiguous() && aligned16(t), msg);
+}
+
+// int32 device counters with an entry at idx
+static void check_counters(const Tensor& t, int64_t idx, const char* msg) {
+  TORCH_CHECK(on_dev(t) && t.scalar_type() == torch::kInt32 && t.is_contiguous() && idx >= 0 && t.numel() > idx, msg);
+}
+
+// contiguous int64 ids
+static void check_ids(const Tensor& t, const char* msg) {
+  TORCH_CHECK(on_dev(t) && t.scalar_type() == torch::kInt64 && t.is_contiguous(), msg);
 }
 
 // ---------------------------------------------------------------------------
@@ -48,13 +105,21 @@ struct GraphHandle {
   void add_shard(const Tensor& indptr, const Tensor& indices, const c10::optional<Tensor>& eids,
                  const c10::optional<Tensor>& weights, int64_t row_begin, int64_t row_end) {
     TORCH_CHECK(tbl.num_parts < kMaxParts, "too many graph shards");
-    TORCH_CHECK(indptr.scalar_type() == torch::kInt64 && indptr.is_contiguous());
-    TORCH_CHECK(indices.is_contiguous());
+    TORCH_CHECK(indptr.scalar_type() == torch::kInt64 && indptr.is_contiguous(),
+                "add_shard: indptr must be contiguous int64");
+    TORCH_CHECK(indices.is_contiguous() &&
+                (indices.scalar_type() == torch::kInt32 || indices.scalar_type() == torch::kInt64),
+                "add_shard: indices must be contiguous int32 or int64");
     int ib = indices.scalar_type() == torch::kInt32 ? 4 : 8;
-    TORCH_CHECK(indices.scalar_type() == torch::kInt32 || indices.scalar_type() == torch::kInt64);
     if (tbl.num_parts == 0) tbl.idx_bytes = ib;
     TORCH_CHECK(tbl.idx_bytes == ib, "all shards must share the column id width");
     TORCH_CHECK(indptr.numel() == row_end - row_begin + 1, "indptr size != rows + 1");
+    TORCH_CHECK(!has(eids) || (eids->scalar_type() == torch::kInt64 && eids->is_contiguous() &&
+                               eids->numel() == indices.numel()),
+                "add_shard: eids must be contiguous int64, one per column index");
+    TORCH_CHECK(!has(weights) || (weights->scalar_type() == torch::kFloat32 && weights->is_contiguous() &&
+                                  weights->numel() == indices.numel()),
+                "add_shard: weights must be contiguous fp32, one per column index");
     CsrShard& s = tbl.parts[tbl.num_parts++];
     s.indptr = reinterpret_cast<const int64_t*>(dev_ptr(indptr));
     s.indices = dev_ptr(indices);
@@ -62,15 +127,13 @@ struct GraphHandle {
     s.weights = nullptr;
     keep.push_back(indptr);
     keep.push_back(indices);
-    if (eids.has_value() && eids->defined()) {
-      TORCH_CHECK(eids->scalar_type() == torch::kInt64);
+    if (has(eids)) {
       s.eids = reinterpret_cast<const int64_t*>(dev_ptr(*eids));
       keep.push_back(*eids);
     } else {
       has_eids = false;
     }
-    if (weights.has_value() && weights->defined()) {
-      TORCH_CHECK(weights->scalar_type() == torch::kFloat32);
+    if (has(weights)) {
       s.weights = reinterpret_cast<const float*>(dev_ptr(*weights));
       keep.push_back(*weights);
     } else {
@@ -90,7 +153,7 @@ struct GraphHandle {
                                                     bool weighted, bool replace, int64_t seed,
                                                     int64_t stream) {
     c10::cuda::CUDAGuard guard(device);
-    TORCH_CHECK(seeds.is_cuda() && seeds.scalar_type() == torch::kInt64 && seeds.is_contiguous());
+    check_ids(seeds, "sample_one_hop: seeds must be contiguous int64 on the graph's device");
     TORCH_CHECK(k > 0 && k <= 512, "fanout must be in [1, 512] (use -1 for all neighbours)");
     TORCH_CHECK(!with_edge || has_eids, "graph has no edge ids");
     TORCH_CHECK(!weighted || has_weights, "graph has no edge weights on the device");
@@ -107,6 +170,7 @@ struct GraphHandle {
 
   Tensor lookup_degree(const Tensor& ids) {
     c10::cuda::CUDAGuard guard(device);
+    check_ids(ids, "lookup_degree: ids must be contiguous int64 on the graph's device");
     Tensor out = torch::empty({ids.numel()}, opts(torch::kInt64));
     launch_lookup_degree(tbl, ids.data_ptr<int64_t>(), ids.numel(), out.data_ptr<int64_t>(), cur_stream());
     check_cuda_err("lookup_degree");
@@ -147,6 +211,7 @@ struct GraphHandle {
   Tensor random_walk(const Tensor& starts, int64_t walk_len, double p, double q, int64_t seed,
                      int64_t stream) {
     c10::cuda::CUDAGuard guard(device);
+    check_ids(starts, "random_walk: starts must be contiguous int64 on the graph's device");
     Tensor out = torch::empty({starts.numel(), walk_len + 1}, opts(torch::kInt64));
     launch_random_walk(tbl, starts.data_ptr<int64_t>(), starts.numel(), walk_len, p, q, seed, stream,
                        out.data_ptr<int64_t>(), cur_stream());
@@ -156,6 +221,9 @@ struct GraphHandle {
 
   Tensor nbr_prob(GraphHandle& nbr_graph, const Tensor& last, const Tensor& nbr_last, int64_t k) {
     c10::cuda::CUDAGuard guard(device);
+    for (const Tensor* t : {&last, &nbr_last})
+      TORCH_CHECK(on_dev(*t) && t->scalar_type() == torch::kFloat32 && t->is_contiguous(),
+                  "nbr_prob: last and nbr_last must be contiguous fp32 on the graph's device");
     Tensor cur = torch::zeros_like(last);
     launch_nbr_prob(tbl, nbr_graph.tbl, last.data_ptr<float>(), nbr_last.data_ptr<float>(),
                     std::min<int64_t>(last.numel(), num_rows), nbr_last.numel(), k,
@@ -200,7 +268,7 @@ struct DeviceTable {
   // unordered insert; returns local ids (int32).  New keys are appended to `nodes`.
   Tensor insert(const Tensor& k) {
     c10::cuda::CUDAGuard guard(device);
-    TORCH_CHECK(k.is_cuda() && k.scalar_type() == torch::kInt64 && k.is_contiguous());
+    check_ids(k, "DeviceTable.insert: keys must be contiguous int64 on the table's device");
     Tensor out = torch::empty({k.numel()}, torch::TensorOptions().dtype(torch::kInt32).device(k.device()));
     launch_table_insert(ht, k.data_ptr<int64_t>(), k.numel(), nodes.data_ptr<int64_t>(),
                         cursor.data_ptr<int32_t>(), cap_nodes, out.data_ptr<int32_t>(), cur_stream());
@@ -212,7 +280,7 @@ struct DeviceTable {
   // ordered (first-occurrence) insert into an empty table; returns local ids
   Tensor init_ordered(const Tensor& k) {
     c10::cuda::CUDAGuard guard(device);
-    TORCH_CHECK(k.is_cuda() && k.scalar_type() == torch::kInt64 && k.is_contiguous());
+    check_ids(k, "DeviceTable.init_ordered: keys must be contiguous int64 on the table's device");
     TORCH_CHECK(k.numel() <= cap_nodes, "table capacity exceeded");
     auto o32 = torch::TensorOptions().dtype(torch::kInt32).device(k.device());
     Tensor out = torch::empty({k.numel()}, o32);
@@ -227,6 +295,7 @@ struct DeviceTable {
 
   Tensor lookup(const Tensor& k) {
     c10::cuda::CUDAGuard guard(device);
+    check_ids(k, "DeviceTable.lookup: keys must be contiguous int64 on the table's device");
     Tensor out = torch::empty({k.numel()}, torch::TensorOptions().dtype(torch::kInt32).device(k.device()));
     launch_table_lookup(ht, k.data_ptr<int64_t>(), k.numel(), out.data_ptr<int32_t>(), cur_stream());
     check_cuda_err("table lookup");
@@ -359,14 +428,14 @@ struct SamplerArena {
   void sample(GraphHandle& g, const Tensor& seeds, const c10::optional<Tensor>& n_dev, int64_t seed,
               int64_t stream_base, bool weighted, bool replace, bool use_dev_step, int64_t step_inc) {
     c10::cuda::CUDAGuard guard(device);
-    TORCH_CHECK(seeds.is_cuda() && seeds.scalar_type() == torch::kInt64 && seeds.is_contiguous());
+    check_ids(seeds, "SamplerArena.sample: seeds must be contiguous int64 on the arena's device");
     TORCH_CHECK(seeds.numel() <= max_seeds, "more seeds than the arena was built for");
+    if (has(n_dev)) check_counters(*n_dev, 0, "SamplerArena.sample: n_dev must be int32 [>= 1] on the arena's device");
     TORCH_CHECK(!with_edge || g.has_eids, "graph has no edge ids");
     TORCH_CHECK(!weighted || g.has_weights, "graph has no device edge weights");
     cudaStream_t s = cur_stream();
     launch_table_clear(table->ht, s);
-    const int32_t* nd = (n_dev.has_value() && n_dev->defined()) ? n_dev->data_ptr<int32_t>() : nullptr;
-    launch_init_seeds(seeds.data_ptr<int64_t>(), seeds.numel(), nd, table->ht, nodes.data_ptr<int64_t>(),
+    launch_init_seeds(seeds.data_ptr<int64_t>(), seeds.numel(), opt_ptr<int32_t>(n_dev), table->ht, nodes.data_ptr<int64_t>(),
                       seed_local.data_ptr<int32_t>(), scratch.data_ptr<int32_t>(), bc(),
                       (use_dev_step && step_inc != 0) ? step.data_ptr<int32_t>() : nullptr,
                       static_cast<int>(step_inc), s);
@@ -469,12 +538,14 @@ struct HeteroArena {
     c10::cuda::CUDAGuard guard(device);
     TORCH_CHECK(n_rel >= 1 && static_cast<int>(key_type.size()) == n_rel && static_cast<int>(nbr_type.size()) == n_rel &&
                 static_cast<int>(fanouts.size()) == n_rel, "HeteroArena: one (graph, key type, nbr type, fanouts) per relation");
-    TORCH_CHECK(static_cast<int>(num_nodes.size()) == n_types && static_cast<int>(max_seeds.size()) == n_types);
+    TORCH_CHECK(static_cast<int>(num_nodes.size()) == n_types && static_cast<int>(max_seeds.size()) == n_types,
+                "HeteroArena: num_nodes and max_seeds need one entry per node type");
     hops = fanouts[0].size();
     TORCH_CHECK(hops >= 1 && hops <= 4, "1..4 hops supported by the arena");
     for (int r = 0; r < n_rel; ++r) {
       TORCH_CHECK(static_cast<int>(fanouts[r].size()) == hops, "all relations need the same number of hops");
-      TORCH_CHECK(key_type[r] >= 0 && key_type[r] < n_types && nbr_type[r] >= 0 && nbr_type[r] < n_types);
+      TORCH_CHECK(key_type[r] >= 0 && key_type[r] < n_types && nbr_type[r] >= 0 && nbr_type[r] < n_types,
+                  "HeteroArena: key and neighbour types must be in [0, n_types)");
       TORCH_CHECK(!with_edge || graphs[r]->has_eids, "graph has no edge ids");
       TORCH_CHECK(!weighted || graphs[r]->has_weights, "graph has no device edge weights");
       for (int h = 0; h < hops; ++h) {
@@ -608,7 +679,7 @@ struct HeteroArena {
   // seeds of one or more node types -> multi-hop sample of every relation; no host synchronisation
   void sample(const std::vector<int64_t>& seed_types, const std::vector<Tensor>& seeds, int64_t step_inc) {
     c10::cuda::CUDAGuard guard(device);
-    TORCH_CHECK(seed_types.size() == seeds.size() && !seeds.empty());
+    TORCH_CHECK(seed_types.size() == seeds.size() && !seeds.empty(), "HeteroArena.sample: one seed type per seed tensor");
     cudaStream_t s = cur_stream();
     int32_t* cbase = counters.data_ptr<int32_t>();
     cudaMemsetAsync(cbase, 0, sizeof(int32_t) * ctr_overflow(), s);          // every cum / cursor / edge counter
@@ -617,7 +688,8 @@ struct HeteroArena {
     for (size_t i = 0; i < seeds.size(); ++i) {
       const int t = static_cast<int>(seed_types[i]);
       const Tensor& sd = seeds[i];
-      TORCH_CHECK(t >= 0 && t < n_types && sd.is_cuda() && sd.scalar_type() == torch::kInt64 && sd.is_contiguous());
+      TORCH_CHECK(t >= 0 && t < n_types, "HeteroArena.sample: seed type outside [0, n_types)");
+      check_ids(sd, "HeteroArena.sample: seeds must be contiguous int64 on the arena's device");
       TORCH_CHECK(sd.numel() <= max_seeds[t], "more seeds than the arena was built for");
       BatchCounters c{cbase + ctr_type_base(t), cbase + ctr_overflow() + 1 /* scratch */, cbase + ctr_type_base(t) + 6,
                       cbase + ctr_overflow()};
@@ -732,15 +804,15 @@ struct RowTableHandle {
 
   Tensor gather(const Tensor& idx, const c10::optional<Tensor>& id2index, int64_t out_width) {
     c10::cuda::CUDAGuard guard(device);
-    TORCH_CHECK(idx.is_cuda() && idx.scalar_type() == torch::kInt64 && idx.is_contiguous());
+    check_ids(idx, "gather: idx must be contiguous int64 on the table's device");
+    if (has(id2index)) check_ids(*id2index, "gather: id2index must be contiguous int64 on the table's device");
     if (out_width <= 0) out_width = width;
-    TORCH_CHECK(out_width >= width);
+    TORCH_CHECK(out_width >= width, "gather: out_width must be at least the table's width");
     auto o = torch::TensorOptions().dtype(dtype).device(torch::kCUDA, device);
     Tensor out = out_width == width ? torch::empty({idx.numel(), width}, o)
                                     : torch::zeros({idx.numel(), out_width}, o);
-    const int64_t* map = (id2index.has_value() && id2index->defined()) ? id2index->data_ptr<int64_t>() : nullptr;
-    launch_gather_rows(tbl, idx.data_ptr<int64_t>(), map, idx.numel(), nullptr, out.data_ptr(),
-                       out_width * out.element_size(), cur_stream(), map ? id2index->numel() : 0);
+    launch_gather_rows(tbl, idx.data_ptr<int64_t>(), opt_ptr<int64_t>(id2index), idx.numel(), nullptr, out.data_ptr(),
+                       out_width * out.element_size(), cur_stream(), has(id2index) ? id2index->numel() : 0);
     check_cuda_err("gather_rows");
     return out;
   }
@@ -752,7 +824,7 @@ struct RowTableHandle {
     c10::cuda::CUDAGuard guard(device);
     TORCH_CHECK(dtype == torch::kUInt8 && d % 128 == 0 && width >= d + d / 32 && width % 16 == 0,
                 "gather_mxfp8: table must hold uint8 rows of d + d/32 (+pad) bytes, d a multiple of 128");
-    TORCH_CHECK(idx.is_cuda() && idx.scalar_type() == torch::kInt64 && idx.is_contiguous());
+    check_ids(idx, "gather_mxfp8: idx must be contiguous int64 on the table's device");
     Tensor out = torch::empty({idx.numel(), d}, torch::TensorOptions().dtype(torch::kBFloat16).device(torch::kCUDA, device));
     launch_gather_mxfp8(tbl, idx.data_ptr<int64_t>(), idx.numel(), d, out.data_ptr(), cur_stream());
     check_cuda_err("gather_mxfp8");
@@ -770,16 +842,15 @@ struct RowTableHandle {
     c10::cuda::CUDAGuard guard(device);
     TORCH_CHECK(d % 32 == 0 && d >= 32 && d <= 1024, "gather_mxfp8_into: d must be a multiple of 32 in [32, 1024]");
     TORCH_CHECK(holds_mxfp8(d), "gather_mxfp8_into: the table must hold uint8 rows of mxfp8_row_bytes(d) bytes");
-    TORCH_CHECK(idx.is_cuda() && idx.scalar_type() == torch::kInt64 && idx.is_contiguous(),
-                "gather_mxfp8_into: idx must be a contiguous int64 CUDA tensor");
-    TORCH_CHECK(out.is_cuda() && out.scalar_type() == torch::kBFloat16 && out.dim() == 2 && out.stride(1) == 1 &&
-                out.size(0) >= idx.numel() && out.size(1) >= d && out.stride(0) % 8 == 0 &&
-                reinterpret_cast<uintptr_t>(out.data_ptr()) % 16 == 0,
+    check_ids(idx, "gather_mxfp8_into: idx must be a contiguous int64 CUDA tensor");
+    if (has(id2index)) check_ids(*id2index, "gather_mxfp8_into: id2index must be contiguous int64 on the table's device");
+    if (has(n_dev)) check_counters(*n_dev, 0, "gather_mxfp8_into: n_dev must be int32 [>= 1] on the table's device");
+    check_block(out, torch::kBFloat16, 0, d,
                 "gather_mxfp8_into: destination must be bf16 [>= rows, >= d] with unit inner stride and 16-byte aligned rows");
-    const int64_t* map = (id2index.has_value() && id2index->defined()) ? id2index->data_ptr<int64_t>() : nullptr;
-    const int32_t* nd = (n_dev.has_value() && n_dev->defined()) ? n_dev->data_ptr<int32_t>() : nullptr;
-    launch_gather_mxfp8_rows(tbl, idx.data_ptr<int64_t>(), map, idx.numel(), nd, static_cast<int>(d), out.data_ptr(),
-                             out.stride(0) * 2, cur_stream(), map ? id2index->numel() : 0);
+    TORCH_CHECK(out.size(0) >= idx.numel(), "gather_mxfp8_into: destination must be bf16 [>= rows, >= d]");
+    launch_gather_mxfp8_rows(tbl, idx.data_ptr<int64_t>(), opt_ptr<int64_t>(id2index), idx.numel(),
+                             opt_ptr<int32_t>(n_dev), static_cast<int>(d), out.data_ptr(), out.stride(0) * 2, cur_stream(),
+                             has(id2index) ? id2index->numel() : 0);
     check_cuda_err("gather_mxfp8_into");
   }
 
@@ -787,12 +858,14 @@ struct RowTableHandle {
   void gather_into(const Tensor& idx, const c10::optional<Tensor>& id2index,
                    const c10::optional<Tensor>& n_dev, Tensor out) {
     c10::cuda::CUDAGuard guard(device);
-    const int64_t* map = (id2index.has_value() && id2index->defined()) ? id2index->data_ptr<int64_t>() : nullptr;
-    const int32_t* nd = (n_dev.has_value() && n_dev->defined()) ? n_dev->data_ptr<int32_t>() : nullptr;
-    TORCH_CHECK(out.dim() == 2 && out.stride(1) == 1 && out.size(0) >= idx.numel() && out.size(1) >= width &&
-                (out.stride(0) * out.element_size()) % 16 == 0, "gather_into: [rows, >= width] destination with unit inner stride");
-    launch_gather_rows(tbl, idx.data_ptr<int64_t>(), map, idx.numel(), nd, out.data_ptr(),
-                       out.stride(0) * out.element_size(), cur_stream(), map ? id2index->numel() : 0);
+    check_ids(idx, "gather_into: idx must be contiguous int64 on the table's device");
+    if (has(id2index)) check_ids(*id2index, "gather_into: id2index must be contiguous int64 on the table's device");
+    if (has(n_dev)) check_counters(*n_dev, 0, "gather_into: n_dev must be int32 [>= 1] on the table's device");
+    check_block(out, dtype, 0, width, "gather_into: [rows, >= width] destination of the table's dtype with unit inner stride");
+    TORCH_CHECK(out.size(0) >= idx.numel(), "gather_into: [rows, >= width] destination with a row per id");
+    launch_gather_rows(tbl, idx.data_ptr<int64_t>(), opt_ptr<int64_t>(id2index), idx.numel(), opt_ptr<int32_t>(n_dev),
+                       out.data_ptr(), out.stride(0) * out.element_size(), cur_stream(),
+                       has(id2index) ? id2index->numel() : 0);
     check_cuda_err("gather_into");
   }
 };
@@ -800,16 +873,24 @@ struct RowTableHandle {
 // ---------------------------------------------------------------------------
 // GraphSAGE engine kernels
 // ---------------------------------------------------------------------------
-static void fill_ell(const std::vector<Tensor>& ell, const std::vector<int64_t>& ks,
-                     const int32_t** out_ell, int* out_k) {
-  TORCH_CHECK(ell.size() == ks.size() && ell.size() <= 4);
+// The ELL blocks of the hops and the degree array: int32, contiguous, on the device.  Returns deg's pointer.
+static const int32_t* fill_ell(const std::vector<Tensor>& ell, const std::vector<int64_t>& ks, const Tensor& deg,
+                               const int32_t** out_ell, int* out_k) {
+  TORCH_CHECK(ell.size() == ks.size() && ell.size() <= 4, "ell and ks need one entry per hop, at most 4");
+  TORCH_CHECK(on_dev(deg) && deg.scalar_type() == torch::kInt32 && deg.is_contiguous(),
+              "deg must be contiguous int32 on the device");
   for (size_t i = 0; i < 4; ++i) { out_ell[i] = nullptr; out_k[i] = 1; }
-  for (size_t i = 0; i < ell.size(); ++i) { out_ell[i] = ell[i].data_ptr<int32_t>(); out_k[i] = ks[i]; }
+  for (size_t i = 0; i < ell.size(); ++i) {
+    TORCH_CHECK(on_dev(ell[i]) && ell[i].scalar_type() == torch::kInt32 && ell[i].is_contiguous(),
+                "ELL blocks must be contiguous int32 on the device");
+    out_ell[i] = ell[i].data_ptr<int32_t>();
+    out_k[i] = ks[i];
+  }
+  return deg.data_ptr<int32_t>();
 }
 
 // The aggregation / scatter kernels cover at most 128 16-byte vectors per row, i.e. 1024 bf16 columns (the lane-group
 // dispatch, dispatch_lanes in csrc/cuda/launch_utils.h).
-// `msg` is one string: a TORCH_CHECK message assembled from several arguments crashes this extension when thrown.
 static void check_sage_width(int64_t d, const char* msg) {
   TORCH_CHECK(d % 8 == 0 && d >= 8 && d <= 1024, msg);
 }
@@ -827,23 +908,24 @@ static SageAggArgs make_agg(RowTableHandle* feat, const c10::optional<Tensor>& n
                             int64_t n_hops_targets, int64_t cap_targets, const std::vector<Tensor>& ell,
                             const std::vector<int64_t>& ks, const Tensor& deg, void* out) {
   SageAggArgs a{};
-  if (src_local.has_value() && src_local->defined()) {
-    TORCH_CHECK(src_local->scalar_type() == torch::kBFloat16 && src_local->is_contiguous());
+  if (has(src_local)) {
+    check_rows(*src_local, torch::kBFloat16, d, "aggregation: src_local must be contiguous bf16 [rows, d]");
     a.src_local = src_local->data_ptr();
   } else {
-    TORCH_CHECK(feat != nullptr && nodes.has_value(), "layer-1 aggregation needs a feature table + nodes");
+    TORCH_CHECK(feat != nullptr && has(nodes), "layer-1 aggregation needs a feature table + nodes");
     check_feature_table(feat, d);
+    check_ids(*nodes, "aggregation: nodes must be contiguous int64 on the device");
     a.feat = feat->tbl;
     a.feat_fp8 = feat->dtype == torch::kUInt8 ? 1 : 0;
     a.nodes = nodes->data_ptr<int64_t>();
   }
   TORCH_CHECK(d % 8 == 0, "feature width must be a multiple of 8");
+  check_counters(counters, n_hops_targets, "aggregation: counters must be int32 [> n_hops_targets] on the device");
   a.d = d;
   a.cum = counters.data_ptr<int32_t>();
   a.n_hops_targets = n_hops_targets;
   a.cap_targets = cap_targets;
-  fill_ell(ell, ks, a.ell, a.k);
-  a.deg = deg.data_ptr<int32_t>();
+  a.deg = fill_ell(ell, ks, deg, a.ell, a.k);
   a.out = out;
   return a;
 }
@@ -854,7 +936,7 @@ static void sage_aggregate(RowTableHandle* feat, const c10::optional<Tensor>& no
                            const std::vector<int64_t>& ks, const Tensor& deg, Tensor out) {
   c10::cuda::CUDAGuard guard(out.device());
   check_sage_width(d, "sage_aggregate: d must be a multiple of 8 in [8, 1024]");
-  TORCH_CHECK(out.scalar_type() == torch::kBFloat16 && out.is_contiguous() && out.size(1) == 2 * d);
+  check_rows(out, torch::kBFloat16, 2 * d, "sage_aggregate: out must be contiguous bf16 [rows, 2d]");
   SageAggArgs a = make_agg(feat, nodes, src_local, d, counters, n_hops_targets, out.size(0), ell, ks,
                            deg, out.data_ptr());
   launch_sage_aggregate(a, cur_stream());
@@ -868,8 +950,8 @@ static void sage_aggregate_block(RowTableHandle* feat, const c10::optional<Tenso
                                  const std::vector<int64_t>& ks, const Tensor& deg, Tensor out, int64_t mean_col) {
   c10::cuda::CUDAGuard guard(out.device());
   check_sage_width(d, "sage_aggregate_block: d must be a multiple of 8 in [8, 1024]");
-  TORCH_CHECK(out.scalar_type() == torch::kBFloat16 && out.dim() == 2 && out.stride(1) == 1 &&
-              mean_col >= 0 && mean_col % 8 == 0 && mean_col + d <= out.size(1) && out.stride(0) % 8 == 0);
+  check_block(out, torch::kBFloat16, mean_col, d,
+              "sage_aggregate_block: out must be a bf16 view with 16-byte aligned rows holding columns [mean_col, mean_col + d)");
   SageAggArgs a = make_agg(feat, nodes, src_local, d, counters, n_hops_targets, out.size(0), ell, ks,
                            deg, out.data_ptr());
   a.out_ld = static_cast<int>(out.stride(0));
@@ -884,17 +966,17 @@ static void sage_scatter_block(const Tensor& dA, int64_t d, int64_t mean_col, co
                                const std::vector<int64_t>& ks, const Tensor& deg, Tensor dH) {
   c10::cuda::CUDAGuard guard(dA.device());
   check_sage_width(d, "sage_scatter_block: d must be a multiple of 8 in [8, 1024]");
-  TORCH_CHECK(dA.scalar_type() == torch::kBFloat16 && dA.dim() == 2 && dA.stride(1) == 1 && dA.stride(0) % 8 == 0 &&
-              mean_col >= 0 && mean_col % 8 == 0 && mean_col + d <= dA.size(1));
-  TORCH_CHECK(dH.scalar_type() == torch::kFloat32 && dH.is_contiguous() && dH.size(1) == d);
+  check_block(dA, torch::kBFloat16, mean_col, d,
+              "sage_scatter_block: dA must be a bf16 view with 16-byte aligned rows holding columns [mean_col, mean_col + d)");
+  check_rows(dH, torch::kFloat32, d, "sage_scatter_block: dH must be contiguous fp32 [rows, d]");
+  check_counters(counters, n_hops_targets, "sage_scatter_block: counters must be int32 [> n_hops_targets] on the device");
   SageScatterArgs a{};
   a.dA = dA.data_ptr();
   a.d = d;
   a.cum = counters.data_ptr<int32_t>();
   a.n_hops_targets = n_hops_targets;
   a.cap_targets = dA.size(0);
-  fill_ell(ell, ks, a.ell, a.k);
-  a.deg = deg.data_ptr<int32_t>();
+  a.deg = fill_ell(ell, ks, deg, a.ell, a.k);
   a.dH = dH.data_ptr<float>();
   a.dA_ld = static_cast<int>(dA.stride(0));
   a.mean_col = static_cast<int>(mean_col);
@@ -910,13 +992,13 @@ static void sage_full_aggregate(GraphHandle* graph, RowTableHandle* feat, const 
   c10::cuda::CUDAGuard guard(out.device());
   TORCH_CHECK(graph != nullptr && graph->tbl.num_parts > 0, "sage_full_aggregate: graph has no shards");
   TORCH_CHECK(!(combine && mean_only), "sage_full_aggregate: mean_only writes the mean block of the concat mode, not combine");
-  TORCH_CHECK(d % 8 == 0 && d >= 8 && d <= 1024, "sage_full_aggregate: d must be a multiple of 8 in [8, 1024]");
+  check_sage_width(d, "sage_full_aggregate: d must be a multiple of 8 in [8, 1024]");
   TORCH_CHECK(0 <= r0 && r0 <= r1 && r1 <= graph->num_rows, "sage_full_aggregate: rows [r0, r1) outside the graph");
-  TORCH_CHECK(out.is_cuda() && out.scalar_type() == torch::kBFloat16 && out.dim() == 2 && out.stride(1) == 1 &&
-              out.stride(0) % 8 == 0 && reinterpret_cast<uintptr_t>(out.data_ptr()) % 16 == 0 &&
-              out.size(0) >= r1 - r0 && out.size(1) >= (combine || mean_only ? d : 2 * d),
-              combine || mean_only ? "sage_full_aggregate: out must be bf16 [>= r1 - r0, >= d] with unit inner stride and 16-byte aligned rows"
-                                   : "sage_full_aggregate: out must be bf16 [>= r1 - r0, >= 2d] with unit inner stride and 16-byte aligned rows");
+  const char* out_msg = combine || mean_only
+      ? "sage_full_aggregate: out must be bf16 [>= r1 - r0, >= d] with unit inner stride and 16-byte aligned rows"
+      : "sage_full_aggregate: out must be bf16 [>= r1 - r0, >= 2d] with unit inner stride and 16-byte aligned rows";
+  check_block(out, torch::kBFloat16, 0, combine || mean_only ? d : 2 * d, out_msg);
+  TORCH_CHECK(out.size(0) >= r1 - r0, out_msg);
   SageFullAggArgs a{};
   a.g = graph->tbl;
   a.d = static_cast<int>(d);
@@ -926,14 +1008,13 @@ static void sage_full_aggregate(GraphHandle* graph, RowTableHandle* feat, const 
   a.out = out.data_ptr();
   a.out_ld = out.stride(0);
   a.mean_only = mean_only ? 1 : 0;
-  if (src.has_value() && src->defined()) {
-    TORCH_CHECK(src->is_cuda() && src->scalar_type() == torch::kBFloat16 && src->dim() == 2 && src->stride(1) == 1 &&
-                src->stride(0) % 8 == 0 && reinterpret_cast<uintptr_t>(src->data_ptr()) % 16 == 0,
-                "sage_full_aggregate: src must be a bf16 CUDA table with unit inner stride and 16-byte aligned rows");
+  if (has(src)) {
+    const char* src_msg = "sage_full_aggregate: src must be a bf16 CUDA table with unit inner stride and 16-byte aligned "
+                          "rows, and column blocks [src_col, src_col + d), [self_col, self_col + d) inside them";
+    check_block(*src, torch::kBFloat16, src_col, d, src_msg);
+    check_block(*src, torch::kBFloat16, self_col, d, src_msg);
     // (mean only: src is the source type's table, read only at neighbour ids -- those outside it read as zero rows)
     TORCH_CHECK(mean_only || src->size(0) >= graph->num_rows, "sage_full_aggregate: src needs one row per graph node");
-    TORCH_CHECK(src_col >= 0 && src_col % 8 == 0 && src_col + d <= src->size(1) && self_col >= 0 && self_col % 8 == 0 &&
-                self_col + d <= src->size(1), "sage_full_aggregate: column blocks outside src");
     a.src = src->data_ptr();
     a.n_src = src->size(0);
     a.src_ld = src->stride(0);
@@ -946,10 +1027,8 @@ static void sage_full_aggregate(GraphHandle* graph, RowTableHandle* feat, const 
     a.feat = feat->tbl;
     a.feat_fp8 = feat->dtype == torch::kUInt8 ? 1 : 0;
   }
-  if (combine && bias.has_value() && bias->defined()) {
-    TORCH_CHECK(bias->is_cuda() && bias->scalar_type() == torch::kBFloat16 && bias->numel() == d &&
-                bias->is_contiguous() && reinterpret_cast<uintptr_t>(bias->data_ptr()) % 16 == 0,
-                "sage_full_aggregate: bias must be a 16-byte aligned bf16 [d] CUDA tensor");
+  if (combine && has(bias)) {
+    check_vec(*bias, torch::kBFloat16, d, "sage_full_aggregate: bias must be a 16-byte aligned bf16 [d] CUDA tensor");
     a.bias = bias->data_ptr();
   }
   a.relu = relu ? 1 : 0;
@@ -959,9 +1038,11 @@ static void sage_full_aggregate(GraphHandle* graph, RowTableHandle* feat, const 
 
 static void add_block_f32(const Tensor& dA, int64_t col, int64_t d, const Tensor& counters, int64_t n_hops, Tensor dH) {
   c10::cuda::CUDAGuard guard(dA.device());
-  TORCH_CHECK(dA.scalar_type() == torch::kBFloat16 && dA.dim() == 2 && dA.stride(1) == 1 && dA.stride(0) % 8 == 0 &&
-              col % 8 == 0 && col + d <= dA.size(1) && d % 8 == 0);
-  TORCH_CHECK(dH.scalar_type() == torch::kFloat32 && dH.is_contiguous() && dH.size(1) == d);
+  TORCH_CHECK(d % 8 == 0, "add_block_f32: d must be a multiple of 8");
+  check_block(dA, torch::kBFloat16, col, d,
+              "add_block_f32: dA must be a bf16 view with 16-byte aligned rows holding columns [col, col + d)");
+  check_rows(dH, torch::kFloat32, d, "add_block_f32: dH must be contiguous fp32 [rows, d]");
+  check_counters(counters, n_hops, "add_block_f32: counters must be int32 [> n_hops] on the device");
   launch_add_block_f32(dA.data_ptr(), dA.stride(0), col, d, counters.data_ptr<int32_t>(), n_hops,
                        std::min<int64_t>(dA.size(0), dH.size(0)), dH.data_ptr<float>(), cur_stream());
   check_cuda_err("add_block_f32");
@@ -973,9 +1054,11 @@ static void sage_gather_bwd(const Tensor& dA, int64_t d, SamplerArena& ar, int64
                             bool prezeroed, double gscale) {
   c10::cuda::CUDAGuard guard(dA.device());
   TORCH_CHECK(ar.tr_hops >= n_hops_targets && n_hops_targets >= 1, "enable_transpose(n_hops) covers too few hops");
-  TORCH_CHECK(dA.scalar_type() == torch::kBFloat16 && dA.is_contiguous() && dA.size(1) == 2 * d && d % 8 == 0);
-  TORCH_CHECK(dPre.scalar_type() == torch::kBFloat16 && dPre.is_contiguous() && dPre.size(1) == d);
-  TORCH_CHECK(d <= 1024, "sage_gather_bwd: d <= 1024");
+  TORCH_CHECK(ar.device == dA.get_device(), "sage_gather_bwd: dA must be on the arena's device");
+  check_sage_width(d, "sage_gather_bwd: d must be a multiple of 8 in [8, 1024]");
+  check_rows(dA, torch::kBFloat16, 2 * d, "sage_gather_bwd: dA must be contiguous bf16 [rows, 2d]");
+  check_rows(dPre, torch::kBFloat16, d, "sage_gather_bwd: dPre must be contiguous bf16 [rows, d]");
+  TORCH_CHECK(dPre.size(0) <= ar.cap_nodes, "dPre has more rows than the arena has nodes");
   SageGatherBwdArgs a{};
   a.dA = dA.data_ptr();
   a.d = static_cast<int>(d);
@@ -983,7 +1066,6 @@ static void sage_gather_bwd(const Tensor& dA, int64_t d, SamplerArena& ar, int64
   a.n_hops_targets = static_cast<int>(n_hops_targets);
   a.cap_targets = static_cast<int>(dA.size(0));
   a.cap_src = static_cast<int>(dPre.size(0));
-  TORCH_CHECK(a.cap_src <= ar.cap_nodes, "dPre has more rows than the arena has nodes");
   a.deg = ar.deg.data_ptr<int32_t>();
   a.off = ar.tr_off.data_ptr<int32_t>();
   a.cnt_upto = ar.tr_cnt.data_ptr<int32_t>() + (n_hops_targets - 1) * ar.cap_nodes;
@@ -991,15 +1073,16 @@ static void sage_gather_bwd(const Tensor& dA, int64_t d, SamplerArena& ar, int64
   a.meta = ar.tr_meta.data_ptr<int32_t>();
   a.meta_inv = ar.tr_meta_inv.data_ptr<float>();
   a.Z = nullptr;
-  if (Z.has_value() && Z->defined()) {
-    TORCH_CHECK(Z->scalar_type() == torch::kBFloat16 && Z->is_contiguous() && Z->size(1) == d && Z->size(0) >= dPre.size(0));
+  if (has(Z)) {
+    check_rows(*Z, torch::kBFloat16, d, "sage_gather_bwd: Z must be contiguous bf16 [rows, d]");
+    TORCH_CHECK(Z->size(0) >= dPre.size(0), "sage_gather_bwd: Z has fewer rows than dPre");
     a.Z = Z->data_ptr();
   }
   a.dPre = dPre.data_ptr();
   a.colsum = nullptr;
-  if (colsum.has_value() && colsum->defined()) {
-    TORCH_CHECK(colsum->scalar_type() == torch::kFloat32 && colsum->numel() >= d && d % 4 == 0 &&
-                reinterpret_cast<uintptr_t>(colsum->data_ptr()) % 16 == 0, "colsum: fp32 [d], 16-byte aligned");
+  if (has(colsum)) {
+    TORCH_CHECK(d % 4 == 0 && colsum->numel() >= d, "colsum: fp32 [d], 16-byte aligned");
+    check_vec(*colsum, torch::kFloat32, colsum->numel(), "colsum: fp32 [d], 16-byte aligned");
     a.colsum = colsum->data_ptr<float>();
   }
   a.colsum_prezeroed = prezeroed ? 1 : 0;
@@ -1012,17 +1095,16 @@ static void sage_gather_bwd(const Tensor& dA, int64_t d, SamplerArena& ar, int64
 static int64_t relu_bwd_cast(const Tensor& dH, const Tensor& Z, const Tensor& counters, int64_t n_hops,
                              Tensor dPre, const c10::optional<Tensor>& colsum, bool prezeroed, double gscale, bool relu) {
   c10::cuda::CUDAGuard guard(dH.device());
-  TORCH_CHECK(dPre.size(0) <= dH.size(0) && dPre.size(0) <= Z.size(0) && dPre.size(1) % 8 == 0);
-  TORCH_CHECK(dH.scalar_type() == torch::kFloat32 && Z.scalar_type() == torch::kBFloat16 &&
-              dPre.scalar_type() == torch::kBFloat16, "relu_bwd_cast: dH fp32, Z/dPre bf16");
-  TORCH_CHECK(dH.is_contiguous() && Z.is_contiguous() && dPre.is_contiguous() && dH.size(1) == dPre.size(1) &&
-              Z.size(1) == dPre.size(1), "relu_bwd_cast: contiguous [rows, d] operands of equal width");
-  const bool has_colsum = colsum.has_value() && colsum->defined();
-  TORCH_CHECK(!has_colsum || (colsum->scalar_type() == torch::kFloat32 && colsum->is_contiguous() &&
-                              colsum->numel() == dPre.size(1)), "relu_bwd_cast: colsum must be fp32 [d]");
+  const int64_t d = dPre.dim() == 2 ? dPre.size(1) : 0;
+  TORCH_CHECK(d % 8 == 0, "relu_bwd_cast: width must be a multiple of 8");
+  check_rows(dH, torch::kFloat32, d, "relu_bwd_cast: dH must be contiguous fp32 [rows, d]");
+  check_rows(Z, torch::kBFloat16, d, "relu_bwd_cast: Z must be contiguous bf16 [rows, d]");
+  check_rows(dPre, torch::kBFloat16, d, "relu_bwd_cast: dPre must be contiguous bf16 [rows, d]");
+  TORCH_CHECK(dPre.size(0) <= dH.size(0) && dPre.size(0) <= Z.size(0), "relu_bwd_cast: dH / Z have fewer rows than dPre");
+  check_counters(counters, n_hops, "relu_bwd_cast: counters must be int32 [> n_hops] on the device");
+  if (has(colsum)) check_vec(*colsum, torch::kFloat32, d, "relu_bwd_cast: colsum must be fp32 [d]");
   const int n = launch_relu_bwd_cast(dH.data_ptr<float>(), Z.data_ptr(), counters.data_ptr<int32_t>(), n_hops,
-                                     dPre.size(0), dPre.size(1), dPre.data_ptr(),
-                                     has_colsum ? colsum->data_ptr<float>() : nullptr, cur_stream(),
+                                     dPre.size(0), d, dPre.data_ptr(), opt_ptr<float>(colsum), cur_stream(),
                                      prezeroed, static_cast<float>(gscale), relu);
   check_cuda_err("relu_bwd_cast");
   return n;
@@ -1030,18 +1112,10 @@ static int64_t relu_bwd_cast(const Tensor& dH, const Tensor& Z, const Tensor& co
 
 // ---- relational GAT (cuda/gat.cu) -------------------------------------------------------------------------------
 // H = heads * C must be a multiple of 64 in [64, 1024] (the lane-group dispatch covers 1024 columns, see
-// check_sage_width) with C a multiple of 8 (one 16-byte vector never straddles two heads).  Messages are single
-// strings (see check_sage_width).
+// check_sage_width) with C a multiple of 8 (one 16-byte vector never straddles two heads).
 static void check_gat_width(int64_t H, int64_t heads) {
   TORCH_CHECK(H % 64 == 0 && H >= 64 && H <= 1024 && heads >= 1 && H % heads == 0 && (H / heads) % 8 == 0,
               "gat: H must be a multiple of 64 in [64, 1024] and heads must divide H into head widths C with C % 8 == 0");
-}
-
-static bool has(const c10::optional<Tensor>& t) { return t.has_value() && t->defined(); }
-
-static void check_rows(const Tensor& t, c10::ScalarType dt, int64_t w, const char* msg) {
-  TORCH_CHECK(t.is_cuda() && t.scalar_type() == dt && t.dim() == 2 && t.size(1) == w && t.is_contiguous() &&
-              reinterpret_cast<uintptr_t>(t.data_ptr()) % 16 == 0, msg);
 }
 
 static void gat_fill_hops(const std::vector<Tensor>& ell, const std::vector<int64_t>& ks, const std::vector<Tensor>& bufs,
@@ -1049,7 +1123,7 @@ static void gat_fill_hops(const std::vector<Tensor>& ell, const std::vector<int6
   TORCH_CHECK(bufs.size() == ell.size(), "gat: one alpha buffer per hop");
   for (size_t h = 0; h < 4; ++h) out[h] = nullptr;
   for (size_t h = 0; h < bufs.size(); ++h) {
-    TORCH_CHECK(bufs[h].is_cuda() && bufs[h].scalar_type() == torch::kFloat32 && bufs[h].is_contiguous() &&
+    TORCH_CHECK(on_dev(bufs[h]) && bufs[h].scalar_type() == torch::kFloat32 && bufs[h].is_contiguous() &&
                 bufs[h].numel() >= ell[h].numel() * heads, "gat: alpha buffers must be fp32 [ELL slots of the hop, heads]");
     out[h] = bufs[h].data_ptr<float>();
   }
@@ -1067,18 +1141,18 @@ static void gat_scores(const Tensor& P0, const Tensor& att0, Tensor out0, const 
   a.H = H; a.heads = heads;
   check_rows(P0, torch::kBFloat16, H, "gat_scores: P must be contiguous bf16 [rows, H]");
   check_rows(out0, torch::kFloat32, heads, "gat_scores: out must be contiguous fp32 [rows, heads]");
-  TORCH_CHECK(att0.scalar_type() == torch::kBFloat16 && att0.numel() == H && att0.is_contiguous() &&
-              reinterpret_cast<uintptr_t>(att0.data_ptr()) % 16 == 0, "gat_scores: att must be 16-byte aligned bf16 [H]");
+  check_vec(att0, torch::kBFloat16, H, "gat_scores: att must be 16-byte aligned bf16 [H]");
   TORCH_CHECK(out0.size(0) >= P0.size(0), "gat_scores: out has fewer rows than P");
+  check_counters(counters0, idx0, "gat_scores: counters must be int32 [> idx] on the device");
   a.P[0] = P0.data_ptr(); a.att[0] = att0.data_ptr(); a.out[0] = out0.data_ptr<float>();
   a.cum[0] = counters0.data_ptr<int32_t>(); a.idx[0] = idx0; a.cap[0] = P0.size(0);
   if (has(P1)) {
     TORCH_CHECK(has(att1) && has(out1) && has(counters1), "gat_scores: the second set needs P, att, out and counters");
     check_rows(*P1, torch::kBFloat16, H, "gat_scores: P must be contiguous bf16 [rows, H]");
     check_rows(*out1, torch::kFloat32, heads, "gat_scores: out must be contiguous fp32 [rows, heads]");
-    TORCH_CHECK(att1->scalar_type() == torch::kBFloat16 && att1->numel() == H && att1->is_contiguous() &&
-                reinterpret_cast<uintptr_t>(att1->data_ptr()) % 16 == 0, "gat_scores: att must be 16-byte aligned bf16 [H]");
+    check_vec(*att1, torch::kBFloat16, H, "gat_scores: att must be 16-byte aligned bf16 [H]");
     TORCH_CHECK(out1->size(0) >= P1->size(0), "gat_scores: out has fewer rows than P");
+    check_counters(*counters1, idx1, "gat_scores: counters must be int32 [> idx] on the device");
     a.P[1] = P1->data_ptr(); a.att[1] = att1->data_ptr(); a.out[1] = out1->data_ptr<float>();
     a.cum[1] = counters1->data_ptr<int32_t>(); a.idx[1] = idx1; a.cap[1] = P1->size(0);
   } else {
@@ -1107,14 +1181,14 @@ static void gat_aggregate(const Tensor& P, const Tensor& as, const Tensor& ad, i
   check_rows(ad, torch::kFloat32, heads, "gat_aggregate: ad must be contiguous fp32 [rows, heads]");
   TORCH_CHECK(as.size(0) >= P.size(0), "gat_aggregate: as has fewer rows than P");
   TORCH_CHECK(p >= 0.0 && p < 1.0, "gat_aggregate: dropout p must be in [0, 1)");
+  check_counters(counters, n_hops_targets, "gat_aggregate: counters must be int32 [> n_hops_targets] on the device");
   GatAggArgs a{};
   a.P = P.data_ptr(); a.as = as.data_ptr<float>(); a.ad = ad.data_ptr<float>();
   a.H = H; a.heads = heads;
   a.cum = counters.data_ptr<int32_t>();
   a.n_hops_targets = n_hops_targets;
   int64_t cap = ad.size(0);
-  fill_ell(ell, ks, a.ell, a.k);
-  a.deg = deg.data_ptr<int32_t>();
+  a.deg = fill_ell(ell, ks, deg, a.ell, a.k);
   gat_fill_hops(ell, ks, alpha, heads, a.alpha);
   a.first = first ? 1 : 0; a.last = last ? 1 : 0;
   if (!(first && last)) {
@@ -1129,9 +1203,8 @@ static void gat_aggregate(const Tensor& P, const Tensor& as, const Tensor& ad, i
     cap = std::min<int64_t>(cap, Z->size(0));
     a.z = Z->data_ptr();
     if (has(bias)) {
-      TORCH_CHECK(bias->is_cuda() && bias->scalar_type() == torch::kBFloat16 && bias->is_contiguous() &&
-                  bias->numel() % H == 0 && reinterpret_cast<uintptr_t>(bias->data_ptr()) % 16 == 0,
-                  "gat_aggregate: bias must be 16-byte aligned bf16 [n_bias * H]");
+      TORCH_CHECK(bias->numel() % H == 0, "gat_aggregate: bias must be 16-byte aligned bf16 [n_bias * H]");
+      check_vec(*bias, torch::kBFloat16, bias->numel(), "gat_aggregate: bias must be 16-byte aligned bf16 [n_bias * H]");
       a.bias = bias->data_ptr();
       a.n_bias = bias->numel() / H;
     }
@@ -1141,7 +1214,7 @@ static void gat_aggregate(const Tensor& P, const Tensor& as, const Tensor& ad, i
     a.seed = static_cast<uint64_t>(seed);
     a.layer = layer;
     if (has(step_dev)) {
-      TORCH_CHECK(step_dev->scalar_type() == torch::kInt32 && step_dev->is_cuda(), "gat_aggregate: int32 step_dev");
+      check_counters(*step_dev, 0, "gat_aggregate: int32 step_dev");
       a.step_dev = step_dev->data_ptr<int32_t>();
     }
   }
@@ -1163,13 +1236,13 @@ static void gat_backward(const Tensor& G, const Tensor& P, int64_t heads, const 
   check_rows(da_src, torch::kFloat32, heads, "gat_backward: da_src must be contiguous fp32 [rows, heads]");
   check_rows(da_dst, torch::kFloat32, heads, "gat_backward: da_dst must be contiguous fp32 [rows, heads]");
   TORCH_CHECK(dP.size(0) >= P.size(0) && da_src.size(0) >= P.size(0), "gat_backward: dP / da_src have fewer rows than P");
+  check_counters(counters, n_hops_targets, "gat_backward: counters must be int32 [> n_hops_targets] on the device");
   GatBwdArgs a{};
   a.G = G.data_ptr(); a.P = P.data_ptr(); a.H = H; a.heads = heads;
   a.cum = counters.data_ptr<int32_t>();
   a.n_hops_targets = n_hops_targets;
   a.cap_targets = std::min<int64_t>(G.size(0), da_dst.size(0));
-  fill_ell(ell, ks, a.ell, a.k);
-  a.deg = deg.data_ptr<int32_t>();
+  a.deg = fill_ell(ell, ks, deg, a.ell, a.k);
   float* al[4];
   gat_fill_hops(ell, ks, alpha, heads, al);
   for (int h = 0; h < 4; ++h) a.alpha[h] = al[h];
@@ -1196,11 +1269,11 @@ static void gat_score_bwd(const Tensor& P_src, const Tensor& dP_src, const Tenso
   TORCH_CHECK(dP_src.size(0) >= P_src.size(0) && dPb_src.size(0) >= P_src.size(0) && da_src.size(0) >= P_src.size(0),
               "gat_score_bwd: source buffers have fewer rows than P");
   for (const Tensor* t : {&att_src, &att_dst})
-    TORCH_CHECK(t->scalar_type() == torch::kBFloat16 && t->numel() == H && t->is_contiguous() &&
-                reinterpret_cast<uintptr_t>(t->data_ptr()) % 16 == 0, "gat_score_bwd: att must be 16-byte aligned bf16 [H]");
+    check_vec(*t, torch::kBFloat16, H, "gat_score_bwd: att must be 16-byte aligned bf16 [H]");
   for (const Tensor* t : {&g_att_src, &g_att_dst})
-    TORCH_CHECK(t->scalar_type() == torch::kFloat32 && t->numel() == H && t->is_contiguous(),
-                "gat_score_bwd: attention gradients must be fp32 [H]");
+    check_vec(*t, torch::kFloat32, H, "gat_score_bwd: attention gradients must be fp32 [H]");
+  check_counters(ctr_src, idx_src, "gat_score_bwd: ctr_src must be int32 [> idx_src] on the device");
+  check_counters(ctr_dst, idx_dst, "gat_score_bwd: ctr_dst must be int32 [> idx_dst] on the device");
   GatScoreBwdArgs a{};
   a.H = H; a.heads = heads;
   auto& s = a.seg[0];
@@ -1233,6 +1306,7 @@ static void gat_act_bwd(const c10::optional<Tensor>& dH, const c10::optional<Ten
   TORCH_CHECK(d % 64 == 0 && d >= 64 && d <= 1024, "gat_act_bwd: width must be a multiple of 64 in [64, 1024]");
   check_rows(dPre, torch::kBFloat16, d, "gat_act_bwd: dPre must be contiguous bf16 [rows, d]");
   TORCH_CHECK(p >= 0.0 && p < 1.0, "gat_act_bwd: dropout p must be in [0, 1)");
+  check_counters(counters, n_hops, "gat_act_bwd: counters must be int32 [> n_hops] on the device");
   GatActBwdArgs a{};
   a.dPre = dPre.data_ptr(); a.cum = counters.data_ptr<int32_t>(); a.n_hops = n_hops; a.cap = dPre.size(0); a.d = d;
   if (has(dH)) {
@@ -1248,12 +1322,12 @@ static void gat_act_bwd(const c10::optional<Tensor>& dH, const c10::optional<Ten
   a.seed = static_cast<uint64_t>(seed);
   a.layer = layer;
   if (has(step_dev)) {
-    TORCH_CHECK(step_dev->scalar_type() == torch::kInt32 && step_dev->is_cuda(), "gat_act_bwd: int32 step_dev");
+    check_counters(*step_dev, 0, "gat_act_bwd: int32 step_dev");
     a.step_dev = step_dev->data_ptr<int32_t>();
   }
   if (has(bias_g)) {
-    TORCH_CHECK(bias_g->is_cuda() && bias_g->scalar_type() == torch::kFloat32 && bias_g->is_contiguous() &&
-                bias_g->numel() % d == 0 && bias_g->numel() > 0, "gat_act_bwd: bias_g must be fp32 [n_bias * d]");
+    TORCH_CHECK(bias_g->numel() % d == 0 && bias_g->numel() > 0, "gat_act_bwd: bias_g must be fp32 [n_bias * d]");
+    check_vec(*bias_g, torch::kFloat32, bias_g->numel(), "gat_act_bwd: bias_g must be fp32 [n_bias * d]");
     a.bias_g = bias_g->data_ptr<float>();
     a.n_bias = bias_g->numel() / d;
   }
@@ -1275,14 +1349,11 @@ static void hgt_fill_rels(RelT* rel, int64_t H, int64_t heads, const std::vector
               "hgt: kv, prior, ell, ks, deg and alpha need one entry per relation");
   for (size_t r = 0; r < R; ++r) {
     check_rows(kv[r], torch::kBFloat16, 3 * H, "hgt: source rows must be contiguous bf16 [rows, 3H] = [K | Q | V]");
-    TORCH_CHECK(prior[r].is_cuda() && prior[r].scalar_type() == torch::kFloat32 && prior[r].numel() == heads &&
-                prior[r].is_contiguous(), "hgt: prior must be fp32 [heads]");
-    TORCH_CHECK(deg[r].is_cuda() && deg[r].scalar_type() == torch::kInt32, "hgt: deg must be int32");
+    check_vec(prior[r], torch::kFloat32, heads, "hgt: prior must be fp32 [heads]");
     TORCH_CHECK(static_cast<int64_t>(ell[r].size()) == n_hops, "hgt: one ELL block per target hop");
     rel[r].kv = kv[r].data_ptr();
     rel[r].prior = prior[r].data_ptr<float>();
-    rel[r].deg = deg[r].data_ptr<int32_t>();
-    fill_ell(ell[r], ks[r], rel[r].ell, rel[r].k);
+    rel[r].deg = fill_ell(ell[r], ks[r], deg[r], rel[r].ell, rel[r].k);
     float* al[4];
     gat_fill_hops(ell[r], ks[r], alpha[r], heads, al);
     for (int h = 0; h < 4; ++h) rel[r].alpha[h] = al[h];
@@ -1306,6 +1377,7 @@ static void hgt_attention(const Tensor& qq, Tensor u, int64_t heads, const Tenso
   check_hgt_width(H, heads);
   check_rows(qq, torch::kBFloat16, R * H, "hgt_attention: qq must be contiguous bf16 [rows, n_rel * H]");
   check_rows(u, torch::kBFloat16, R * H, "hgt_attention: u must be contiguous bf16 [rows, n_rel * H]");
+  check_counters(counters, n_hops_targets, "hgt_attention: counters must be int32 [> n_hops_targets] on the device");
   HgtAttnArgs a{};
   a.qq = qq.data_ptr(); a.u = u.data_ptr();
   a.H = H; a.heads = heads; a.n_rel = R; a.kv_ld = 3 * H; a.v_off = 2 * H;
@@ -1335,6 +1407,7 @@ static void hgt_attention_bwd(const Tensor& du, const Tensor& qq, Tensor dqq, in
   check_rows(dqq, torch::kBFloat16, R * H, "hgt_attention_bwd: dqq must be contiguous bf16 [rows, n_rel * H]");
   TORCH_CHECK(dal.size() == static_cast<size_t>(R) && dkv.size() == static_cast<size_t>(R) &&
               dprior.size() == static_cast<size_t>(R), "hgt_attention_bwd: dal, dkv and dprior need one entry per relation");
+  check_counters(counters, n_hops_targets, "hgt_attention_bwd: counters must be int32 [> n_hops_targets] on the device");
   HgtAttnBwdArgs a{};
   a.du = du.data_ptr(); a.qq = qq.data_ptr(); a.dqq = dqq.data_ptr();
   a.H = H; a.heads = heads; a.n_rel = R; a.kv_ld = 3 * H; a.v_off = 2 * H;
@@ -1347,7 +1420,7 @@ static void hgt_attention_bwd(const Tensor& du, const Tensor& qq, Tensor dqq, in
     TORCH_CHECK(dal[r].size() == ell[r].size(), "hgt_attention_bwd: one dal buffer per hop");
     for (size_t h = 0; h < 4; ++h) a.rel[r].dal[h] = nullptr;
     for (size_t h = 0; h < dal[r].size(); ++h) {
-      TORCH_CHECK(dal[r][h].is_cuda() && dal[r][h].scalar_type() == torch::kFloat32 && dal[r][h].is_contiguous() &&
+      TORCH_CHECK(on_dev(dal[r][h]) && dal[r][h].scalar_type() == torch::kFloat32 && dal[r][h].is_contiguous() &&
                   dal[r][h].numel() >= 2 * ell[r][h].numel() * heads &&
                   reinterpret_cast<uintptr_t>(dal[r][h].data_ptr()) % 8 == 0,
                   "hgt_attention_bwd: dal buffers must be fp32 [ELL slots of the hop, heads, 2]");
@@ -1355,8 +1428,7 @@ static void hgt_attention_bwd(const Tensor& du, const Tensor& qq, Tensor dqq, in
     }
     check_rows(dkv[r], torch::kFloat32, 2 * H, "hgt_attention_bwd: dkv must be contiguous fp32 [rows, 2H]");
     TORCH_CHECK(dkv[r].size(0) >= kv[r].size(0), "hgt_attention_bwd: dkv has fewer rows than the source rows");
-    TORCH_CHECK(dprior[r].is_cuda() && dprior[r].scalar_type() == torch::kFloat32 && dprior[r].numel() == heads,
-                "hgt_attention_bwd: dprior must be fp32 [heads]");
+    check_vec(dprior[r], torch::kFloat32, heads, "hgt_attention_bwd: dprior must be fp32 [heads]");
     a.rel[r].dkv = dkv[r].data_ptr<float>();
     a.rel[r].dprior = dprior[r].data_ptr<float>();
   }
@@ -1399,9 +1471,8 @@ static void gat_full_aggregate(GraphHandle* graph, const Tensor& P, const Tensor
     TORCH_CHECK(Z->size(0) >= r1 - r0, "gat_full_aggregate: Z needs r1 - r0 rows");
     a.z = Z->data_ptr();
     if (has(bias)) {
-      TORCH_CHECK(bias->is_cuda() && bias->scalar_type() == torch::kBFloat16 && bias->is_contiguous() &&
-                  bias->numel() % H == 0 && reinterpret_cast<uintptr_t>(bias->data_ptr()) % 16 == 0,
-                  "gat_full_aggregate: bias must be 16-byte aligned bf16 [n_bias * H]");
+      TORCH_CHECK(bias->numel() % H == 0, "gat_full_aggregate: bias must be 16-byte aligned bf16 [n_bias * H]");
+      check_vec(*bias, torch::kBFloat16, bias->numel(), "gat_full_aggregate: bias must be 16-byte aligned bf16 [n_bias * H]");
       a.bias = bias->data_ptr();
       a.n_bias = bias->numel() / H;
     }
@@ -1433,8 +1504,7 @@ static void hgt_full_attention(const std::vector<GraphHandle*>& graphs, const Te
     TORCH_CHECK(graphs[r] != nullptr && graphs[r]->tbl.num_parts > 0, "hgt_full_attention: graph has no shards");
     TORCH_CHECK(r1 <= graphs[r]->num_rows, "hgt_full_attention: rows [r0, r1) outside a relation graph");
     check_rows(kv[r], torch::kBFloat16, 3 * H, "hgt_full_attention: kv must be contiguous bf16 [rows, 3H]");
-    TORCH_CHECK(prior[r].is_cuda() && prior[r].scalar_type() == torch::kFloat32 && prior[r].numel() == heads &&
-                prior[r].is_contiguous(), "hgt_full_attention: prior must be fp32 [heads]");
+    check_vec(prior[r], torch::kFloat32, heads, "hgt_full_attention: prior must be fp32 [heads]");
     tbl[r] = graphs[r]->tbl;
     a.kv[r] = kv[r].data_ptr();
     a.n_src[r] = kv[r].size(0);
@@ -1460,13 +1530,14 @@ static void hgt_gelu(const Tensor& X, Tensor Y, const Tensor& counters, int64_t 
   TORCH_CHECK(d % 8 == 0, "hgt_gelu: width must be a multiple of 8");
   check_rows(X, torch::kBFloat16, d, "hgt_gelu: X must be contiguous bf16 [rows, d]");
   check_rows(Y, torch::kBFloat16, d, "hgt_gelu: Y must be contiguous bf16 [rows, d]");
+  check_counters(counters, n_hops, "hgt_gelu: counters must be int32 [> n_hops] on the device");
   int64_t cap = std::min<int64_t>(X.size(0), Y.size(0));
   if (has(dY)) {
     check_rows(*dY, torch::kBFloat16, d, "hgt_gelu: dY must be contiguous bf16 [rows, d]");
     cap = std::min<int64_t>(cap, dY->size(0));
   }
   launch_hgt_gelu(X.data_ptr(), Y.data_ptr(), counters.data_ptr<int32_t>(), n_hops, cap, d,
-                  has(dY) ? dY->data_ptr() : nullptr, cur_stream());
+                  opt_ptr(dY), cur_stream());
   check_cuda_err("hgt_gelu");
 }
 
@@ -1479,13 +1550,14 @@ static void hgt_gate(const Tensor& A, const Tensor& X, Tensor out, const Tensor&
   check_rows(A, torch::kBFloat16, d, "hgt_gate: A must be contiguous bf16 [rows, d]");
   check_rows(X, torch::kBFloat16, d, "hgt_gate: X must be contiguous bf16 [rows, d]");
   check_rows(out, torch::kBFloat16, d, "hgt_gate: out must be contiguous bf16 [rows, d]");
-  TORCH_CHECK(skip.is_cuda() && skip.scalar_type() == torch::kFloat32 && skip.numel() == 1, "hgt_gate: skip must be fp32 [1]");
+  check_vec(skip, torch::kFloat32, 1, "hgt_gate: skip must be fp32 [1]");
+  check_counters(counters, n_hops, "hgt_gate: counters must be int32 [> n_hops] on the device");
   HgtGateArgs a{};
   a.A = A.data_ptr(); a.X = X.data_ptr(); a.out = out.data_ptr(); a.skip = skip.data_ptr<float>();
   a.cum = counters.data_ptr<int32_t>(); a.n_hops = n_hops; a.d = d;
   int64_t cap = std::min<int64_t>(std::min<int64_t>(A.size(0), X.size(0)), out.size(0));
   if (has(dZ)) {
-    TORCH_CHECK(dZ->is_cuda() && dZ->is_contiguous() && dZ->dim() == 2 && dZ->size(1) == d &&
+    TORCH_CHECK(on_dev(*dZ) && dZ->is_contiguous() && dZ->dim() == 2 && dZ->size(1) == d &&
                 (dZ->scalar_type() == torch::kFloat32 || dZ->scalar_type() == torch::kBFloat16),
                 "hgt_gate: dZ must be contiguous fp32 or bf16 [rows, d]");
     cap = std::min<int64_t>(cap, dZ->size(0));
@@ -1496,8 +1568,7 @@ static void hgt_gate(const Tensor& A, const Tensor& X, Tensor out, const Tensor&
       a.dX = dX->data_ptr<float>();
     }
     if (has(skip_g)) {
-      TORCH_CHECK(skip_g->is_cuda() && skip_g->scalar_type() == torch::kFloat32 && skip_g->numel() == 1,
-                  "hgt_gate: skip_g must be fp32 [1]");
+      check_vec(*skip_g, torch::kFloat32, 1, "hgt_gate: skip_g must be fp32 [1]");
       a.skip_g = skip_g->data_ptr<float>();
     }
   }
@@ -1512,7 +1583,7 @@ static void hgt_blocks(const Tensor& att, const Tensor& msg, Tensor att_img, Ten
                        const c10::optional<Tensor>& att_dense, const c10::optional<Tensor>& msg_dense,
                        const c10::optional<Tensor>& att_g, const c10::optional<Tensor>& msg_g) {
   c10::cuda::CUDAGuard guard(att.device());
-  TORCH_CHECK(att.dim() == 4 && att.size(2) == att.size(3) && msg.sizes() == att.sizes() && att.is_contiguous() &&
+  TORCH_CHECK(on_dev(att) && on_dev(msg) && att.dim() == 4 && att.size(2) == att.size(3) && msg.sizes() == att.sizes() && att.is_contiguous() &&
               msg.is_contiguous() && att.scalar_type() == torch::kBFloat16 && msg.scalar_type() == torch::kBFloat16,
               "hgt_blocks: att and msg must be contiguous bf16 [n_rel, heads, D, D]");
   const int64_t R = att.size(0), heads = att.size(1), D = att.size(2), H = heads * D;
@@ -1527,10 +1598,10 @@ static void hgt_blocks(const Tensor& att, const Tensor& msg, Tensor att_img, Ten
   if (has(att_g)) {
     TORCH_CHECK(has(msg_g) && has(att_dense) && has(msg_dense), "hgt_blocks: the gradient map needs all four buffers");
     for (const Tensor* t : {&*att_g, &*msg_g})
-      TORCH_CHECK(t->is_cuda() && t->scalar_type() == torch::kFloat32 && t->is_contiguous() && t->numel() == R * H * D,
+      TORCH_CHECK(on_dev(*t) && t->scalar_type() == torch::kFloat32 && t->is_contiguous() && t->numel() == R * H * D,
                   "hgt_blocks: att_g / msg_g must be fp32 [n_rel, heads, D, D]");
     for (const Tensor* t : {&*att_dense, &*msg_dense})
-      TORCH_CHECK(t->is_cuda() && t->scalar_type() == torch::kFloat32 && t->is_contiguous() && t->numel() == R * H * H,
+      TORCH_CHECK(on_dev(*t) && t->scalar_type() == torch::kFloat32 && t->is_contiguous() && t->numel() == R * H * H,
                   "hgt_blocks: the dense gradients must be fp32 [n_rel * H, H] / [H, n_rel * H]");
     a.att_dense = att_dense->data_ptr<float>(); a.msg_dense = msg_dense->data_ptr<float>();
     a.att_g = att_g->data_ptr<float>(); a.msg_g = msg_g->data_ptr<float>();
@@ -1547,17 +1618,18 @@ static void hgt_kqv_cast(Tensor dkv, const c10::optional<Tensor>& dq, Tensor out
   TORCH_CHECK(H % 64 == 0 && H >= 64 && H <= 1024, "hgt_kqv_cast: H must be a multiple of 64 in [64, 1024]");
   check_rows(out, torch::kBFloat16, 3 * H, "hgt_kqv_cast: out must be contiguous bf16 [rows, 3H]");
   check_rows(dkv, torch::kFloat32, 2 * H, "hgt_kqv_cast: dkv must be contiguous fp32 [rows, 2H]");
+  check_counters(counters, idx, "hgt_kqv_cast: counters must be int32 [> idx] on the device");
   HgtKqvCastArgs a{};
   a.dkv = dkv.data_ptr<float>(); a.out = out.data_ptr(); a.cum = counters.data_ptr<int32_t>();
   a.idx = idx; a.idx_q = idx_q; a.H = H;
   a.cap = std::min<int64_t>(out.size(0), dkv.size(0));
   if (has(dq)) {
     check_rows(*dq, torch::kBFloat16, H, "hgt_kqv_cast: dq must be contiguous bf16 [rows, H]");
+    check_counters(counters, idx_q, "hgt_kqv_cast: counters must be int32 [> idx_q] on the device");
     a.dq = dq->data_ptr();
   }
   if (has(bias_g)) {
-    TORCH_CHECK(bias_g->is_cuda() && bias_g->scalar_type() == torch::kFloat32 && bias_g->numel() == 3 * H &&
-                bias_g->is_contiguous(), "hgt_kqv_cast: bias_g must be fp32 [3H]");
+    check_vec(*bias_g, torch::kFloat32, 3 * H, "hgt_kqv_cast: bias_g must be fp32 [3H]");
     a.bias_g = bias_g->data_ptr<float>();
   }
   launch_hgt_kqv_cast(a, cur_stream());
@@ -1570,18 +1642,17 @@ static void link_seeds(GraphHandle* graph, const Tensor& pos, int64_t num_nodes,
                        const Tensor& step, Tensor seeds, Tensor n_pairs) {
   c10::cuda::CUDAGuard guard(seeds.device());
   TORCH_CHECK(graph != nullptr && graph->tbl.num_parts > 0, "link_seeds: graph has no shards");
-  TORCH_CHECK(pos.is_cuda() && pos.scalar_type() == torch::kInt64 && pos.is_contiguous() && pos.dim() == 2 &&
+  TORCH_CHECK(on_dev(pos) && pos.scalar_type() == torch::kInt64 && pos.is_contiguous() && pos.dim() == 2 &&
               pos.size(0) == 2, "link_seeds: pos must be a contiguous int64 [2, B] CUDA tensor");
   TORCH_CHECK(neg_ratio >= 1, "link_seeds: neg_ratio must be >= 1");
   TORCH_CHECK(num_nodes >= 1 && num_nodes <= graph->num_rows && num_nodes < (1LL << 32),
               "link_seeds: num_nodes must be in [1, graph rows] and < 2^32");
   const int64_t B = pos.size(1), P = (1 + neg_ratio) * B;
   TORCH_CHECK(P < (1LL << 30), "link_seeds: batch too large");
-  TORCH_CHECK(seeds.is_cuda() && seeds.scalar_type() == torch::kInt64 && seeds.is_contiguous() &&
-              seeds.numel() == 2 * P, "link_seeds: seeds must be a contiguous int64 [2 (1 + k) B] CUDA tensor");
-  TORCH_CHECK(step.is_cuda() && step.scalar_type() == torch::kInt32 && step.numel() >= 1, "link_seeds: int32 step");
-  TORCH_CHECK(n_pairs.is_cuda() && n_pairs.scalar_type() == torch::kInt32 && n_pairs.numel() >= 1,
-              "link_seeds: int32 n_pairs");
+  check_ids(seeds, "link_seeds: seeds must be a contiguous int64 [2 (1 + k) B] CUDA tensor");
+  TORCH_CHECK(seeds.numel() == 2 * P, "link_seeds: seeds must be a contiguous int64 [2 (1 + k) B] CUDA tensor");
+  check_counters(step, 0, "link_seeds: int32 step");
+  check_counters(n_pairs, 0, "link_seeds: int32 n_pairs");
   launch_link_seeds(graph->tbl, pos.data_ptr<int64_t>(), static_cast<int>(B), static_cast<int>(neg_ratio), num_nodes,
                     static_cast<uint64_t>(seed), step.data_ptr<int32_t>(), seeds.data_ptr<int64_t>(),
                     n_pairs.data_ptr<int32_t>(), cur_stream());
@@ -1592,28 +1663,22 @@ static void link_seeds(GraphHandle* graph, const Tensor& pos, int64_t num_nodes,
 static void link_bce(const Tensor& Z, int64_t C, const Tensor& seed_local, int64_t P, int64_t B, const Tensor& n_pairs,
                      Tensor loss, const c10::optional<Tensor>& correct, const c10::optional<Tensor>& dZ) {
   c10::cuda::CUDAGuard guard(Z.device());
-  TORCH_CHECK(Z.is_cuda() && Z.scalar_type() == torch::kBFloat16 && Z.is_contiguous() && Z.dim() == 2,
+  TORCH_CHECK(Z.scalar_type() == torch::kBFloat16 && Z.is_contiguous() && Z.dim() == 2,
               "link_bce: Z must be a contiguous bf16 [rows, ld] CUDA tensor");
   TORCH_CHECK(C % 8 == 0 && C >= 8 && C <= 512 && C <= Z.size(1) && Z.size(1) % 8 == 0,
               "link_bce: C must be a multiple of 8 in [8, 512] and <= Z's width");
-  TORCH_CHECK(0 <= B && B <= P && seed_local.is_cuda() && seed_local.scalar_type() == torch::kInt32 &&
-              seed_local.numel() >= 2 * P, "link_bce: seed_local must be int32 [>= 2P]");
-  TORCH_CHECK(n_pairs.is_cuda() && n_pairs.scalar_type() == torch::kInt32 && n_pairs.numel() >= 1);
-  TORCH_CHECK(loss.is_cuda() && loss.scalar_type() == torch::kFloat32 && loss.numel() >= 1);
-  int32_t* corr = nullptr;
-  if (correct.has_value() && correct->defined()) {
-    TORCH_CHECK(correct->is_cuda() && correct->scalar_type() == torch::kInt32 && correct->numel() >= 1);
-    corr = correct->data_ptr<int32_t>();
-  }
-  float* dz = nullptr;
-  if (dZ.has_value() && dZ->defined()) {
-    TORCH_CHECK(dZ->is_cuda() && dZ->scalar_type() == torch::kFloat32 && dZ->is_contiguous() &&
-                dZ->sizes() == Z.sizes(), "link_bce: dZ must be a contiguous fp32 tensor of Z's shape");
-    dz = dZ->data_ptr<float>();
-  }
+  TORCH_CHECK(0 <= B && B <= P && on_dev(seed_local) && seed_local.scalar_type() == torch::kInt32 &&
+              seed_local.is_contiguous() && seed_local.numel() >= 2 * P, "link_bce: seed_local must be int32 [>= 2P]");
+  check_counters(n_pairs, 0, "link_bce: n_pairs must be int32 [>= 1] on the device");
+  TORCH_CHECK(on_dev(loss) && loss.scalar_type() == torch::kFloat32 && loss.numel() >= 1,
+              "link_bce: loss must be fp32 [>= 1] on the device");
+  if (has(correct)) check_counters(*correct, 0, "link_bce: correct must be int32 [>= 1] on the device");
+  if (has(dZ))
+    TORCH_CHECK(on_dev(*dZ) && dZ->scalar_type() == torch::kFloat32 && dZ->is_contiguous() && dZ->sizes() == Z.sizes(),
+                "link_bce: dZ must be a contiguous fp32 tensor of Z's shape");
   launch_link_bce(Z.data_ptr(), static_cast<int>(Z.size(1)), static_cast<int>(C), seed_local.data_ptr<int32_t>(),
-                  static_cast<int>(P), static_cast<int>(B), n_pairs.data_ptr<int32_t>(), loss.data_ptr<float>(), corr,
-                  dz, cur_stream());
+                  static_cast<int>(P), static_cast<int>(B), n_pairs.data_ptr<int32_t>(), loss.data_ptr<float>(),
+                  opt_ptr<int32_t>(correct), opt_ptr<float>(dZ), cur_stream());
   check_cuda_err("link_bce");
 }
 
@@ -1623,13 +1688,11 @@ static void dropout_bf16(Tensor Z, const Tensor& counters, int64_t n_hops, doubl
   TORCH_CHECK(Z.scalar_type() == torch::kBFloat16 && Z.is_contiguous() && Z.dim() == 2 && Z.size(1) % 8 == 0,
               "dropout_bf16: contiguous bf16 [rows, d], d % 8 == 0");
   TORCH_CHECK(p >= 0.0 && p < 1.0, "dropout_bf16: p in [0, 1)");
-  const int32_t* st = nullptr;
-  if (step_dev.has_value() && step_dev->defined()) {
-    TORCH_CHECK(step_dev->scalar_type() == torch::kInt32 && step_dev->is_cuda());
-    st = step_dev->data_ptr<int32_t>();
-  }
+  check_counters(counters, n_hops, "dropout_bf16: counters must be int32 [> n_hops] on the device");
+  if (has(step_dev)) check_counters(*step_dev, 0, "dropout_bf16: step_dev must be int32 [>= 1] on the device");
   launch_dropout_bf16(Z.data_ptr(), counters.data_ptr<int32_t>(), n_hops, Z.size(0), Z.size(1),
-                      static_cast<float>(p), static_cast<uint64_t>(seed), static_cast<int>(layer), st, cur_stream());
+                      static_cast<float>(p), static_cast<uint64_t>(seed), static_cast<int>(layer),
+                      opt_ptr<int32_t>(step_dev), cur_stream());
   check_cuda_err("dropout_bf16");
 }
 
@@ -1639,49 +1702,65 @@ static int64_t softmax_nll(const Tensor& logits, int64_t C, const c10::optional<
                         const Tensor& counters, Tensor loss, Tensor dlogits,
                         const c10::optional<Tensor>& correct, const c10::optional<Tensor>& colsum, bool prezeroed) {
   c10::cuda::CUDAGuard guard(logits.device());
-  TORCH_CHECK(logits.scalar_type() == torch::kBFloat16 && logits.is_contiguous());
-  TORCH_CHECK(dlogits.sizes() == logits.sizes() && dlogits.is_contiguous());
-  const bool direct = y.has_value() && y->defined();
-  TORCH_CHECK(direct || (labels_all.has_value() && nodes.has_value()), "need y or (labels_all, nodes)");
   TORCH_CHECK(logits.dim() == 2 && logits.size(1) % 8 == 0 && 1 <= C && C <= logits.size(1),
               "softmax_nll: logits must be [rows, ld] with ld a multiple of 8 and 1 <= C <= ld");
-  const bool has_colsum = colsum.has_value() && colsum->defined();
-  TORCH_CHECK(!has_colsum || (colsum->scalar_type() == torch::kFloat32 && colsum->is_contiguous() &&
-                              colsum->numel() == logits.size(1)), "softmax_nll: colsum must be fp32 [ld]");
+  check_rows(logits, torch::kBFloat16, logits.size(1), "softmax_nll: logits must be contiguous bf16 [rows, ld]");
+  check_rows(dlogits, torch::kBFloat16, logits.size(1), "softmax_nll: dlogits must be contiguous bf16 of logits' shape");
+  TORCH_CHECK(dlogits.size(0) == logits.size(0), "softmax_nll: dlogits must be contiguous bf16 of logits' shape");
+  const bool direct = has(y);
+  TORCH_CHECK(direct || (has(labels_all) && has(nodes)), "need y or (labels_all, nodes)");
+  if (direct) {
+    check_ids(*y, "softmax_nll: y must be contiguous int64 on the device");
+  } else {
+    check_ids(*labels_all, "softmax_nll: labels_all must be contiguous int64 on the device");
+    check_ids(*nodes, "softmax_nll: nodes must be contiguous int64 on the device");
+  }
+  check_counters(counters, 1, "softmax_nll: counters must be int32 [> 1] on the device");
+  TORCH_CHECK(on_dev(loss) && loss.scalar_type() == torch::kFloat32 && loss.numel() >= 1,
+              "softmax_nll: loss must be fp32 [>= 1] on the device");
+  if (has(correct)) check_counters(*correct, 0, "softmax_nll: correct must be int32 [>= 1] on the device");
+  if (has(colsum)) check_vec(*colsum, torch::kFloat32, logits.size(1), "softmax_nll: colsum must be fp32 [ld]");
   const int n = launch_softmax_nll(logits.data_ptr(), logits.size(1), C, direct ? y->data_ptr<int64_t>() : nullptr,
                                    direct ? nullptr : labels_all->data_ptr<int64_t>(),
                                    direct ? nullptr : nodes->data_ptr<int64_t>(),
                                    counters.data_ptr<int32_t>(), logits.size(0), loss.data_ptr<float>(),
-                                   dlogits.data_ptr(),
-                                   (correct.has_value() && correct->defined()) ? correct->data_ptr<int32_t>() : nullptr,
-                                   has_colsum ? colsum->data_ptr<float>() : nullptr, cur_stream(), prezeroed);
+                                   dlogits.data_ptr(), opt_ptr<int32_t>(correct), opt_ptr<float>(colsum), cur_stream(),
+                                   prezeroed);
   check_cuda_err("softmax_nll");
   return n;
 }
 
 static void zero_grads(Tensor g, const c10::optional<Tensor>& loss, const c10::optional<Tensor>& correct) {
   c10::cuda::CUDAGuard guard(g.device());
-  TORCH_CHECK(g.scalar_type() == torch::kFloat32 && g.is_contiguous() &&
-              reinterpret_cast<uintptr_t>(g.data_ptr()) % 16 == 0);
-  launch_zero_grads(g.data_ptr<float>(), g.numel(),
-                    (loss.has_value() && loss->defined()) ? loss->data_ptr<float>() : nullptr,
-                    (correct.has_value() && correct->defined()) ? correct->data_ptr<int32_t>() : nullptr, cur_stream());
+  TORCH_CHECK(g.scalar_type() == torch::kFloat32 && g.is_contiguous() && aligned16(g),
+              "zero_grads: g must be contiguous 16-byte aligned fp32");
+  if (has(loss))
+    TORCH_CHECK(on_dev(*loss) && loss->scalar_type() == torch::kFloat32 && loss->numel() >= 1,
+                "zero_grads: loss must be fp32 [>= 1] on the device");
+  if (has(correct)) check_counters(*correct, 0, "zero_grads: correct must be int32 [>= 1] on the device");
+  launch_zero_grads(g.data_ptr<float>(), g.numel(), opt_ptr<float>(loss), opt_ptr<int32_t>(correct), cur_stream());
   check_cuda_err("zero_grads");
 }
 
 static void colsum_bf16(const Tensor& X, const Tensor& counters, int64_t n_hops, Tensor out) {
   c10::cuda::CUDAGuard guard(X.device());
-  TORCH_CHECK(X.scalar_type() == torch::kBFloat16 && X.is_contiguous() && X.size(1) % 8 == 0);
-  TORCH_CHECK(out.scalar_type() == torch::kFloat32 && out.numel() == X.size(1) && X.size(1) <= 2048);
-  launch_colsum_bf16(X.data_ptr(), counters.data_ptr<int32_t>(), n_hops, X.size(0), X.size(1),
-                     out.data_ptr<float>(), cur_stream());
+  const int64_t d = X.dim() == 2 ? X.size(1) : 0;
+  TORCH_CHECK(d % 8 == 0 && d <= 2048, "colsum_bf16: width must be a multiple of 8 up to 2048");
+  check_rows(X, torch::kBFloat16, d, "colsum_bf16: X must be contiguous bf16 [rows, d]");
+  check_vec(out, torch::kFloat32, d, "colsum_bf16: out must be fp32 [d]");
+  check_counters(counters, n_hops, "colsum_bf16: counters must be int32 [> n_hops] on the device");
+  launch_colsum_bf16(X.data_ptr(), counters.data_ptr<int32_t>(), n_hops, X.size(0), d, out.data_ptr<float>(),
+                     cur_stream());
   check_cuda_err("colsum_bf16");
 }
 
 static void zero_rows(Tensor p, const Tensor& counters, int64_t n_hops) {
   c10::cuda::CUDAGuard guard(p.device());
-  TORCH_CHECK(p.scalar_type() == torch::kFloat32 && p.is_contiguous() && p.size(1) % 4 == 0);
-  launch_zero_rows(p.data_ptr<float>(), counters.data_ptr<int32_t>(), n_hops, p.size(0), p.size(1), cur_stream());
+  const int64_t d = p.dim() == 2 ? p.size(1) : 0;
+  TORCH_CHECK(d % 4 == 0, "zero_rows: width must be a multiple of 4");
+  check_rows(p, torch::kFloat32, d, "zero_rows: p must be contiguous fp32 [rows, d]");
+  check_counters(counters, n_hops, "zero_rows: counters must be int32 [> n_hops] on the device");
+  launch_zero_rows(p.data_ptr<float>(), counters.data_ptr<int32_t>(), n_hops, p.size(0), d, cur_stream());
   check_cuda_err("zero_rows");
 }
 
@@ -1689,15 +1768,16 @@ static void adam_step(Tensor p, const Tensor& g, Tensor m, Tensor v, const c10::
                       double lr, double b1, double b2, double eps, double wd, const Tensor& step_dev,
                       double gscale) {
   c10::cuda::CUDAGuard guard(p.device());
-  TORCH_CHECK(step_dev.scalar_type() == torch::kInt32 && step_dev.numel() >= 2,
-              "step_dev must be int32[2]: {steps taken, block ticket}");
-  TORCH_CHECK(p.scalar_type() == torch::kFloat32 && g.scalar_type() == torch::kFloat32 &&
-              m.scalar_type() == torch::kFloat32 && v.scalar_type() == torch::kFloat32, "adam: fp32 state");
+  check_counters(step_dev, 1, "step_dev must be int32[2]: {steps taken, block ticket}");
+  for (const Tensor* t : std::initializer_list<const Tensor*>{&p, &g, &m, &v})
+    TORCH_CHECK(on_dev(*t) && t->scalar_type() == torch::kFloat32, "adam: fp32 state");
   TORCH_CHECK(g.numel() >= p.numel() && m.numel() >= p.numel() && v.numel() >= p.numel() && p.is_contiguous() &&
               g.is_contiguous() && m.is_contiguous() && v.is_contiguous(), "adam: state size / layout mismatch");
-  launch_adam(p.data_ptr<float>(), g.data_ptr<float>(), m.data_ptr<float>(), v.data_ptr<float>(),
-              (p_bf16.has_value() && p_bf16->defined()) ? p_bf16->data_ptr() : nullptr, p.numel(), lr,
-              b1, b2, eps, wd, step_dev.data_ptr<int32_t>(), gscale, cur_stream());
+  if (has(p_bf16))
+    TORCH_CHECK(on_dev(*p_bf16) && p_bf16->scalar_type() == torch::kBFloat16 && p_bf16->is_contiguous() &&
+                p_bf16->numel() >= p.numel(), "adam: p_bf16 must be a contiguous bf16 shadow of p on the device");
+  launch_adam(p.data_ptr<float>(), g.data_ptr<float>(), m.data_ptr<float>(), v.data_ptr<float>(), opt_ptr(p_bf16),
+              p.numel(), lr, b1, b2, eps, wd, step_dev.data_ptr<int32_t>(), gscale, cur_stream());
   check_cuda_err("adam");
 }
 
@@ -1707,16 +1787,18 @@ static void sage_fused(RowTableHandle* feat, const c10::optional<Tensor>& nodes,
                        const std::vector<int64_t>& ks, const Tensor& deg, const Tensor& w_packed,
                        const Tensor& bias, bool relu, Tensor z, const c10::optional<Tensor>& a_save) {
   c10::cuda::CUDAGuard guard(z.device());
-  const bool local = src_local.has_value() && src_local->defined();
+  const bool local = has(src_local);
   const bool fp8 = feat != nullptr && !local && feat->dtype == torch::kUInt8;
   TORCH_CHECK(!fp8 || d == 128, "the MXFP8 loader of the fused kernel supports d = 128");
-  TORCH_CHECK(z.scalar_type() == torch::kBFloat16 && z.is_contiguous());
-  const int64_t n_out = z.size(1);
-  TORCH_CHECK(sage_fused_supported(d, n_out), "unsupported fused shape d=", d, " n_out=", n_out);
+  const int64_t n_out = z.dim() == 2 ? z.size(1) : 0;
+  check_rows(z, torch::kBFloat16, n_out, "sage_fused: z must be contiguous bf16 [rows, n_out]");
+  TORCH_CHECK(sage_fused_supported(d, n_out),
+              fmt("unsupported fused shape d=%lld n_out=%lld", static_cast<long long>(d), static_cast<long long>(n_out)));
   TORCH_CHECK(local || feat == nullptr || sage_fused_supported(d, n_out, &feat->tbl),
               "sage_fused: the fused kernel's 32-bit row handles cannot address this feature table "
               "(more than 16 parts, or a part of 2^28 rows or more)");
-  TORCH_CHECK(w_packed.numel() == 2 * d * n_out && w_packed.scalar_type() == torch::kBFloat16);
+  check_vec(w_packed, torch::kBFloat16, 2 * d * n_out, "sage_fused: w_packed must be packed bf16 [n_out * 2d]");
+  check_vec(bias, torch::kBFloat16, n_out, "sage_fused: bias must be bf16 [n_out]");
   SageFusedArgs f{};
   f.agg = make_agg(feat, nodes, src_local, d, counters, n_hops_targets, z.size(0), ell, ks, deg, nullptr);
   f.w_packed = w_packed.data_ptr();
@@ -1726,14 +1808,14 @@ static void sage_fused(RowTableHandle* feat, const c10::optional<Tensor>& nodes,
   f.z = z.data_ptr();
   f.feat_fp8 = fp8 ? 1 : 0;
   f.a_save = nullptr;
-  if (a_save.has_value() && a_save->defined()) {
-    TORCH_CHECK(a_save->size(0) >= z.size(0) && a_save->size(1) == 2 * d && a_save->is_contiguous());
+  if (has(a_save)) {
+    check_rows(*a_save, torch::kBFloat16, 2 * d, "sage_fused: a_save must be contiguous bf16 [>= rows of z, 2d]");
+    TORCH_CHECK(a_save->size(0) >= z.size(0), "sage_fused: a_save must be contiguous bf16 [>= rows of z, 2d]");
     f.a_save = a_save->data_ptr();
   }
   launch_sage_fused(f, at::cuda::getCurrentDeviceProperties()->multiProcessorCount, cur_stream());
   check_cuda_err("sage_fused");
 }
-
 
 // ---------------------------------------------------------------------------
 // TcGemm: a cached launch of the TMA-fed wgmma GEMM kernel (csrc/cuda/tc_gemm.cu) over fixed engine buffers.
@@ -1754,13 +1836,13 @@ struct TcGemm {
   }
   static int pick_bn(int64_t n) { return n % 256 == 0 ? 256 : (n % 128 == 0 ? 128 : 64); }
   void check_bf16(const Tensor& t, const char* what) {
-    TORCH_CHECK(t.is_cuda() && t.scalar_type() == torch::kBFloat16 && t.dim() == 2 && t.stride(1) == 1 &&
-                (t.stride(0) * 2) % 16 == 0 && reinterpret_cast<uintptr_t>(t.data_ptr()) % 16 == 0,
-                "TcGemm: ", what, " must be a 2-D bf16 CUDA tensor with unit inner stride and 16-byte aligned rows");
+    TORCH_CHECK(on_dev(t) && t.scalar_type() == torch::kBFloat16 && t.dim() == 2 && t.stride(1) == 1 &&
+                (t.stride(0) * 2) % 16 == 0 && aligned16(t),
+                fmt("TcGemm: %s must be a 2-D bf16 CUDA tensor with unit inner stride and 16-byte aligned rows", what));
   }
   void tmap(int slot, const Tensor& t, int box_cols, int box_rows) {
     const int rc = make_tmap_bf16_2d(L.maps[slot], t.data_ptr(), t.size(0), t.size(1), t.stride(0), box_cols, box_rows);
-    TORCH_CHECK(rc == 0, "TcGemm: cuTensorMapEncodeTiled failed (rc=", rc, ")");
+    TORCH_CHECK(rc == 0, fmt("TcGemm: cuTensorMapEncodeTiled failed (rc=%d)", rc));
     keep.push_back(t);
   }
   TcProblem& next() {
@@ -1768,7 +1850,7 @@ struct TcGemm {
     return L.args.p[L.args.n_prob];
   }
   void set_dyn(TcProblem& p, const Tensor& counters, int64_t idx, int64_t cap, bool is_k) {
-    TORCH_CHECK(counters.is_cuda() && counters.scalar_type() == torch::kInt32 && idx >= 0 && idx < counters.numel());
+    check_counters(counters, idx, "TcGemm: counters must be int32 [> dyn_idx] on the device");
     p.dyn = counters.data_ptr<int32_t>();
     p.dyn_idx = static_cast<int>(idx);
     p.dyn_cap = static_cast<int>(cap);
@@ -1781,16 +1863,16 @@ struct TcGemm {
     c10::cuda::CUDAGuard guard(A.device());
     check_bf16(A, "A"); check_bf16(W, "W"); check_bf16(Z, "Z");
     const int64_t K = A.size(1), N = W.size(0);
-    TORCH_CHECK(W.size(1) == K && Z.size(1) == N && Z.size(0) >= A.size(0) && N % 64 == 0 && K % 8 == 0);
+    TORCH_CHECK(W.size(1) == K && Z.size(1) == N && Z.size(0) >= A.size(0) && N % 64 == 0 && K % 8 == 0,
+                "TcGemm.add_forward: A [rows, K], W [N, K], Z [>= rows, N] with N a multiple of 64 and K of 8");
     const int slot = 3 * L.args.n_prob;
     TcProblem& p = next();
     p.a_mn = 0; p.b_mn = 0; p.epi = 0; p.bn = pick_bn(N);
     p.m = A.size(0); p.n = N; p.k = K;
     set_dyn(p, counters, dyn_idx, A.size(0), false);
     p.bias = nullptr;
-    if (bias.has_value() && bias->defined()) {
-      TORCH_CHECK(bias->scalar_type() == torch::kBFloat16 && bias->numel() == N &&
-                  reinterpret_cast<uintptr_t>(bias->data_ptr()) % 16 == 0);
+    if (has(bias)) {
+      check_vec(*bias, torch::kBFloat16, N, "TcGemm.add_forward: bias must be 16-byte aligned bf16 [N]");
       p.bias = bias->data_ptr();
       keep.push_back(*bias);
     }
@@ -1806,7 +1888,8 @@ struct TcGemm {
     c10::cuda::CUDAGuard guard(dPre.device());
     check_bf16(dPre, "dPre"); check_bf16(W, "W"); check_bf16(dA, "dA");
     const int64_t Kd = dPre.size(1), N = W.size(1);
-    TORCH_CHECK(W.size(0) == Kd && dA.size(1) == N && dA.size(0) >= dPre.size(0) && N % 64 == 0 && Kd % 8 == 0);
+    TORCH_CHECK(W.size(0) == Kd && dA.size(1) == N && dA.size(0) >= dPre.size(0) && N % 64 == 0 && Kd % 8 == 0,
+                "TcGemm.add_dgrad: dPre [rows, Kd], W [Kd, N], dA [>= rows, N] with N a multiple of 64 and Kd of 8");
     const int slot = 3 * L.args.n_prob;
     TcProblem& p = next();
     p.a_mn = 0; p.b_mn = 1; p.epi = 0; p.bn = pick_bn(N);
@@ -1825,8 +1908,9 @@ struct TcGemm {
     c10::cuda::CUDAGuard guard(dPre.device());
     check_bf16(dPre, "dPre"); check_bf16(A, "A");
     const int64_t M = dPre.size(1), N = A.size(1);
-    TORCH_CHECK(A.size(0) >= dPre.size(0) && N % 64 == 0 && M % 8 == 0);
-    TORCH_CHECK(gW.is_cuda() && gW.scalar_type() == torch::kFloat32 && gW.dim() == 2 && gW.size(0) == M &&
+    TORCH_CHECK(A.size(0) >= dPre.size(0) && N % 64 == 0 && M % 8 == 0,
+                "TcGemm.add_wgrad: dPre [rows, M], A [>= rows, N] with N a multiple of 64 and M of 8");
+    TORCH_CHECK(on_dev(gW) && gW.scalar_type() == torch::kFloat32 && gW.dim() == 2 && gW.size(0) == M &&
                 gW.size(1) == N && gW.stride(1) == 1 && gW.stride(0) % 4 == 0 &&
                 reinterpret_cast<uintptr_t>(gW.data_ptr()) % 16 == 0, "TcGemm: gW must be fp32 [M, N], 16-byte aligned");
     const int slot = 3 * L.args.n_prob;
@@ -1856,10 +1940,10 @@ static void enable_peer_access(int dev, int peer) {
   c10::cuda::CUDAGuard guard(dev);
   int can = 0;
   cudaDeviceCanAccessPeer(&can, dev, peer);
-  TORCH_CHECK(can, "GPU ", dev, " cannot access peer GPU ", peer);
+  TORCH_CHECK(can, fmt("GPU %d cannot access peer GPU %d", dev, peer));
   cudaError_t e = cudaDeviceEnablePeerAccess(peer, 0);
   if (e == cudaErrorPeerAccessAlreadyEnabled) { cudaGetLastError(); return; }
-  TORCH_CHECK(e == cudaSuccess, "cudaDeviceEnablePeerAccess: ", cudaGetErrorString(e));
+  TORCH_CHECK(e == cudaSuccess, fmt("cudaDeviceEnablePeerAccess: %s", cudaGetErrorString(e)));
 }
 
 // ---------------------------------------------------------------------------
@@ -1889,7 +1973,7 @@ struct PeerBuffer : public std::enable_shared_from_this<PeerBuffer> {
     b->device = device;
     b->bytes = std::max<int64_t>(nbytes, 256);
     cudaError_t e = cudaMalloc(&b->ptr, b->bytes);
-    TORCH_CHECK(e == cudaSuccess, "cudaMalloc(", b->bytes, ") failed: ", cudaGetErrorString(e));
+    TORCH_CHECK(e == cudaSuccess, fmt("cudaMalloc(%zu) failed: %s", b->bytes, cudaGetErrorString(e)));
     return b;
   }
 
@@ -1898,7 +1982,7 @@ struct PeerBuffer : public std::enable_shared_from_this<PeerBuffer> {
     c10::cuda::CUDAGuard guard(device);
     cudaIpcMemHandle_t h;
     cudaError_t e = cudaIpcGetMemHandle(&h, ptr);
-    TORCH_CHECK(e == cudaSuccess, "cudaIpcGetMemHandle failed: ", cudaGetErrorString(e));
+    TORCH_CHECK(e == cudaSuccess, fmt("cudaIpcGetMemHandle failed: %s", cudaGetErrorString(e)));
     return py::bytes(reinterpret_cast<const char*>(&h), sizeof(h));
   }
 
@@ -1912,7 +1996,7 @@ struct PeerBuffer : public std::enable_shared_from_this<PeerBuffer> {
     b->bytes = nbytes;
     b->imported = true;
     cudaError_t e = cudaIpcOpenMemHandle(&b->ptr, h, cudaIpcMemLazyEnablePeerAccess);
-    TORCH_CHECK(e == cudaSuccess, "cudaIpcOpenMemHandle failed: ", cudaGetErrorString(e));
+    TORCH_CHECK(e == cudaSuccess, fmt("cudaIpcOpenMemHandle failed: %s", cudaGetErrorString(e)));
     return b;
   }
 
@@ -1936,12 +2020,15 @@ struct PeerGroup {
 
   PeerGroup(int dev, int rank, std::vector<Tensor> grads, std::vector<Tensor> flags) : device(dev) {
     c10::cuda::CUDAGuard guard(dev);
-    TORCH_CHECK(grads.size() == flags.size() && grads.size() <= kMaxParts);
+    TORCH_CHECK(grads.size() == flags.size() && grads.size() <= kMaxParts,
+                "PeerGroup: one gradient buffer and one flag array per rank, at most 16 ranks");
     p.world = grads.size();
     p.rank = rank;
     for (size_t r = 0; r < grads.size(); ++r) {
-      TORCH_CHECK(grads[r].scalar_type() == torch::kFloat32 && flags[r].scalar_type() == torch::kInt32);
-      TORCH_CHECK(flags[r].numel() >= 2 * p.world);
+      TORCH_CHECK(grads[r].is_cuda() && grads[r].scalar_type() == torch::kFloat32 && grads[r].is_contiguous(),
+                  "PeerGroup: gradient buffers must be contiguous fp32 CUDA tensors");
+      TORCH_CHECK(flags[r].is_cuda() && flags[r].scalar_type() == torch::kInt32 && flags[r].is_contiguous() &&
+                  flags[r].numel() >= 2 * p.world, "PeerGroup: flags must be contiguous int32 [2 * world] CUDA tensors");
       p.g[r] = grads[r].data_ptr<float>();
       p.flags[r] = flags[r].data_ptr<int32_t>();
       keep.push_back(grads[r]);
@@ -1962,27 +2049,34 @@ struct PeerGroup {
             double eps, double wd, const Tensor& step_dev, double gscale) {
     c10::cuda::CUDAGuard guard(device);
     TORCH_CHECK(param.numel() % 4 == 0, "flat parameter buffer must be padded to a multiple of 4");
-    TORCH_CHECK(step_dev.scalar_type() == torch::kInt32 && step_dev.numel() >= 2,
-                "step_dev must be int32[2]: {steps taken, block ticket}");
-    launch_adam_peer(p, param.data_ptr<float>(), m.data_ptr<float>(), v.data_ptr<float>(),
-                     (p_bf16.has_value() && p_bf16->defined()) ? p_bf16->data_ptr() : nullptr, param.numel(), lr,
-                     b1, b2, eps, wd, step_dev.data_ptr<int32_t>(), gscale, cur_stream(), err.data_ptr<int32_t>());
+    check_counters(step_dev, 1, "step_dev must be int32[2]: {steps taken, block ticket}");
+    for (const Tensor* t : {&param, &m, &v})
+      TORCH_CHECK(on_dev(*t) && t->scalar_type() == torch::kFloat32 && t->is_contiguous() && t->numel() == param.numel(),
+                  "PeerGroup.adam: param, m and v must be contiguous fp32 of one size on the group's device");
+    if (has(p_bf16))
+      TORCH_CHECK(on_dev(*p_bf16) && p_bf16->scalar_type() == torch::kBFloat16 && p_bf16->is_contiguous() &&
+                  p_bf16->numel() >= param.numel(), "PeerGroup.adam: p_bf16 must be a contiguous bf16 shadow of param");
+    launch_adam_peer(p, param.data_ptr<float>(), m.data_ptr<float>(), v.data_ptr<float>(), opt_ptr(p_bf16),
+                     param.numel(), lr, b1, b2, eps, wd, step_dev.data_ptr<int32_t>(), gscale, cur_stream(),
+                     err.data_ptr<int32_t>());
     check_cuda_err("adam_peer");
   }
 };
 
 static void multimem_copy(const Tensor& src, int64_t mc_ptr, int64_t dst_byte_offset) {
   c10::cuda::CUDAGuard guard(src.device());
-  TORCH_CHECK(src.is_cuda() && src.is_contiguous());
+  TORCH_CHECK(src.is_contiguous() && aligned16(src), "multimem_copy: src must be contiguous and 16-byte aligned");
   const int64_t nbytes = src.numel() * src.element_size();
-  TORCH_CHECK(nbytes % 16 == 0 && dst_byte_offset % 16 == 0 && mc_ptr != 0);
+  TORCH_CHECK(nbytes % 16 == 0 && dst_byte_offset % 16 == 0 && mc_ptr != 0,
+              "multimem_copy: size and destination offset must be multiples of 16 bytes, mc_ptr non-null");
   launch_multimem_copy(src.data_ptr(), reinterpret_cast<void*>(mc_ptr + dst_byte_offset), nbytes, cur_stream());
   check_cuda_err("multimem_copy");
 }
 
 static Tensor pack_weight(const Tensor& w) {
   c10::cuda::CUDAGuard guard(w.device());
-  TORCH_CHECK(w.scalar_type() == torch::kBFloat16 && w.is_contiguous() && w.dim() == 2);
+  TORCH_CHECK(w.scalar_type() == torch::kBFloat16 && w.is_contiguous() && w.dim() == 2,
+              "pack_weight: w must be contiguous bf16 [N, K]");
   TORCH_CHECK(w.size(1) % 64 == 0 && w.size(0) % 16 == 0, "W must be [N%16, K%64]");
   Tensor out = torch::empty_like(w);
   launch_pack_weight(w.data_ptr(), w.size(0), w.size(1), out.data_ptr(), cur_stream());
@@ -1992,8 +2086,9 @@ static Tensor pack_weight(const Tensor& w) {
 
 static void pack_weight_into(const Tensor& w, Tensor out) {
   c10::cuda::CUDAGuard guard(w.device());
-  TORCH_CHECK(w.scalar_type() == torch::kBFloat16 && w.is_contiguous() && w.dim() == 2);
-  TORCH_CHECK(out.numel() == w.numel() && out.scalar_type() == torch::kBFloat16);
+  TORCH_CHECK(w.scalar_type() == torch::kBFloat16 && w.is_contiguous() && w.dim() == 2,
+              "pack_weight_into: w must be contiguous bf16 [N, K]");
+  check_vec(out, torch::kBFloat16, w.numel(), "pack_weight_into: out must be contiguous bf16 of w's size");
   launch_pack_weight(w.data_ptr(), w.size(0), w.size(1), out.data_ptr(), cur_stream());
   check_cuda_err("pack_weight");
 }

@@ -24,10 +24,11 @@ namespace glt {
 
 using torch::Tensor;
 
+// One message argument per TORCH_CHECK (see fmt in bindings.cc): the message is built first.
 static inline void check_i64(const Tensor& t, const char* name) {
-  TORCH_CHECK(t.device().is_cpu(), name, " must be a CPU tensor");
-  TORCH_CHECK(t.scalar_type() == torch::kInt64, name, " must be int64");
-  TORCH_CHECK(t.is_contiguous(), name, " must be contiguous");
+  TORCH_CHECK(t.device().is_cpu(), std::string(name) + " must be a CPU tensor");
+  TORCH_CHECK(t.scalar_type() == torch::kInt64, std::string(name) + " must be int64");
+  TORCH_CHECK(t.is_contiguous(), std::string(name) + " must be contiguous");
 }
 
 // ----------------------------------------------------------------------------
