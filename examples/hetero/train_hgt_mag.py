@@ -10,6 +10,13 @@ dependency-free `models.HGT`, the graph is synthetic with the MAG schema (no net
 sm_90a kernels, loss, backward and Adam) as one CUDA graph on one GPU, with the reference's hyper-parameters.  The
 engine's model has a per-type input `Linear` + ReLU in front of its HGT layers, as the reference's model does; the
 loader mode trains `models.HGT`, which has no input Linear, so the two modes do not train the same architecture.
+
+`--featureless metapath2vec` (needs a GPU) gives every node type except paper the embeddings `models.MetaPath2VecEngine`
+trains over the metapath author -> paper -> field_of_study -> paper -> author -> institution -> author, with PyG's
+MetaPath2Vec hyper-parameters (the reference's `OGB_MAG(preprocess='metapath2vec')` vectors come from that recipe).
+It runs for --m2v-steps steps of 128 start authors (default: one pass over the authors).  On synthetic data it
+replaces the random features of those types; the default, `--featureless mean`, keeps the neighbour means of
+`load_mag_from_disk`.
 """
 import argparse
 import os
@@ -24,11 +31,48 @@ from common import glt, synthetic_mag  # noqa: E402
 from graphlearn_for_pytorch_b200.models import HGT  # noqa: E402
 
 
+MAG_METAPATH = [('author', 'writes', 'paper'), ('paper', 'has_topic', 'field_of_study'),
+                ('field_of_study', 'rev_has_topic', 'paper'), ('paper', 'rev_writes', 'author'),
+                ('author', 'affiliated_with', 'institution'), ('institution', 'rev_affiliated_with', 'author')]
+M2V_ARGS = dict(embedding_dim=128, walk_length=64, context_size=7, walks_per_node=5, num_negative_samples=5,
+                batch_size=128, lr=0.01)
+
+
+def metapath2vec_features(edges, sizes, feats, steps=0, seed=0):
+  """feats with every type except paper replaced by metapath2vec embeddings of the paper features' width, trained by
+  MetaPath2VecEngine on cuda:0 for `steps` steps (0: one pass over the authors)."""
+  from graphlearn_for_pytorch_b200.models import MetaPath2VecEngine
+  dev = torch.device('cuda', 0)
+  graphs = {e: glt.data.Graph(glt.data.Topology(edges[e], layout='CSR', num_nodes=max(sizes[e[0]], sizes[e[2]])),
+                              'CUDA', 0) for e in MAG_METAPATH}
+  hp = dict(M2V_ARGS, embedding_dim=feats['paper'].shape[1])
+  eng = MetaPath2VecEngine(graphs, sizes, MAG_METAPATH, seed=seed, device=dev, **hp)
+  eng.warmup_and_capture()
+  B = hp['batch_size']
+  steps = steps or -(-sizes['author'] // B)
+  t0, done, losses = time.time(), 0, []
+  while done < steps:
+    perm = torch.randperm(sizes['author'], device=dev)
+    for i in range(0, perm.numel(), B):
+      losses.append(eng.train_step(perm[i:i + B]).clone())
+      done += 1
+      if done == steps:
+        break
+  print(f'metapath2vec: {steps} steps, loss {float(losses[0]):.4f} -> {float(torch.stack(losses[-10:]).mean()):.4f}, '
+        f'{time.time() - t0:.1f}s')
+  out = dict(feats)
+  for t in eng.node_types:
+    if t != 'paper':
+      out[t] = eng.embedding(t).cpu()
+  return out
+
+
 def load_mag_from_disk(root, name='ogbn-mag'):
   """ogbn-mag from its OGB directory: reverse relations are added (what T.ToUndirected(merge=True) does in the
   reference script) and node types that ship without features get the mean of their featured neighbours' rows,
   propagated until every type has some (author <- papers written, institution <- authors, field <- papers); the
-  reference substitutes pre-trained metapath2vec vectors there (examples/hetero/train_hgt_mag.py:33-36)."""
+  reference substitutes pre-trained metapath2vec vectors there (examples/hetero/train_hgt_mag.py:33-36), which
+  `--featureless metapath2vec` trains with MetaPath2VecEngine."""
   d = glt.utils.load_ogb_hetero_dataset(root, name)
   edges = dict(d['edge_index'])
   for (s, r, t), ei in list(edges.items()):
@@ -52,12 +96,20 @@ def load_mag_from_disk(root, name='ogbn-mag'):
   return edges, feats, labels, sizes, d['split']
 
 
-def build_dataset(args, cuda, device_index=0):
+def load_data(args):
+  """(edges, feats, labels, sizes, split or None) from --root or synthetic, with the --featureless choice applied."""
   split = None
   if getattr(args, 'root', None):
     edges, feats, labels, sizes, split = load_mag_from_disk(args.root, args.dataset)
   else:
     edges, feats, labels, sizes = synthetic_mag(args.papers)
+  if getattr(args, 'featureless', 'mean') == 'metapath2vec':
+    feats = metapath2vec_features(edges, sizes, feats, args.m2v_steps)
+  return edges, feats, labels, sizes, split
+
+
+def build_dataset(args, cuda, device_index=0):
+  edges, feats, labels, sizes, split = load_data(args)
   ds = glt.data.Dataset()
   ds.init_graph(edges, graph_mode=('ZERO_COPY' if args.zero_copy else 'CUDA') if cuda else 'CPU', num_nodes=sizes,
                 device=device_index)
@@ -118,6 +170,11 @@ def parse():
   p.add_argument('--eval', choices=['sampled', 'full'], default='sampled',
                  help='--mode engine: validation accuracy from sampled batches (evaluate_batch), or validation and test '
                       'accuracy of exact layer-wise full-neighbourhood inference (HeteroHgtEngine.inference)')
+  p.add_argument('--featureless', choices=['mean', 'metapath2vec'], default='mean',
+                 help='features of the types other than paper: neighbour means (--root) or the synthetic ones, or '
+                      'metapath2vec embeddings trained by MetaPath2VecEngine (needs a GPU)')
+  p.add_argument('--m2v-steps', type=int, default=0,
+                 help='--featureless metapath2vec: training steps of 128 start authors (0: one pass over the authors)')
   return p.parse_args()
 
 
@@ -126,11 +183,7 @@ def run_engine(args):
   from graphlearn_for_pytorch_b200.models import HeteroHgtEngine
   dev = torch.device('cuda', 0)
   torch.cuda.set_device(dev)
-  if args.root:
-    edges, feats, labels, sizes, split = load_mag_from_disk(args.root, args.dataset)
-  else:
-    edges, feats, labels, sizes = synthetic_mag(args.papers)
-    split = None
+  edges, feats, labels, sizes, split = load_data(args)
   if split and 'train' in split and 'paper' in split['train']:
     train_idx, val_idx = split['train']['paper'], split.get('valid', split['train'])['paper']
     test_idx = split.get('test', split.get('valid', split['train']))['paper']
@@ -181,6 +234,9 @@ def run_engine(args):
 
 if __name__ == '__main__':
   args = parse()
+  if args.featureless == 'metapath2vec' and not torch.cuda.is_available():
+    sys.exit('--featureless metapath2vec trains MetaPath2VecEngine, which needs a CUDA GPU; use --featureless mean '
+             'without one')
   if args.mode == 'engine':
     if not torch.cuda.is_available():
       sys.exit('--mode engine trains HeteroHgtEngine, which needs a CUDA GPU; use the default --mode loader without one')

@@ -1682,6 +1682,162 @@ static void link_bce(const Tensor& Z, int64_t C, const Tensor& seed_local, int64
   check_cuda_err("link_bce");
 }
 
+// ---------------------------------------------------------------------------
+// MetaPath: device view of a metapath for the skip-gram kernels (cuda/skipgram.cu): the R relation graphs (CSR rows =
+// source ids) as a device array of GraphTables, and the node type of every walk position slot as (first row in the
+// concatenated embedding table, node count).  Slot 0 is the source type of relation 0, slot r + 1 the destination
+// type of relation r.
+// ---------------------------------------------------------------------------
+struct MetaPath {
+  int device, R;
+  std::vector<GraphHandle*> graphs;
+  MetaPathTypes types{};
+  int64_t rows = 0;       // rows the embedding tables must have: max over slots of off + n
+  Tensor tables;          // uint8 [R * sizeof(GraphTable)]
+
+  MetaPath(int dev, std::vector<GraphHandle*> graphs_, std::vector<int64_t> slot_off, std::vector<int64_t> slot_n)
+      : device(dev), R(static_cast<int>(graphs_.size())), graphs(std::move(graphs_)) {
+    c10::cuda::CUDAGuard guard(device);
+    TORCH_CHECK(R >= 1 && R <= kMaxMetaPath, fmt("MetaPath: 1 to %d relations", kMaxMetaPath));
+    TORCH_CHECK(static_cast<int>(slot_off.size()) == R + 1 && static_cast<int>(slot_n.size()) == R + 1,
+                "MetaPath: slot_off and slot_n need R + 1 entries");
+    std::vector<GraphTable> t(R);
+    for (int r = 0; r < R; ++r) {
+      TORCH_CHECK(graphs[r] != nullptr && graphs[r]->tbl.num_parts > 0, "MetaPath: every relation needs a device graph");
+      TORCH_CHECK(graphs[r]->device == device, "MetaPath: the relation graphs must live on the metapath's device");
+      t[r] = graphs[r]->tbl;
+    }
+    for (int s = 0; s <= R; ++s) {
+      TORCH_CHECK(slot_n[s] >= 1 && slot_n[s] < (1LL << 32) && slot_off[s] >= 0 && slot_off[s] + slot_n[s] < (1LL << 40),
+                  "MetaPath: every slot needs 1 <= n < 2^32 nodes at a non-negative row offset");
+      types.off[s] = slot_off[s];
+      types.n[s] = slot_n[s];
+      rows = std::max(rows, slot_off[s] + slot_n[s]);
+    }
+    tables = torch::empty({static_cast<int64_t>(R * sizeof(GraphTable))},
+                          torch::TensorOptions().dtype(torch::kUInt8).device(torch::kCUDA, device));
+    cudaMemcpy(tables.data_ptr(), t.data(), R * sizeof(GraphTable), cudaMemcpyHostToDevice);
+    check_cuda_err("MetaPath setup");
+  }
+  const GraphTable* dev_tables() const { return reinterpret_cast<const GraphTable*>(tables.data_ptr()); }
+};
+
+// walks int64 [n_walks, L + 1] with L >= 1 and 2 <= C <= L + 1; returns (n_walks, L)
+static std::pair<int64_t, int64_t> check_walks(const Tensor& walks, int64_t C, const char* msg) {
+  TORCH_CHECK(on_dev(walks) && walks.scalar_type() == torch::kInt64 && walks.dim() == 2 && walks.is_contiguous() &&
+              walks.size(1) >= 2 && walks.size(0) < (1LL << 31), msg);
+  const int64_t L = walks.size(1) - 1;
+  TORCH_CHECK(C >= 2 && C <= L + 1, fmt("context_size must be in [2, walk_length + 1 = %lld]", (long long)(L + 1)));
+  return {walks.size(0), L};
+}
+
+// negatives int64 [n_walks (L + 2 - C) K, C]
+static void check_negatives(const Tensor& neg, int64_t n_walks, int64_t L, int64_t C, int64_t K, const char* msg) {
+  TORCH_CHECK(K >= 1, "num_negative_samples must be >= 1");
+  const int64_t n = n_walks * (L + 2 - C) * K;
+  TORCH_CHECK(n < (1LL << 31), "too many negative windows (>= 2^31)");
+  TORCH_CHECK(on_dev(neg) && neg.scalar_type() == torch::kInt64 && neg.dim() == 2 && neg.is_contiguous() &&
+              neg.size(0) == n && neg.size(1) == C, msg);
+}
+
+// Walks of one step: walk i starts at starts[i / walks_per_node]; n_valid = #windows of C valid entries.
+static void metapath_walk(const MetaPath& mp, const Tensor& starts, int64_t walks_per_node, int64_t context_size,
+                          int64_t seed, const Tensor& step, Tensor walks, Tensor n_valid) {
+  c10::cuda::CUDAGuard guard(mp.device);
+  check_ids(starts, "metapath_walk: starts must be contiguous int64 on the metapath's device");
+  TORCH_CHECK(walks_per_node >= 1, "metapath_walk: walks_per_node must be >= 1");
+  const auto [n_walks, L] = check_walks(walks, context_size,
+                                        "metapath_walk: walks must be a contiguous int64 [n_walks, walk_length + 1] "
+                                        "tensor on the metapath's device");
+  TORCH_CHECK(n_walks == starts.numel() * walks_per_node, "metapath_walk: walks needs starts * walks_per_node rows");
+  check_counters(step, 0, "metapath_walk: step must be int32 [>= 1] on the device");
+  check_counters(n_valid, 0, "metapath_walk: n_valid must be int32 [>= 1] on the device");
+  if (n_walks == 0) return;
+  launch_metapath_walk(mp.dev_tables(), mp.R, mp.types, starts.data_ptr<int64_t>(), static_cast<int>(n_walks),
+                       static_cast<int>(walks_per_node), static_cast<int>(L), static_cast<int>(context_size),
+                       static_cast<uint64_t>(seed), step.data_ptr<int32_t>(), walks.data_ptr<int64_t>(),
+                       n_valid.data_ptr<int32_t>(), cur_stream());
+  check_cuda_err("metapath_walk");
+}
+
+static void sgns_negatives(const MetaPath& mp, const Tensor& walks, int64_t context_size, int64_t num_neg, int64_t seed,
+                           const Tensor& step, Tensor neg) {
+  c10::cuda::CUDAGuard guard(mp.device);
+  const auto [n_walks, L] = check_walks(walks, context_size,
+                                        "sgns_negatives: walks must be a contiguous int64 [n_walks, walk_length + 1] "
+                                        "tensor on the metapath's device");
+  check_negatives(neg, n_walks, L, context_size, num_neg,
+                  "sgns_negatives: neg must be a contiguous int64 [n_walks * windows * K, C] tensor on the device");
+  check_counters(step, 0, "sgns_negatives: step must be int32 [>= 1] on the device");
+  if (neg.numel() == 0) return;
+  launch_sgns_negatives(walks.data_ptr<int64_t>(), static_cast<int>(n_walks), static_cast<int>(L),
+                        static_cast<int>(context_size), static_cast<int>(num_neg), mp.R, mp.types,
+                        static_cast<uint64_t>(seed), step.data_ptr<int32_t>(), neg.data_ptr<int64_t>(), cur_stream());
+  check_cuda_err("sgns_negatives");
+}
+
+// emb / grad fp32 [rows >= mp.rows, D], D a multiple of 8 in [8, 512]; touched uint8 [rows]
+static void check_sgns_tables(const MetaPath& mp, const Tensor& emb, const Tensor& grad, const Tensor& touched,
+                              const char* who) {
+  const int64_t D = emb.dim() == 2 ? emb.size(1) : 0;
+  TORCH_CHECK(D % 8 == 0 && D >= 8 && D <= 512,
+              fmt("%s: emb must be fp32 [rows, D] with D a multiple of 8 in [8, 512]", who));
+  check_rows(emb, torch::kFloat32, D, fmt("%s: emb must be a contiguous fp32 [rows, D] tensor on the device", who).c_str());
+  TORCH_CHECK(emb.size(0) >= mp.rows, fmt("%s: emb has fewer rows than the metapath's node types", who));
+  check_rows(grad, torch::kFloat32, D, fmt("%s: grad must be a contiguous fp32 tensor of emb's shape", who).c_str());
+  TORCH_CHECK(grad.size(0) == emb.size(0), fmt("%s: grad must be a contiguous fp32 tensor of emb's shape", who));
+  TORCH_CHECK(on_dev(touched) && touched.scalar_type() == torch::kUInt8 && touched.is_contiguous() &&
+              touched.numel() == emb.size(0), fmt("%s: touched must be contiguous uint8 [rows] on the device", who));
+}
+
+// SGNS loss of the walks' valid windows and their negatives (written to loss[0]); gradient red.added into grad and
+// touched[row] = 1 for every row looked up.
+static void sgns_loss_grad(const MetaPath& mp, const Tensor& walks, const Tensor& neg, int64_t context_size,
+                           int64_t num_neg, const Tensor& emb, const Tensor& n_valid, Tensor grad, Tensor touched,
+                           Tensor loss) {
+  c10::cuda::CUDAGuard guard(mp.device);
+  const auto [n_walks, L] = check_walks(walks, context_size,
+                                        "sgns_loss_grad: walks must be a contiguous int64 [n_walks, walk_length + 1] "
+                                        "tensor on the metapath's device");
+  check_negatives(neg, n_walks, L, context_size, num_neg,
+                  "sgns_loss_grad: neg must be a contiguous int64 [n_walks * windows * K, C] tensor on the device");
+  check_sgns_tables(mp, emb, grad, touched, "sgns_loss_grad");
+  check_counters(n_valid, 0, "sgns_loss_grad: n_valid must be int32 [>= 1] on the device");
+  TORCH_CHECK(on_dev(loss) && loss.scalar_type() == torch::kFloat32 && loss.numel() >= 1,
+              "sgns_loss_grad: loss must be fp32 [>= 1] on the device");
+  launch_sgns_loss_grad(walks.data_ptr<int64_t>(), neg.data_ptr<int64_t>(), static_cast<int>(n_walks),
+                        static_cast<int>(L), static_cast<int>(context_size), static_cast<int>(num_neg), mp.R, mp.types,
+                        emb.data_ptr<float>(), static_cast<int>(emb.size(1)), n_valid.data_ptr<int32_t>(),
+                        grad.data_ptr<float>(), touched.data_ptr<uint8_t>(), loss.data_ptr<float>(), cur_stream());
+  check_cuda_err("sgns_loss_grad");
+}
+
+// torch.optim.SparseAdam step t = step[0] on the touched rows of emb / m / v; clears their grad rows and flags.
+static void sparse_adam(const MetaPath& mp, Tensor emb, Tensor grad, Tensor m, Tensor v, Tensor touched,
+                        const Tensor& step, double lr, double b1, double b2, double eps) {
+  c10::cuda::CUDAGuard guard(mp.device);
+  check_sgns_tables(mp, emb, grad, touched, "sparse_adam");
+  for (const Tensor* t : {&m, &v})
+    TORCH_CHECK(on_dev(*t) && t->scalar_type() == torch::kFloat32 && t->is_contiguous() && aligned16(*t) &&
+                t->sizes() == emb.sizes(), "sparse_adam: m and v must be contiguous fp32 tensors of emb's shape");
+  check_counters(step, 0, "sparse_adam: step must be int32 [>= 1] on the device");
+  TORCH_CHECK(lr > 0 && b1 >= 0 && b1 < 1 && b2 >= 0 && b2 < 1 && eps > 0,
+              "sparse_adam: need lr > 0, 0 <= betas < 1 and eps > 0");
+  launch_sparse_adam(emb.data_ptr<float>(), grad.data_ptr<float>(), m.data_ptr<float>(), v.data_ptr<float>(),
+                     touched.data_ptr<uint8_t>(), emb.size(0), static_cast<int>(emb.size(1)), step.data_ptr<int32_t>(),
+                     static_cast<float>(lr), static_cast<float>(b1), static_cast<float>(b2), static_cast<float>(eps),
+                     cur_stream());
+  check_cuda_err("sparse_adam");
+}
+
+// state int32 [3] = [next walk step, Adam step, walk step of the current step]
+static void m2v_begin(Tensor state) {
+  c10::cuda::CUDAGuard guard(state.device());
+  check_counters(state, 2, "m2v_begin: state must be int32 [>= 3] on the device");
+  launch_m2v_begin(state.data_ptr<int32_t>(), cur_stream());
+  check_cuda_err("m2v_begin");
+}
+
 static void dropout_bf16(Tensor Z, const Tensor& counters, int64_t n_hops, double p, int64_t seed, int64_t layer,
                          const c10::optional<Tensor>& step_dev) {
   c10::cuda::CUDAGuard guard(Z.device());
@@ -2242,6 +2398,21 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("seed"), py::arg("step"), py::arg("seeds"), py::arg("n_pairs"));
   m.def("link_bce", &link_bce, py::arg("Z"), py::arg("C"), py::arg("seed_local"), py::arg("P"), py::arg("B"),
         py::arg("n_pairs"), py::arg("loss"), py::arg("correct"), py::arg("dZ"));
+  py::class_<MetaPath>(m, "MetaPath")
+      .def(py::init<int, std::vector<GraphHandle*>, std::vector<int64_t>, std::vector<int64_t>>(), py::arg("device"),
+           py::arg("graphs"), py::arg("slot_off"), py::arg("slot_n"), py::keep_alive<1, 3>())
+      .def_readonly("R", &MetaPath::R)
+      .def_readonly("rows", &MetaPath::rows);
+  m.def("metapath_walk", &metapath_walk, py::arg("metapath"), py::arg("starts"), py::arg("walks_per_node"),
+        py::arg("context_size"), py::arg("seed"), py::arg("step"), py::arg("walks"), py::arg("n_valid"));
+  m.def("sgns_negatives", &sgns_negatives, py::arg("metapath"), py::arg("walks"), py::arg("context_size"),
+        py::arg("num_neg"), py::arg("seed"), py::arg("step"), py::arg("neg"));
+  m.def("sgns_loss_grad", &sgns_loss_grad, py::arg("metapath"), py::arg("walks"), py::arg("neg"),
+        py::arg("context_size"), py::arg("num_neg"), py::arg("emb"), py::arg("n_valid"), py::arg("grad"),
+        py::arg("touched"), py::arg("loss"));
+  m.def("sparse_adam", &sparse_adam, py::arg("metapath"), py::arg("emb"), py::arg("grad"), py::arg("m"), py::arg("v"),
+        py::arg("touched"), py::arg("step"), py::arg("lr"), py::arg("b1"), py::arg("b2"), py::arg("eps"));
+  m.def("m2v_begin", &m2v_begin, py::arg("state"));
   m.def("dropout_bf16", &dropout_bf16, py::arg("Z"), py::arg("counters"), py::arg("n_hops"), py::arg("p"),
         py::arg("seed"), py::arg("layer"), py::arg("step_dev") = py::none());
   m.def("zero_grads", &zero_grads);

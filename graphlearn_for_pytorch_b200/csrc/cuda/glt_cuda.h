@@ -325,6 +325,34 @@ void launch_link_seeds(GraphTable g, const int64_t* pos, int B, int k, int64_t n
 void launch_link_bce(const void* Z, int ld, int C, const int32_t* seed_local, int P, int B, const int32_t* n_pairs,
                      float* loss, int32_t* correct, float* dZ, cudaStream_t s);
 
+// ---- skipgram.cu (metapath2vec / DeepWalk skip-gram step) ---------------------------------------------------------
+constexpr int kMaxMetaPath = 8;
+// Node type of each walk position slot: slot 0 = source type of metapath[0], slot r + 1 = destination type of
+// metapath[r]; position p > 0 has slot (p - 1) % R + 1.  off = first row of the type in the concatenated embedding
+// table, n = node count of the type.
+struct MetaPathTypes {
+  int64_t off[kMaxMetaPath + 1];
+  int64_t n[kMaxMetaPath + 1];
+};
+// state = [next walk step, Adam step, walk step of the current step]: [2] = [0]; [0] += 1; [1] += 1.
+void launch_m2v_begin(int32_t* state, cudaStream_t s);
+// rel: device array of R GraphTables (CSR rows = source ids).  out: int64 [n_walks, L + 1]; walk i starts at
+// starts[i / W] and ends (-1 tail) at a dead end or an id outside its type.  *n_valid = #windows of C valid entries.
+void launch_metapath_walk(const GraphTable* rel, int R, MetaPathTypes types, const int64_t* starts, int n_walks, int W,
+                          int L, int C, uint64_t seed, const int32_t* step_dev, int64_t* out, int32_t* n_valid,
+                          cudaStream_t s);
+// neg: int64 [n_walks * (L + 2 - C) * K, C]; K negative windows per window of the walks (all -1 for an invalid one).
+void launch_sgns_negatives(const int64_t* walks, int n_walks, int L, int C, int K, int R, MetaPathTypes types,
+                           uint64_t seed, const int32_t* step_dev, int64_t* neg, cudaStream_t s);
+// SGNS loss (written to *loss) and its gradient red.added into grad (fp32 [rows, D], D % 8 == 0, D <= 512); sets
+// touched[row] for every row looked up.
+void launch_sgns_loss_grad(const int64_t* walks, const int64_t* neg, int n_walks, int L, int C, int K, int R,
+                           MetaPathTypes types, const float* emb, int D, const int32_t* n_valid, float* grad,
+                           uint8_t* touched, float* loss, cudaStream_t s);
+// torch.optim.SparseAdam step *t_dev on the touched rows of w / m / v, then clears their grad rows and flags.
+void launch_sparse_adam(float* w, float* grad, float* m, float* v, uint8_t* touched, int64_t rows, int D,
+                        const int32_t* t_dev, float lr, float b1, float b2, float eps, cudaStream_t s);
+
 // ---- gat.cu (relational GAT engine kernels; H = heads * C, H a multiple of 64 in [64, 1024], C % 8 == 0) -----------
 // Per-node attention scores of two row sets: out[set][row * heads + h] = <att[set][h], P[set][row, h*C : (h+1)*C]>
 // for row < min(cum[set][idx[set]], cap[set]).  P[1] == nullptr skips the second set.  zero (optional, fp32

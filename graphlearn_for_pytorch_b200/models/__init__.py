@@ -7,3 +7,4 @@ from .hgt import HGT, HGTConv
 from .hetero_engine import HeteroSageEngine
 from .hetero_gat_engine import HeteroGatEngine
 from .hetero_hgt_engine import HeteroHgtEngine
+from .metapath2vec import MetaPath2VecEngine
