@@ -1760,6 +1760,34 @@ static void metapath_walk(const MetaPath& mp, const Tensor& starts, int64_t walk
   check_cuda_err("metapath_walk");
 }
 
+// node2vec's p / q walks of one step over a metapath of one relation from a type to itself; the same contract as
+// metapath_walk.  max(1, 1/p, 1/q) / min(1, 1/p, 1/q) <= 64 bounds the rejection sampler's expected proposals.
+static void node2vec_walk(const MetaPath& mp, const Tensor& starts, int64_t walks_per_node, int64_t context_size,
+                          int64_t seed, const Tensor& step, Tensor walks, Tensor n_valid, double p, double q) {
+  c10::cuda::CUDAGuard guard(mp.device);
+  TORCH_CHECK(std::isfinite(p) && std::isfinite(q) && p > 0 && q > 0, "node2vec_walk: p and q must be finite and > 0");
+  const double hi = std::max({1.0, 1.0 / p, 1.0 / q}), lo = std::min({1.0, 1.0 / p, 1.0 / q});
+  TORCH_CHECK(hi / lo <= 64.0, "node2vec_walk: max(1, 1/p, 1/q) / min(1, 1/p, 1/q) must be <= 64");
+  TORCH_CHECK(mp.R == 1 && mp.types.off[0] == mp.types.off[1] && mp.types.n[0] == mp.types.n[1],
+              "node2vec_walk: the metapath must be one relation from a node type to itself");
+  check_ids(starts, "node2vec_walk: starts must be contiguous int64 on the metapath's device");
+  TORCH_CHECK(walks_per_node >= 1, "node2vec_walk: walks_per_node must be >= 1");
+  const auto [n_walks, L] = check_walks(walks, context_size,
+                                        "node2vec_walk: walks must be a contiguous int64 [n_walks, walk_length + 1] "
+                                        "tensor on the metapath's device");
+  TORCH_CHECK(L <= kNode2VecMaxWalk, fmt("node2vec_walk: walk_length must be <= %d", kNode2VecMaxWalk));
+  TORCH_CHECK(n_walks == starts.numel() * walks_per_node, "node2vec_walk: walks needs starts * walks_per_node rows");
+  check_counters(step, 0, "node2vec_walk: step must be int32 [>= 1] on the device");
+  check_counters(n_valid, 0, "node2vec_walk: n_valid must be int32 [>= 1] on the device");
+  if (n_walks == 0) return;
+  launch_node2vec_walk(mp.dev_tables(), mp.types, starts.data_ptr<int64_t>(), static_cast<int>(n_walks),
+                       static_cast<int>(walks_per_node), static_cast<int>(L), static_cast<int>(context_size),
+                       static_cast<float>(1.0 / p / hi), static_cast<float>(1.0 / hi), static_cast<float>(1.0 / q / hi),
+                       static_cast<uint64_t>(seed), step.data_ptr<int32_t>(), walks.data_ptr<int64_t>(),
+                       n_valid.data_ptr<int32_t>(), cur_stream());
+  check_cuda_err("node2vec_walk");
+}
+
 static void sgns_negatives(const MetaPath& mp, const Tensor& walks, int64_t context_size, int64_t num_neg, int64_t seed,
                            const Tensor& step, Tensor neg) {
   c10::cuda::CUDAGuard guard(mp.device);
@@ -2405,6 +2433,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def_readonly("rows", &MetaPath::rows);
   m.def("metapath_walk", &metapath_walk, py::arg("metapath"), py::arg("starts"), py::arg("walks_per_node"),
         py::arg("context_size"), py::arg("seed"), py::arg("step"), py::arg("walks"), py::arg("n_valid"));
+  m.def("node2vec_walk", &node2vec_walk, py::arg("metapath"), py::arg("starts"), py::arg("walks_per_node"),
+        py::arg("context_size"), py::arg("seed"), py::arg("step"), py::arg("walks"), py::arg("n_valid"), py::arg("p"),
+        py::arg("q"));
   m.def("sgns_negatives", &sgns_negatives, py::arg("metapath"), py::arg("walks"), py::arg("context_size"),
         py::arg("num_neg"), py::arg("seed"), py::arg("step"), py::arg("neg"));
   m.def("sgns_loss_grad", &sgns_loss_grad, py::arg("metapath"), py::arg("walks"), py::arg("neg"),

@@ -88,9 +88,8 @@ __device__ __forceinline__ int64_t load_col(const GraphTable& g, int part, int64
   return __ldg(reinterpret_cast<const int64_t*>(g.parts[part].indices) + pos);
 }
 
-// Strict edge test: is c a neighbour of r?  Binary search of r's row (rows are column-sorted, Topology guarantees it).
-__device__ __forceinline__ bool edge_exists(const GraphTable& g, int64_t r, int64_t c) {
-  const RowRef row = load_row(g, r);
+// Is c in the (column-sorted) row already located by load_row?  Binary search.
+__device__ __forceinline__ bool row_has_col(const GraphTable& g, const RowRef& row, int64_t c) {
   int64_t lo = 0, hi = row.deg;
   while (lo < hi) {
     const int64_t mid = (lo + hi) >> 1;
@@ -99,6 +98,11 @@ __device__ __forceinline__ bool edge_exists(const GraphTable& g, int64_t r, int6
     if (x < c) lo = mid + 1; else hi = mid;
   }
   return false;
+}
+
+// Strict edge test: is c a neighbour of r?  Binary search of r's row (rows are column-sorted, Topology guarantees it).
+__device__ __forceinline__ bool edge_exists(const GraphTable& g, int64_t r, int64_t c) {
+  return row_has_col(g, load_row(g, r), c);
 }
 
 __device__ __forceinline__ unsigned lanemask_lt() {

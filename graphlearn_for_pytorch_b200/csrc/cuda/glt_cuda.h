@@ -341,6 +341,14 @@ void launch_m2v_begin(int32_t* state, cudaStream_t s);
 void launch_metapath_walk(const GraphTable* rel, int R, MetaPathTypes types, const int64_t* starts, int n_walks, int W,
                           int L, int C, uint64_t seed, const int32_t* step_dev, int64_t* out, int32_t* n_valid,
                           cudaStream_t s);
+// node2vec's second-order walk over one relation from a type to itself (column-sorted CSR rows): the same output and
+// dead-end contract as launch_metapath_walk.  w_ret / w_in / w_out are the unnormalised weights 1/p, 1 and 1/q divided
+// by their maximum; L <= kNode2VecMaxWalk keeps the draw counters from wrapping.
+constexpr int kNode2VecMaxProposals = 4096;
+constexpr int kNode2VecMaxWalk = 1 << 20;
+void launch_node2vec_walk(const GraphTable* rel, MetaPathTypes types, const int64_t* starts, int n_walks, int W, int L,
+                          int C, float w_ret, float w_in, float w_out, uint64_t seed, const int32_t* step_dev,
+                          int64_t* out, int32_t* n_valid, cudaStream_t s);
 // neg: int64 [n_walks * (L + 2 - C) * K, C]; K negative windows per window of the walks (all -1 for an invalid one).
 void launch_sgns_negatives(const int64_t* walks, int n_walks, int L, int C, int K, int R, MetaPathTypes types,
                            uint64_t seed, const int32_t* step_dev, int64_t* neg, cudaStream_t s);

@@ -2,6 +2,7 @@
 // SGNS loss + gradient, and a sparse Adam over the rows the step looked up.  One training step is
 //   k_m2v_begin       advance the device step counters (walk step, Adam step)
 //   k_metapath_walk   thread per walk: uniform neighbour in relation metapath[(s - 1) % R]; counts valid windows
+//     or k_node2vec_walk  warp per walk: node2vec's p / q second-order rule, 32 rejection-sampling proposals at a time
 //   k_sgns_negatives  thread per (window, k): a negative window keeps the centre, draws each context position
 //   k_sgns_loss_grad  lane group per window: its C - 1 positive pairs and K negative windows share the centre row
 //   k_sparse_adam     warp per 32 rows: the rows flagged "touched" get torch.optim.SparseAdam's update
@@ -21,6 +22,7 @@ namespace {
 // Philox streams of the walk and negative draws; the draw row is (step << 32) | item, so steps never collide.
 constexpr uint32_t kWalkStream = 0x4D325657u;
 constexpr uint32_t kNegStream = 0x4D32564Eu;
+constexpr uint32_t kN2vStream = 0x4E325657u;   // node2vec proposals: the counter word is (walk step, proposal)
 constexpr float kSgnsEps = 1e-15f;   // PyG MetaPath2Vec's EPS inside the logs
 
 // Position p of a walk has the node type of slot(p): slot 0 is the source type of metapath[0], slot r + 1 the
@@ -72,6 +74,74 @@ __global__ void __launch_bounds__(128) k_metapath_walk(const GraphTable* rel, in
 #pragma unroll
     for (int off = 16; off > 0; off >>= 1) win += __shfl_xor_sync(0xffffffffu, win, off);
     if ((threadIdx.x & 31) == 0 && win > 0) atomicAdd(n_valid, win);
+  }
+}
+
+// node2vec's second-order walk (Grover & Leskovec 2016) over one relation from a type to itself, warp per walk.  Walk
+// i starts at starts[i / W].  Step 1 moves to a uniform neighbour.  Step s >= 2, at v with previous node t, weighs every
+// entry x of v's row 1/p if x == t, 1 if t's row holds x, 1/q otherwise, and samples it by rejection: propose x
+// uniformly from v's row and accept with probability w(x) / max(1, 1/p, 1/q) (w_ret / w_in / w_out are the normalised
+// weights).  Proposal k of step s draws Philox(seed, kN2vStream, (step << 32) | i, counter (s - 1) * 4096 + k): word
+// x picks the entry, word y is the acceptance uniform.  Lane l evaluates proposals l, l + 32, ... (its own binary
+// search of t's row) and the warp takes the lowest-indexed accepted one, which has exactly the distribution of
+// sequential rejection sampling, so a walk is a function of (seed, step, i) alone.  After kNode2VecMaxProposals
+// rejections the last proposal is taken: with r = max/min weight <= 64 (enforced by the binding) each proposal is
+// accepted with probability >= 1/64, so this happens with probability < (63/64)^4096 ~ 1e-28 per walk step.
+// Dead ends, ids outside [0, n) and padded starts end the walk (-1 tail) exactly as in k_metapath_walk, and n_valid +=
+// the walk's windows of C valid entries.  Rows must be column-sorted for row_has_col's binary search.
+__global__ void __launch_bounds__(128) k_node2vec_walk(const GraphTable* rel, MetaPathTypes types,
+                                                       const int64_t* starts, int n_walks, int W, int L, int C,
+                                                       float w_ret, float w_in, float w_out, uint64_t seed,
+                                                       const int32_t* step_dev, int64_t* out, int32_t* n_valid) {
+  pdl_enter();
+  const GraphTable& g = *rel;
+  const uint64_t step = static_cast<uint32_t>(*step_dev);
+  const int lane = threadIdx.x & 31;
+  const int64_t n = types.n[0];
+  // the membership search only decides acceptance when u falls between the two weights of x != t
+  const float w_lo = fminf(w_in, w_out), w_hi = fmaxf(w_in, w_out);
+  for (int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n_walks; i += (gridDim.x * blockDim.x) >> 5) {
+    int64_t* w = out + static_cast<int64_t>(i) * (L + 1);
+    int64_t cur = starts[i / W];
+    if (cur < 0 || cur >= n) cur = -1;
+    if (lane == 0) w[0] = cur;
+    int valid = cur >= 0;
+    int64_t prev = -1;
+    RowRef prow{};
+    const uint32_t row_lo = static_cast<uint32_t>(i), row_hi = static_cast<uint32_t>(step);
+    for (int s = 1; s <= L; ++s) {
+      if (cur >= 0) {                                 // warp-uniform: every lane holds the same walk state
+        const RowRef r = load_row(g, cur);
+        int64_t nxt = -1;
+        if (r.deg > 0) {
+          for (int k0 = 0; k0 < kNode2VecMaxProposals; k0 += 32) {
+            const U4 d = philox4x32_10(static_cast<uint32_t>(seed), static_cast<uint32_t>(seed >> 32),
+                                       U4{row_lo, row_hi, static_cast<uint32_t>(s - 1) * kNode2VecMaxProposals +
+                                                              static_cast<uint32_t>(k0 + lane), kN2vStream});
+            const int64_t x = load_col(g, r.part, r.start + bounded(d.x, static_cast<uint32_t>(r.deg)));
+            const float u = u01(d.y);
+            bool acc;
+            if (prev < 0) acc = true;                 // step 1: uniform
+            else if (x == prev) acc = u < w_ret;
+            else if (u < w_lo) acc = true;
+            else if (u >= w_hi) acc = false;
+            else acc = row_has_col(g, prow, x) ? u < w_in : u < w_out;
+            const unsigned hit = __ballot_sync(0xffffffffu, acc);
+            const int src = hit ? __ffs(hit) - 1 : 31;
+            nxt = __shfl_sync(0xffffffffu, x, src);
+            if (hit) break;
+          }
+          if (nxt >= n) nxt = -1;
+        }
+        prev = cur;
+        prow = r;
+        cur = nxt;
+        valid += cur >= 0;
+      }
+      if (lane == 0) w[s] = cur;
+    }
+    const int win = valid >= C ? valid - C + 1 : 0;
+    if (lane == 0 && win > 0) atomicAdd(n_valid, win);
   }
 }
 
@@ -285,6 +355,14 @@ void launch_metapath_walk(const GraphTable* rel, int R, MetaPathTypes types, con
   cudaMemsetAsync(n_valid, 0, sizeof(int32_t), s);
   launch_k(k_metapath_walk, dim3(grid_for(n_walks, 128)), dim3(128), 0, s, rel, R, types, starts, n_walks, W, L, C,
            seed, step_dev, out, n_valid);
+}
+
+void launch_node2vec_walk(const GraphTable* rel, MetaPathTypes types, const int64_t* starts, int n_walks, int W, int L,
+                          int C, float w_ret, float w_in, float w_out, uint64_t seed, const int32_t* step_dev,
+                          int64_t* out, int32_t* n_valid, cudaStream_t s) {
+  cudaMemsetAsync(n_valid, 0, sizeof(int32_t), s);
+  launch_k(k_node2vec_walk, dim3(grid_for(n_walks, 4)), dim3(128), 0, s, rel, types, starts, n_walks, W, L, C, w_ret,
+           w_in, w_out, seed, step_dev, out, n_valid);
 }
 
 void launch_sgns_negatives(const int64_t* walks, int n_walks, int L, int C, int K, int R, MetaPathTypes types,

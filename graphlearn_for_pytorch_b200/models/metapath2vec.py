@@ -5,12 +5,14 @@ embeddings with the project's sm_90a kernels (csrc/cuda/skipgram.cu).  Per step,
 
   m2v_begin        advance the device step counters (walk step, Adam step)
   metapath_walk    walks_per_node walks per start node along the metapath, -1 after a dead end
+                   (node2vec_walk instead for node2vec's p / q walks)
   sgns_negatives   num_negative_samples negative windows per valid window
   sgns_loss_grad   SGNS loss and its gradient into fp32 gradient rows; marks the rows it looked up
   sparse_adam      torch.optim.SparseAdam on the marked rows, then clears their gradients and marks
 
 No step reads anything back to the host, so the step is captured into one CUDA graph.
 """
+import math
 from typing import Dict, List, Optional, Sequence, Tuple
 
 import torch
@@ -30,6 +32,8 @@ class MetaPath2VecEngine:
     metapath: up to 8 relations that chain (the destination of one is the source of the next); when walk_length
       exceeds their number the path must also close (the last destination is the first source).  A homogeneous
       graph with metapath [('n', 'to', 'n')] trains DeepWalk (node2vec with p = q = 1).
+    p, q: node2vec's return and in-out parameters (default 1, 1: uniform walks).  Other values need a metapath of one
+      relation from a type to itself, finite p, q > 0 and max(1, 1/p, 1/q) / min(1, 1/p, 1/q) <= 64.
     embedding_dim: a multiple of 8 in [8, 512].
     walk_length, context_size, walks_per_node, num_negative_samples: as PyG's `MetaPath2Vec`
       (2 <= context_size <= walk_length + 1).
@@ -45,6 +49,14 @@ class MetaPath2VecEngine:
   position's node type (standard SGNS).  PyG instead slices independent random walks for its negatives, whose
   centres are random too.
 
+  With p, q != 1 the walks are node2vec's second-order walks (PyG `Node2Vec(..., p=p, q=q)`): step 1 is uniform; at
+  step s >= 2, at v coming from t, an entry x of v's row weighs 1/p if x == t, 1 if the graph holds the edge (t, x)
+  and 1/q otherwise.  It is drawn by exact rejection sampling (propose uniformly from v's row, accept with probability
+  weight / max(1, 1/p, 1/q)), as torch_cluster does; after 4096 rejected proposals the last one is taken, which at
+  the ratio bound of 64 happens with probability < 1e-28 per walk step.  The edge test binary-searches t's row, so
+  every CSR row must be column-sorted: graphs built through `Topology` are; shards handed to `Graph.from_shards` must
+  be too.  A dead end ends the walk with -1 as above, where torch_cluster's walker instead stays on an isolated node.
+
   After a step, `walks` (int64 [batch_size * walks_per_node, walk_length + 1]) and `negatives` (int64
   [walks * windows * num_negative_samples, context_size], window-major, all -1 for an invalid window) hold what the
   step used.  `_sample`, `_loss_grad` and `_update` are the step's three stages, for inspection between them.
@@ -53,7 +65,7 @@ class MetaPath2VecEngine:
   def __init__(self, graphs: Dict[EdgeType, object], num_nodes: Dict[str, int], metapath: Sequence[EdgeType],
                embedding_dim: int = 128, walk_length: int = 64, context_size: int = 7, walks_per_node: int = 5,
                num_negative_samples: int = 5, batch_size: int = 128, lr: float = 0.01, seed: int = 0,
-               device: Optional[torch.device] = None, use_cuda_graph: bool = True):
+               device: Optional[torch.device] = None, use_cuda_graph: bool = True, p: float = 1.0, q: float = 1.0):
     metapath = [tuple(e) for e in metapath]
     R = len(metapath)
     if not 1 <= R <= 8:
@@ -81,6 +93,14 @@ class MetaPath2VecEngine:
       raise ValueError('walks_per_node, num_negative_samples and batch_size must be >= 1')
     if not lr > 0:
       raise ValueError(f'lr must be > 0 (got {lr})')
+    p, q = float(p), float(q)
+    if not (math.isfinite(p) and math.isfinite(q) and p > 0 and q > 0):
+      raise ValueError(f'p and q must be finite and > 0 (got p={p}, q={q})')
+    ws = (1.0, 1.0 / p, 1.0 / q)
+    if max(ws) / min(ws) > 64:
+      raise ValueError(f'max(1, 1/p, 1/q) / min(1, 1/p, 1/q) must be <= 64 (got p={p}, q={q})')
+    if (p, q) != (1.0, 1.0) and (R != 1 or metapath[0][0] != metapath[0][2]):
+      raise ValueError('p and q other than 1 need a metapath of one relation from a node type to itself')
     slot_types = [metapath[0][0]] + [e[2] for e in metapath]
     for t in slot_types:
       if t not in num_nodes or not 1 <= int(num_nodes[t]) < 2 ** 32:
@@ -98,6 +118,7 @@ class MetaPath2VecEngine:
     self.embedding_dim, self.walk_length, self.context_size = D, L, C
     self.walks_per_node, self.num_negative_samples, self.batch_size = W, K, B
     self.lr, self.seed, self.use_cuda_graph = float(lr), int(seed), bool(use_cuda_graph)
+    self.p, self.q = p, q
     self.betas, self.eps = (0.9, 0.999), 1e-8
     # one table per node type, concatenated in order of first appearance on the path
     self.node_types: List[str] = list(dict.fromkeys(slot_types))
@@ -136,8 +157,12 @@ class MetaPath2VecEngine:
   def _sample(self):
     nat, cur = self.nat, self.state[2:3]
     nat.m2v_begin(self.state)
-    nat.metapath_walk(self.mp, self.starts, self.walks_per_node, self.context_size, self.seed, cur, self.walks,
-                      self.n_valid)
+    if (self.p, self.q) == (1.0, 1.0):
+      nat.metapath_walk(self.mp, self.starts, self.walks_per_node, self.context_size, self.seed, cur, self.walks,
+                        self.n_valid)
+    else:
+      nat.node2vec_walk(self.mp, self.starts, self.walks_per_node, self.context_size, self.seed, cur, self.walks,
+                        self.n_valid, self.p, self.q)
     nat.sgns_negatives(self.mp, self.walks, self.context_size, self.num_negative_samples, self.seed, cur,
                        self.negatives)
 
