@@ -276,6 +276,7 @@ __global__ void __launch_bounds__(kThreads3, 1) k_sage_fused3(SageFusedArgs f) {
               const int sidx = __ldg(ellrow + j);
               if (sidx < 0) continue;
               const uint8_t* p = src_row(a, sidx);
+              if (p == nullptr) continue;  // an id the table does not hold: a zero row, still counted in dg
               mxfp8x16_accum(ld_nc_v4(p + gl * 16), ld_nc_u32(p + a.d), gl, acc);
             }
           }
@@ -354,6 +355,7 @@ __global__ void __launch_bounds__(kThreads3, 1) k_sage_fused3(SageFusedArgs f) {
             const int sidx = __ldg(ellrow + j);
             if (sidx < 0) continue;
             const uint8_t* p = src_row(a, sidx);
+            if (p == nullptr) continue;  // an id the table does not hold: a zero row, still counted in dg
 #pragma unroll
             for (int c = 0; c < NC; ++c) bf16x8_accum(ld_nc_v4(p + c * kChunkBytes + gl * 16), acc[c]);
           }
