@@ -1627,6 +1627,7 @@ static void hgt_kqv_cast(Tensor dkv, const c10::optional<Tensor>& dq, Tensor out
     check_rows(*dq, torch::kBFloat16, H, "hgt_kqv_cast: dq must be contiguous bf16 [rows, H]");
     check_counters(counters, idx_q, "hgt_kqv_cast: counters must be int32 [> idx_q] on the device");
     a.dq = dq->data_ptr();
+    a.cap_q = dq->size(0);
   }
   if (has(bias_g)) {
     check_vec(*bias_g, torch::kFloat32, 3 * H, "hgt_kqv_cast: bias_g must be fp32 [3H]");

@@ -558,6 +558,7 @@ struct HgtKqvCastArgs {
   float* bias_g;
   const int32_t* cum;
   int idx, idx_q, cap, H;
+  int cap_q;                 // rows of dq: nq is clamped to it like every extent read from a counter
 };
 void launch_hgt_kqv_cast(const HgtKqvCastArgs& a, cudaStream_t s);
 

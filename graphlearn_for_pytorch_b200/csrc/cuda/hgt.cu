@@ -480,15 +480,16 @@ __global__ void __launch_bounds__(256) k_hgt_blocks(HgtBlockArgs a) {
 }
 
 // bf16 gradient rows [dK | dQ | dV] of a type's K/Q/V projection (the A operand of its weight- and data-gradient GEMMs)
-// from the fp32 attention gradients dKV = [dK | dV] (rows < n, re-zeroed after reading) and the bf16 dQ (rows < nq);
-// rows [n, round_up(n, 128)) are zeros.  bias_g [3H] += the column sums of the bf16 rows, one atomic per column per CTA.
+// from the fp32 attention gradients dKV = [dK | dV] (rows < n, re-zeroed after reading) and the bf16 dQ (rows < nq,
+// nq = min(cum[idx_q], n, rows of dQ)); rows [n, round_up(n, 128)) are zeros.  bias_g [3H] += the column sums of the
+// bf16 rows, one atomic per column per CTA.
 // Threads: a chunk of up to 128 vectors (blockIdx.y) times 256 / chunk rows.
 __global__ void __launch_bounds__(256) k_hgt_kqv_cast(HgtKqvCastArgs a) {
   pdl_enter();
   __shared__ float s_acc[256][8];
   const int nv = a.H >> 3, nvec = 3 * nv;
   const int n = min(a.cum[a.idx], a.cap);
-  const int nq = a.dq ? min(a.cum[a.idx_q], n) : 0;
+  const int nq = a.dq ? min(min(a.cum[a.idx_q], n), a.cap_q) : 0;
   const int cw = min(nvec, 128);
   const int c0 = blockIdx.y * 128;
   const int cg = threadIdx.x % cw, rl = threadIdx.x / cw;

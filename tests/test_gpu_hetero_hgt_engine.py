@@ -2,8 +2,9 @@
 
 Kernels: `hgt_attention` and `hgt_attention_bwd` on hand-built ELL batches with 1, 2 and 4 relations into one type,
 each with its own fan-outs (rows of degree 0, 1 and k with a k = 512 hub, -1 slots, three hops, rows with neighbours in
-one relation only and rows with none), at heads 1 to 8 and head widths D from 8 to 256, with equal scores and scores
-near 100 (where an unshifted exp overflows), against float64 autograd with explicit error bounds.
+one relation only and rows with none), at heads 1 to 128 and head widths D from 8 to 256, with equal scores and scores
+near 100 (where an unshifted exp overflows), against float64 autograd with explicit error bounds; and once with 8
+relations x 128 heads, the most per-(relation, head) prior partials the backward reduces in shared memory.
 
 Engine: one step against an fp32 PyTorch recomputation of the HGT model from the arena's COO on the SAME sampled batch,
 rounding to bf16 where the engine stores bf16; the same logits as `models.HGTConv` loaded with the engine's weights;
@@ -25,8 +26,9 @@ DEV = torch.device('cuda', 0)
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), 'examples'))
 EPS32 = 2.0 ** -23
 ROWS = [3, 50, 400]                                     # target rows per hop
-FANS = [(512, 7, 3), (64, 5, 2), (16, 9, 4), (2, 3, 6)]  # per relation: k per hop (relation 0 has the hub)
-N_SRC = [600, 300, 450, 100]
+FANS = [(512, 7, 3), (64, 5, 2), (16, 9, 4), (2, 3, 6),  # per relation: k per hop (relation 0 has the hub)
+        (32, 4, 2), (8, 6, 3), (128, 2, 5), (3, 8, 1)]
+N_SRC = [600, 300, 450, 100, 250, 500, 350, 150]
 
 
 # --------------------------------------------------------------------------- kernels against float64
@@ -77,14 +79,26 @@ def _counters(vals):
   return c.to(DEV)
 
 
-# (heads, D): H = heads * D from 64 to 1024, D in {8, 24, 32, 48, 64, 128, 256}
-SHAPES = [(1, 64), (1, 256), (2, 32), (4, 48), (8, 24), (8, 8), (4, 256), (8, 128)]
+# (heads, D): H = heads * D from 64 to 1024, D in {8, 16, 24, 32, 48, 64, 128, 256}.  Up to 8 heads a lane owns at
+# most one head's softmax statistics; 64 and 128 heads exceed the 32 lanes of a row, so each lane owns 2 or 4 heads.
+SHAPES = [(1, 64), (1, 256), (2, 32), (4, 48), (8, 24), (8, 8), (4, 256), (8, 128),
+          (16, 8), (32, 16), (64, 8), (128, 8)]
 
 
 @pytest.mark.parametrize('scores', ['normal', 'equal', 'large'])
 @pytest.mark.parametrize('R', [1, 2, 4])
 @pytest.mark.parametrize('heads,D', SHAPES)
 def test_hgt_attention_kernels_match_fp64(native, heads, D, R, scores):
+  _attention_case(native, heads, D, R, scores)
+
+
+@pytest.mark.parametrize('scores', ['normal', 'large'])
+def test_hgt_attention_kernels_8_relations_128_heads(native, scores):
+  """8 relations x 128 heads of width 8: the backward's shared prior partials s_prior[kHgtMaxRel * 128] are full."""
+  _attention_case(native, 128, 8, 8, scores)
+
+
+def _attention_case(native, heads, D, R, scores):
   H = heads * D
   cum, degs, ells = _structure(R, seed=H + heads + R)
   T = cum[-1]
@@ -414,7 +428,9 @@ IGBH_WIDTHS = {'paper': 1024, 'author': 256, 'institute': 64, 'fos': 128}
     ('mag', 64, 64, 1, 20, (4, 3)),                   # one head
     ('mag', 128, 256, 8, 20, (4, 3)),                 # eight heads of 32
     ('igbh', IGBH_WIDTHS, 64, 2, 2983, (4, 3, 2)),    # IGBH per-type widths, three layers, 2983 classes
-], ids=['mag-64-h2', 'mag-64-h1', 'mag-256-h8', 'igbh_widths-64-h2-L3-2983'])
+    ('mag', 128, 512, 8, 20, (4, 3)),                 # K/Q/V gradient rows of 192 vectors: two column chunks
+    ('mag', 128, 704, 8, 20, (4, 3)),                 # 264 vectors: three chunks, the last of 8; heads of 88
+], ids=['mag-64-h2', 'mag-64-h1', 'mag-256-h8', 'igbh_widths-64-h2-L3-2983', 'mag-512-h8', 'mag-704-h8'])
 def test_hetero_hgt_engine_gradients_match_fp32(schema, feat_dim, hidden, heads, classes, fan):
   eng, fb, labels, sizes = _build(schema, feat_dim, hidden, heads, classes, fan)
   errs, info = _gradient_errors(eng, fb, labels, sizes)

@@ -286,8 +286,8 @@ def _kernel_graph(n_dst, n_src, seed, hub_deg=600):
   return graph, d, topo.indices.to(DEV).long()
 
 
-# (heads, C): H = heads * C from 64 to 1024
-SHAPES = [(1, 64), (2, 64), (4, 48), (8, 8), (1, 256), (8, 128), (4, 256)]
+# (heads, C): H = heads * C from 64 to 1024; 64 and 128 heads give each lane of a row several heads
+SHAPES = [(1, 64), (2, 64), (4, 48), (8, 8), (1, 256), (8, 128), (4, 256), (16, 8), (32, 16), (64, 8), (128, 8)]
 
 
 @pytest.mark.parametrize('scores', ['normal', 'large'])
