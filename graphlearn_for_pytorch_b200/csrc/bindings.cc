@@ -1867,6 +1867,161 @@ static void m2v_begin(Tensor state) {
   check_cuda_err("m2v_begin");
 }
 
+// ---------------------------------------------------------------------------
+// SealArena: the static per-link arena and parameter layout of SealEngine's step (cuda/seal.cu).
+// ---------------------------------------------------------------------------
+struct SealArena {
+  int device;
+  SealModel model{};
+  SealArenaPtrs ptrs{};
+  int cap_max;
+  std::vector<std::tuple<std::string, int64_t, std::vector<int64_t>>> layout;
+  Tensor nodes, z, meta, sptr, scol, dptr, dcol, X, XW, G, C1, flat, H1, mask, sel, logits, lossv, dlogit, samp, partials;
+
+  SealArena(int dev, int64_t B, int64_t max_nodes, int64_t max_edges, int64_t hidden, int64_t num_layers, int64_t Z,
+            int64_t k, int64_t cap_max_)
+      : device(dev), cap_max(static_cast<int>(cap_max_)) {
+    c10::cuda::CUDAGuard guard(device);
+    TORCH_CHECK(B >= 1 && B <= (1 << 20), "SealArena: batch size must be in [1, 2^20]");
+    TORCH_CHECK(max_nodes >= 2 && max_nodes <= kSealMaxNodes, fmt("SealArena: max_nodes must be in [2, %d]", kSealMaxNodes));
+    TORCH_CHECK(max_edges >= 1 && max_edges <= (1 << 24), "SealArena: max_edges must be in [1, 2^24]");
+    TORCH_CHECK(hidden >= 1 && hidden <= 256, "SealArena: hidden must be in [1, 256]");
+    TORCH_CHECK(num_layers >= 1 && num_layers <= kSealMaxLayers, fmt("SealArena: num_layers must be in [1, %d]", kSealMaxLayers));
+    TORCH_CHECK(Z >= 2 && Z <= (1 << 20), "SealArena: the label count max_z + 1 must be in [2, 2^20]");
+    TORCH_CHECK(k >= 10 && k <= 2 * kSealMaxNodes, fmt("SealArena: sort-pool k must be in [10, %d]", 2 * kSealMaxNodes));
+    TORCH_CHECK(cap_max_ >= 0 && cap_max_ <= max_nodes, "SealArena: neighbour caps must be in [0, max_nodes]");
+    SealModel& m = model;
+    m.H = static_cast<int>(hidden); m.L = static_cast<int>(num_layers); m.Z = static_cast<int>(Z);
+    m.total = m.H * m.L + 1; m.k = static_cast<int>(k); m.dense = (m.k / 2 - 4) * 32;
+    int64_t off = 0;
+    auto add = [&](const std::string& name, std::vector<int64_t> shape) {
+      int64_t n = 1;
+      for (int64_t x : shape) n *= x;
+      layout.emplace_back(name, off, shape);
+      const int64_t at = off;
+      off += n;
+      return at;
+    };
+    for (int l = 0; l <= m.L; ++l) {
+      const int64_t out = l < m.L ? m.H : 1, in = l == 0 ? m.Z : m.H;
+      m.w[l] = add(fmt("convs.%d.lin.weight", l), {out, in});
+      m.bias[l] = add(fmt("convs.%d.bias", l), {out});
+    }
+    m.c1w = add("conv1.weight", {16, 1, m.total});
+    m.c1b = add("conv1.bias", {16});
+    m.c2w = add("conv2.weight", {32, 16, 5});
+    m.c2b = add("conv2.bias", {32});
+    m.l1w = add("mlp.lins.0.weight", {128, m.dense});
+    m.l1b = add("mlp.lins.0.bias", {128});
+    m.l2w = add("mlp.lins.1.weight", {1, 128});
+    m.l2b = add("mlp.lins.1.bias", {1});
+    m.P = off;
+    int optin = 0;
+    cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device);
+    const size_t need = std::max({seal_extract_smem(static_cast<int>(max_nodes)),
+                                  seal_forward_smem(m, static_cast<int>(max_nodes)),
+                                  seal_backward_smem(m, static_cast<int>(max_nodes))});
+    TORCH_CHECK(need <= static_cast<size_t>(optin),
+                fmt("SealArena: the per-link kernels need %zu bytes of shared memory (device limit %d); lower max_nodes, "
+                    "hidden or k", need, optin));
+    const auto f32 = torch::TensorOptions().dtype(torch::kFloat32).device(torch::kCUDA, device);
+    const auto i32 = f32.dtype(torch::kInt32);
+    nodes = torch::full({B, max_nodes}, -1, f32.dtype(torch::kInt64));
+    z = torch::zeros({B, max_nodes}, i32);
+    meta = torch::zeros({B, kSealMeta}, i32);
+    sptr = torch::zeros({B, max_nodes + 1}, i32);
+    dptr = torch::zeros({B, max_nodes + 1}, i32);
+    scol = torch::zeros({B, max_edges}, f32.dtype(torch::kInt16));
+    dcol = torch::zeros({B, max_edges}, f32.dtype(torch::kInt16));
+    X = torch::zeros({B, max_nodes, m.total}, f32);
+    XW = torch::zeros({B, max_nodes, m.H}, f32);
+    G = torch::zeros({B, max_nodes, m.total}, f32);
+    C1 = torch::zeros({B, 16, m.k}, f32);
+    flat = torch::zeros({B, m.dense}, f32);
+    H1 = torch::zeros({B, 128}, f32);
+    mask = torch::zeros({B, 128}, f32);
+    sel = torch::full({B, m.k}, -1, i32);
+    logits = torch::zeros({B}, f32);
+    lossv = torch::zeros({B}, f32);
+    dlogit = torch::zeros({B}, f32);
+    samp = torch::zeros({cap_max > 0 ? B * max_nodes * cap_max : 1}, i32);
+    partials = torch::zeros({B, m.P}, f32);
+    SealArenaPtrs& p = ptrs;
+    p.B = static_cast<int>(B); p.max_nodes = static_cast<int>(max_nodes); p.max_edges = static_cast<int>(max_edges);
+    p.nodes = nodes.data_ptr<int64_t>(); p.z = z.data_ptr<int32_t>(); p.meta = meta.data_ptr<int32_t>();
+    p.sptr = sptr.data_ptr<int32_t>(); p.scol = scol.data_ptr<int16_t>();
+    p.dptr = dptr.data_ptr<int32_t>(); p.dcol = dcol.data_ptr<int16_t>();
+    p.X = X.data_ptr<float>(); p.XW = XW.data_ptr<float>(); p.G = G.data_ptr<float>(); p.C1 = C1.data_ptr<float>();
+    p.flat = flat.data_ptr<float>(); p.H1 = H1.data_ptr<float>(); p.mask = mask.data_ptr<float>();
+    p.sel = sel.data_ptr<int32_t>(); p.logits = logits.data_ptr<float>(); p.lossv = lossv.data_ptr<float>();
+    p.dlogit = dlogit.data_ptr<float>();
+    check_cuda_err("SealArena setup");
+  }
+
+  // links int64 [2, B] on the arena's device; caps: one entry per hop (<= 0: full rows), each <= cap_max.
+  void extract(const GraphHandle& g, const Tensor& links, int64_t num_nodes, int64_t hops, std::vector<int64_t> caps,
+               int64_t seed, const Tensor& step, int64_t max_z, Tensor truncated) {
+    c10::cuda::CUDAGuard guard(device);
+    TORCH_CHECK(g.tbl.num_parts > 0 && g.device == device, "SealArena.extract: graph must be a device graph on the arena's device");
+    TORCH_CHECK(on_dev(links) && links.scalar_type() == torch::kInt64 && links.is_contiguous() && links.dim() == 2 &&
+                links.size(0) == 2 && links.size(1) == ptrs.B,
+                "SealArena.extract: links must be contiguous int64 [2, batch_size] on the arena's device");
+    TORCH_CHECK(num_nodes >= 1, "SealArena.extract: num_nodes must be >= 1");
+    TORCH_CHECK(hops >= 1 && hops <= kSealMaxHops, fmt("SealArena.extract: num_hops must be in [1, %d]", kSealMaxHops));
+    TORCH_CHECK(static_cast<int64_t>(caps.size()) == hops, "SealArena.extract: caps needs one entry per hop");
+    check_counters(step, 0, "SealArena.extract: step must be int32 [>= 1] on the device");
+    check_counters(truncated, 0, "SealArena.extract: truncated must be int32 [>= 1] on the device");
+    TORCH_CHECK(max_z < (1LL << 30), "SealArena.extract: max_z must be < 2^30");
+    SealExtractArgs e{};
+    e.g = g.tbl;
+    e.links = links.data_ptr<int64_t>();
+    e.num_nodes = num_nodes;
+    e.hops = static_cast<int>(hops);
+    e.cap_max = cap_max;
+    for (int h = 0; h < hops; ++h) {
+      TORCH_CHECK(caps[h] <= cap_max, "SealArena.extract: a neighbour cap exceeds the arena's cap_max");
+      e.caps[h] = static_cast<int>(std::max<int64_t>(caps[h], 0));
+    }
+    e.seed = static_cast<uint64_t>(seed);
+    e.step = step.data_ptr<int32_t>();
+    e.max_z = static_cast<int>(max_z);
+    e.samp = samp.data_ptr<int32_t>();
+    e.truncated = truncated.data_ptr<int32_t>();
+    launch_seal_extract(e, ptrs, cur_stream());
+    check_cuda_err("SealArena.extract");
+  }
+
+  void check_params(const Tensor& params, const char* msg) const { check_vec(params, torch::kFloat32, model.P, msg); }
+
+  // labels fp32 [B]; training = 0: no dropout
+  void forward(const Tensor& params, const Tensor& labels, bool training, double p, int64_t seed, const Tensor& step) {
+    c10::cuda::CUDAGuard guard(device);
+    check_params(params, "SealArena.forward: params must be contiguous fp32 [num_params] on the arena's device");
+    check_vec(labels, torch::kFloat32, ptrs.B, "SealArena.forward: labels must be contiguous fp32 [batch_size] on the device");
+    TORCH_CHECK(p >= 0.0 && p < 1.0, "SealArena.forward: dropout must be in [0, 1)");
+    check_counters(step, 0, "SealArena.forward: step must be int32 [>= 1] on the device");
+    launch_seal_forward(model, ptrs, params.data_ptr<float>(), labels.data_ptr<float>(), training ? 1 : 0,
+                        static_cast<float>(p), static_cast<uint64_t>(seed), step.data_ptr<int32_t>(), cur_stream());
+    check_cuda_err("SealArena.forward");
+  }
+
+  void backward(const Tensor& params) {
+    c10::cuda::CUDAGuard guard(device);
+    check_params(params, "SealArena.backward: params must be contiguous fp32 [num_params] on the arena's device");
+    launch_seal_backward(model, ptrs, params.data_ptr<float>(), partials.data_ptr<float>(), cur_stream());
+    check_cuda_err("SealArena.backward");
+  }
+
+  void reduce(Tensor grad, Tensor loss) {
+    c10::cuda::CUDAGuard guard(device);
+    check_params(grad, "SealArena.reduce: grad must be contiguous fp32 [num_params] on the arena's device");
+    check_vec(loss, torch::kFloat32, 1, "SealArena.reduce: loss must be fp32 [1] on the arena's device");
+    launch_seal_reduce(model, ptrs, partials.data_ptr<float>(), grad.data_ptr<float>(), loss.data_ptr<float>(),
+                       cur_stream());
+    check_cuda_err("SealArena.reduce");
+  }
+};
+
 static void dropout_bf16(Tensor Z, const Tensor& counters, int64_t n_hops, double p, int64_t seed, int64_t layer,
                          const c10::optional<Tensor>& step_dev) {
   c10::cuda::CUDAGuard guard(Z.device());
@@ -2432,6 +2587,27 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
            py::arg("graphs"), py::arg("slot_off"), py::arg("slot_n"), py::keep_alive<1, 3>())
       .def_readonly("R", &MetaPath::R)
       .def_readonly("rows", &MetaPath::rows);
+  py::class_<SealArena>(m, "SealArena")
+      .def(py::init<int, int64_t, int64_t, int64_t, int64_t, int64_t, int64_t, int64_t, int64_t>(), py::arg("device"),
+           py::arg("batch_size"), py::arg("max_nodes"), py::arg("max_edges"), py::arg("hidden"), py::arg("num_layers"),
+           py::arg("num_labels"), py::arg("k"), py::arg("cap_max") = 0)
+      .def("extract", &SealArena::extract, py::arg("graph"), py::arg("links"), py::arg("num_nodes"), py::arg("hops"),
+           py::arg("caps"), py::arg("seed"), py::arg("step"), py::arg("max_z"), py::arg("truncated"))
+      .def("forward", &SealArena::forward, py::arg("params"), py::arg("labels"), py::arg("training"), py::arg("p"),
+           py::arg("seed"), py::arg("step"))
+      .def("backward", &SealArena::backward, py::arg("params"))
+      .def("reduce", &SealArena::reduce, py::arg("grad"), py::arg("loss"))
+      .def_property_readonly("num_params", [](const SealArena& a) { return a.model.P; })
+      .def_property_readonly("dense", [](const SealArena& a) { return a.model.dense; })
+      .def_readonly("layout", &SealArena::layout)
+      .def_readonly("nodes", &SealArena::nodes).def_readonly("z", &SealArena::z)
+      .def_readonly("meta", &SealArena::meta).def_readonly("sptr", &SealArena::sptr)
+      .def_readonly("scol", &SealArena::scol).def_readonly("dptr", &SealArena::dptr)
+      .def_readonly("dcol", &SealArena::dcol).def_readonly("X", &SealArena::X)
+      .def_readonly("C1", &SealArena::C1).def_readonly("flat", &SealArena::flat)
+      .def_readonly("H1", &SealArena::H1).def_readonly("mask", &SealArena::mask)
+      .def_readonly("sel", &SealArena::sel).def_readonly("logits", &SealArena::logits)
+      .def_readonly("lossv", &SealArena::lossv).def_readonly("partials", &SealArena::partials);
   m.def("metapath_walk", &metapath_walk, py::arg("metapath"), py::arg("starts"), py::arg("walks_per_node"),
         py::arg("context_size"), py::arg("seed"), py::arg("step"), py::arg("walks"), py::arg("n_valid"));
   m.def("node2vec_walk", &node2vec_walk, py::arg("metapath"), py::arg("starts"), py::arg("walks_per_node"),

@@ -361,6 +361,61 @@ void launch_sgns_loss_grad(const int64_t* walks, const int64_t* neg, int n_walks
 void launch_sparse_adam(float* w, float* grad, float* m, float* v, uint8_t* touched, int64_t rows, int D,
                         const int32_t* t_dev, float lr, float b1, float b2, float eps, cudaStream_t s);
 
+// ---- seal.cu (SEAL link prediction: per-link enclosing subgraph, DRNL and DGCNN, CTA per link) ------------------------
+constexpr int kSealMaxHops = 4;
+constexpr int kSealMaxLayers = 8;    // GCNConv(hidden) layers; one GCNConv(1) follows them
+constexpr int kSealMaxNodes = 1024;  // per-link node capacity (local ids fit int16)
+constexpr int kSealMeta = 5;         // per link: [nodes, edges kept, valid, truncated, edges before truncation]
+
+// Per-link arena, [B, ...] with per-link strides max_nodes / max_edges.  CSRs are local: sptr / scol by source,
+// dptr / dcol by destination, both with the target pair removed.  X holds the concatenated tanh outputs of the GCN
+// layers ([max_nodes, total]), XW a [max_nodes, hidden] scratch, G the gradient of X.  C1 is ReLU(conv1) [16, k],
+// flat ReLU(conv2) [dense], H1 ReLU(lin1) [128] before dropout, mask the dropout scale [128], sel the sort-pool
+// rows [k] (-1 = zero padding).
+struct SealArenaPtrs {
+  int B, max_nodes, max_edges;
+  int64_t* nodes; int32_t* z; int32_t* meta;
+  int32_t* sptr; int16_t* scol; int32_t* dptr; int16_t* dcol;
+  float* X; float* XW; float* G; float* C1; float* flat; float* H1; float* mask; int32_t* sel;
+  float* logits; float* lossv; float* dlogit;
+};
+
+// Offsets of the DGCNN's tensors in the flat fp32 parameter vector.  GCN layer l < L is [hidden, in] (in = Z for
+// l = 0, hidden after), layer L is [1, hidden]; total = hidden * L + 1, dense = (k / 2 - 4) * 32.
+struct SealModel {
+  int H, L, Z, total, k, dense;
+  int64_t w[kSealMaxLayers + 1], bias[kSealMaxLayers + 1];
+  int64_t c1w, c1b, c2w, c2b, l1w, l1b, l2w, l2b, P;
+};
+
+struct SealExtractArgs {
+  GraphTable g;
+  const int64_t* links;        // [2, B]
+  int64_t num_nodes;
+  int hops, cap_max;           // cap_max = max(caps) (0: every hop takes full rows)
+  int caps[kSealMaxHops];      // caps[h] <= 0: full rows at hop h
+  uint64_t seed;
+  const int32_t* step;         // Philox step key of the neighbour draws
+  int max_z;                   // < 0: no clamp
+  int32_t* samp;               // [B, max_nodes, cap_max] scratch of the drawn row positions (cap_max > 0)
+  int32_t* truncated;          // += links that hit a capacity
+};
+
+size_t seal_extract_smem(int max_nodes);
+size_t seal_forward_smem(const SealModel& m, int max_nodes);
+size_t seal_backward_smem(const SealModel& m, int max_nodes);
+// Enclosing subgraphs, local CSRs and DRNL labels of the B links (CTA per link).
+void launch_seal_extract(const SealExtractArgs& e, const SealArenaPtrs& a, cudaStream_t s);
+// GCN stack, sort-pool, convs, MLP and BCE (CTA per link).  Loss terms and dlogit are divided by the batch's valid
+// links; training = 0 uses no dropout (mask = 1).
+void launch_seal_forward(const SealModel& m, const SealArenaPtrs& a, const float* prm, const float* labels,
+                         int training, float p_drop, uint64_t seed, const int32_t* step, cudaStream_t s);
+// Gradient of the link's loss term into partials[b, :P] (CTA per link; invalid links write nothing).
+void launch_seal_backward(const SealModel& m, const SealArenaPtrs& a, const float* prm, float* partials, cudaStream_t s);
+// grad[i] = sum over valid links b, in order, of partials[b, i]; *loss = sum of the valid links' loss terms.
+void launch_seal_reduce(const SealModel& m, const SealArenaPtrs& a, const float* partials, float* grad, float* loss,
+                        cudaStream_t s);
+
 // ---- gat.cu (relational GAT engine kernels; H = heads * C, H a multiple of 64 in [64, 1024], C % 8 == 0) -----------
 // Per-node attention scores of two row sets: out[set][row * heads + h] = <att[set][h], P[set][row, h*C : (h+1)*C]>
 // for row < min(cum[set][idx[set]], cap[set]).  P[1] == nullptr skips the second set.  zero (optional, fp32

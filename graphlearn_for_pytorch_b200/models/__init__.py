@@ -8,3 +8,4 @@ from .hetero_engine import HeteroSageEngine
 from .hetero_gat_engine import HeteroGatEngine
 from .hetero_hgt_engine import HeteroHgtEngine
 from .metapath2vec import MetaPath2VecEngine
+from .seal_engine import SealEngine
