@@ -39,6 +39,12 @@ class SealEngine:
     max_z: the largest DRNL label (input features are one_hot(z, max_z + 1)); None takes the largest label seen on the
       calibration links.  Labels above it are clamped.
     dropout: dropout probability after the MLP's first layer, in [0, 1).
+    Shared memory bounds hidden and sort_k further: the per-link kernels hold a [hidden, hidden] weight stage, per-node
+    vectors of max_nodes and sort-pool / conv buffers of about 49 * sort_k floats in one CTA, and construction raises
+    ValueError when that exceeds the device's opt-in limit per block.  On an H100 (232,448 bytes), computed from the
+    kernels' formula (seal_smem in seal.cu): hidden <= 238 at max_nodes=256 and <= 235 at max_nodes=1024 (sort_k 10);
+    with num_layers <= 4, sort_k <= 1,123 at hidden 32 and <= 841 at hidden 128 (max_nodes=256), <= 1,091 and <= 809
+    at max_nodes=1024.
     batch_size: links per step; fewer are padded.  lr: Adam learning rate (betas 0.9 / 0.999, eps 1e-8).
     calibration_links: int64 [2, n] links (typically the training links); needed when max_edges, max_z or a
       percentile sort_k must be calibrated.  This is the construction's only host read.
@@ -79,13 +85,13 @@ class SealEngine:
     if max_edges is not None and not 1 <= int(max_edges) <= 2 ** 24:
       raise ValueError(f'max_edges must be in [1, 2^24] (got {max_edges})')
     if not 1 <= int(hidden) <= 256:
-      raise ValueError(f'hidden must be in [1, 256] (got {hidden})')
+      raise ValueError(f'hidden must be in [1, 256], and shared memory bounds it further (got {hidden})')
     if not 1 <= int(num_layers) <= 8:
       raise ValueError(f'num_layers must be in [1, 8] (got {num_layers})')
     if isinstance(sort_k, bool) or not isinstance(sort_k, (int, float)):
       raise ValueError(f'sort_k must be an int >= 10 or a float in (0, 1) (got {sort_k!r})')
     if isinstance(sort_k, int) and not 10 <= sort_k <= 2048:
-      raise ValueError(f'an int sort_k must be in [10, 2048] (got {sort_k})')
+      raise ValueError(f'an int sort_k must be in [10, 2048], and shared memory bounds it further (got {sort_k})')
     if isinstance(sort_k, float) and not 0.0 < sort_k < 1.0:
       raise ValueError(f'a float sort_k must be in (0, 1) (got {sort_k})')
     if max_z is not None and not 1 <= int(max_z) < 2 ** 20:

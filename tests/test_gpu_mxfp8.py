@@ -406,12 +406,15 @@ def test_hetero_inference_on_mxfp8_matches_the_twin_and_is_chunk_invariant(nativ
 
 @pytest.mark.parametrize('kind', list(ENGINES))
 def test_hetero_engine_learns_on_mxfp8_like_on_bf16(native, hetero, kind):
+  # Two runs differ by the arrival order of fp32 atomics.  At lr 5e-3 HGT's loss climbs back above ln(8) before it
+  # falls, and when it recovers varies from run to run: on an H100, four bf16 runs ended at 0.31 to 0.78 accuracy.
+  # At 5e-4 over 800 steps, six runs of each format ended at 0.88 to 0.94.
   accs = {}
   for name, mx in (('mxfp8', True), ('bf16', False)):
-    eng = hetero.engine(kind, mx, use_graph=True, fan=(4, 3, 2), lr=5e-3 if kind == 'hgt' else 1e-2)
+    eng = hetero.engine(kind, mx, use_graph=True, fan=(4, 3, 2), lr=5e-4 if kind == 'hgt' else 1e-2)
     eng.warmup_and_capture(n_eager=1)
     g = torch.Generator().manual_seed(0)
-    for _ in range(400 if kind == 'hgt' else 200):
+    for _ in range(800 if kind == 'hgt' else 200):
       eng.train_step(torch.randperm(SIZES['paper'], generator=g)[:128].to(DEV))
     correct = total = 0
     for i in range(8):
