@@ -2442,7 +2442,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   // ---- CPU ops ----
   m.def("coo_to_csr", &coo_to_csr);
   m.def("cpu_sample_neighbors", &cpu_sample_neighbors);
-  m.def("cpu_sample_neighbors_weighted", &cpu_sample_neighbors_weighted);
+  m.def("cpu_sample_neighbors_weighted", &cpu_sample_neighbors_weighted, py::arg("indptr"), py::arg("indices"),
+        py::arg("eids"), py::arg("weights"), py::arg("seeds"), py::arg("k"), py::arg("with_edge"), py::arg("seed"),
+        py::arg("stream"), py::arg("replace") = false);
   m.def("cpu_negative_sample", &cpu_negative_sample);
   m.def("cpu_node_subgraph", &cpu_node_subgraph);
   m.def("cpu_random_walk", &cpu_random_walk);

@@ -294,17 +294,33 @@ std::tuple<Tensor, Tensor, Tensor> cpu_sample_neighbors(
 }
 
 // ----------------------------------------------------------------------------
-// Weighted sampling without replacement: exponential race
-// (Efraimidis-Spirakis): key_j = -log(u_j)/w_j, keep the k smallest keys.
-// The reference's CPU path samples with replacement from
-// std::discrete_distribution (weighted_sampler.cc:147-165) and has no GPU
-// implementation at all (weighted_sampler.cuh:28-36); this formulation has
-// the same marginal behaviour for k=1 and runs identically on the GPU.
+// Weighted neighbour sampling; a row of degree d <= k (or k < 0) is copied whole.
+//   replace=false: a weighted k-subset by exponential race (Efraimidis-Spirakis):
+//     key_j = -log(u_j)/w_j, keep the k smallest keys.  Zero-weight neighbours
+//     come last, in position order, when fewer than k weights are positive.
+//   replace=true: k independent draws, neighbour j with probability w_j / W
+//     (the reference's std::discrete_distribution, weighted_sampler.cc:147-165).
+//     Draw i inverts the row's CDF at u_i * W with u_i from Philox counter i;
+//     a row whose weights are all 0 picks nothing (count 0).
+// The reference has no GPU implementation (weighted_sampler.cuh:28-36); both
+// formulations run on the GPU as well (cuda/sampling.cu pick_positions).
 // ----------------------------------------------------------------------------
+// Running sums of a row's weights in position order (fp64, as on the GPU); returns the row's total.
+static inline double weight_prefix(const float* w, int64_t d, std::vector<double>& cdf) {
+  cdf.resize(d);
+  double s = 0.0;
+  for (int64_t j = 0; j < d; ++j) cdf[j] = (s += w[j]);
+  return s;
+}
+
+static inline bool any_positive(const float* w, int64_t d) {
+  return std::any_of(w, w + d, [](float x) { return x > 0.f; });
+}
+
 std::tuple<Tensor, Tensor, Tensor> cpu_sample_neighbors_weighted(
     const Tensor& indptr, const Tensor& indices, const c10::optional<Tensor>& eids,
     const Tensor& weights, const Tensor& seeds, int64_t k, bool with_edge,
-    int64_t seed, int64_t stream) {
+    int64_t seed, int64_t stream, bool replace) {
   check_i64(indptr, "indptr");
   check_i64(indices, "indices");
   check_i64(seeds, "seeds");
@@ -326,8 +342,10 @@ std::tuple<Tensor, Tensor, Tensor> cpu_sample_neighbors_weighted(
   std::vector<int64_t> offs(bs + 1, 0);
   glt::parallel_for(0, bs, 16384, [&](int64_t b, int64_t e) {
     for (int64_t i = b; i < e; ++i) {
-      int64_t d = row_degree(ip, num_rows, sd[i]);
+      const int64_t v = sd[i];
+      const int64_t d = row_degree(ip, num_rows, v);
       cnt[i] = (k < 0) ? d : std::min(d, k);
+      if (replace && k >= 0 && d > k && !any_positive(w + ip[v], d)) cnt[i] = 0;
     }
   });
   for (int64_t i = 0; i < bs; ++i) offs[i + 1] = offs[i] + cnt[i];
@@ -337,15 +355,30 @@ std::tuple<Tensor, Tensor, Tensor> cpu_sample_neighbors_weighted(
   int64_t* oe = with_edge ? out_e.data_ptr<int64_t>() : nullptr;
   glt::parallel_for(0, bs, 256, [&](int64_t b, int64_t e) {
     std::vector<std::pair<float, int64_t>> keys;
+    std::vector<double> cdf;
     for (int64_t i = b; i < e; ++i) {
       const int64_t v = sd[i];
       const int64_t d = row_degree(ip, num_rows, v);
-      if (d == 0) continue;
+      if (d == 0 || cnt[i] == 0) continue;
       const int64_t start = ip[v];
       int64_t* o = nb + offs[i];
       if (k < 0 || d <= k) {
         std::memcpy(o, ind + start, sizeof(int64_t) * d);
         if (oe) std::memcpy(oe + offs[i], ei + start, sizeof(int64_t) * d);
+        continue;
+      }
+      if (replace) {
+        const double total = weight_prefix(w + start, d, cdf);
+        int64_t last = d - 1;
+        while (!(w[start + last] > 0.f)) --last;   // cnt > 0: some weight is positive
+        for (int64_t j = 0; j < k; ++j) {
+          const double target = static_cast<double>(u01(philox_draw(seed, stream, v, (uint32_t)j))) * total;
+          // first running sum above the target (sums are non-decreasing, so it sits on a positive weight)
+          int64_t t = std::upper_bound(cdf.begin(), cdf.end(), target) - cdf.begin();
+          if (t > last) t = last;
+          o[j] = ind[start + t];
+          if (oe) oe[offs[i] + j] = ei[start + t];
+        }
         continue;
       }
       keys.resize(d);

@@ -20,7 +20,7 @@ std::tuple<Tensor, Tensor, Tensor> cpu_sample_neighbors(
 std::tuple<Tensor, Tensor, Tensor> cpu_sample_neighbors_weighted(
     const Tensor& indptr, const Tensor& indices, const c10::optional<Tensor>& eids,
     const Tensor& weights, const Tensor& seeds, int64_t k, bool with_edge, int64_t seed,
-    int64_t stream);
+    int64_t stream, bool replace);
 
 class CpuIdTable {
  public:

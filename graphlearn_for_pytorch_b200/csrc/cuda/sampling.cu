@@ -25,6 +25,37 @@ namespace {
 
 constexpr uint32_t kNoPick = 0xFFFFFFFFu;
 
+// Inverse CDF of a row's weights, scanned G consecutive weights at a time with the running sum carried: `pick` is
+// the first position of positive weight whose running sum exceeds `target`, or kNoPick.  Without a pick, `total` is
+// the row's sum and `last` its last position of positive weight (kNoPick if none).  Every lane of the group returns
+// the same.  The sums are fp64: in fp32 one ulp of the running sum of a wide row outgrows its small weights (at 1e5
+// weights alternating 1 and 1000 the ulp is 4), which would skew their probabilities.
+struct CdfScan { double total; uint32_t pick, last; };
+
+template <int G>
+__device__ __forceinline__ CdfScan weight_cdf_find(const float* w, uint32_t d, int gl, unsigned gmask, double target) {
+  const int lane0 = (threadIdx.x & 31) - gl;
+  double carry = 0.0;
+  uint32_t last = kNoPick;
+  for (uint32_t base = 0; base < d; base += G) {
+    const uint32_t e = base + gl;
+    const float we = e < d ? __ldg(w + e) : 0.f;
+    double x = we;
+#pragma unroll
+    for (int off = 1; off < G; off <<= 1) {
+      const double y = __shfl_up_sync(gmask, x, off, G);
+      if (gl >= off) x += y;
+    }
+    const bool pos = we > 0.f;
+    const unsigned hit = (__ballot_sync(gmask, pos && carry + x > target) & gmask) >> lane0;
+    if (hit) return CdfScan{0.0, base + (__ffs(hit) - 1), last};
+    const unsigned any = (__ballot_sync(gmask, pos) & gmask) >> lane0;
+    if (any) last = base + (31 - __clz(any));
+    carry += __shfl_sync(gmask, x, G - 1, G);
+  }
+  return CdfScan{carry, kNoPick, last};
+}
+
 template <int G, int MAXC>
 __device__ __forceinline__ void pick_positions(const GraphTable& g, const RowRef& row, int64_t v,
                                                int k, int gl, unsigned gmask, int weighted,
@@ -44,12 +75,30 @@ __device__ __forceinline__ void pick_positions(const GraphTable& g, const RowRef
     }
     return;
   }
-  if (replace) {
+  if (replace && !weighted) {
 #pragma unroll
     for (int c = 0; c < MAXC; ++c) {
       uint32_t j = c * G + gl;
       if (j < uk) picks[c] = bounded(philox_draw(seed, stream, v, j), d);
     }
+    take = static_cast<int>(uk);
+    return;
+  }
+  if (replace) {
+    // weighted with replacement: k independent draws, position e with probability w[e] / W.  Draw i inverts the
+    // row's CDF at u_i * W, u_i from counter i as in the uniform draws above.  A row of zero weights picks nothing.
+    const float* w = g.parts[row.part].weights + row.start;
+    const CdfScan row_sum = weight_cdf_find<G>(w, d, gl, gmask, __longlong_as_double(0x7ff0000000000000ll));
+    if (row_sum.last == kNoPick) { take = 0; return; }
+    for (uint32_t i = 0; i < uk; ++i) {
+      const double target = static_cast<double>(u01(philox_draw(seed, stream, v, i))) * row_sum.total;
+      uint32_t pick = weight_cdf_find<G>(w, d, gl, gmask, target).pick;
+      if (pick == kNoPick) pick = row_sum.last;   // u * W rounded up past the scan's own running sums
+#pragma unroll
+      for (int c = 0; c < MAXC; ++c)
+        if (i == static_cast<uint32_t>(c * G + gl)) picks[c] = pick;
+    }
+    take = static_cast<int>(uk);
     return;
   }
   if (!weighted) {
@@ -127,7 +176,6 @@ __device__ __forceinline__ void sample_hop_body(const HopArgs& a) {
     int take = 0;
     pick_positions<G, MAXC>(a.g, row, v, a.k, gl, gmask, a.weighted, a.replace, a.seed, rng_stream,
                             picks, take);
-    if (a.replace && row.deg > a.k) take = a.k;
 #pragma unroll
     for (int c = 0; c < MAXC; ++c) {
       const int j = c * G + gl;
@@ -394,7 +442,6 @@ __global__ void __launch_bounds__(256) k_sample_one_hop(GraphTable g, const int6
     uint32_t picks[MAXC];
     int take = 0;
     pick_positions<G, MAXC>(g, row, v, k, gl, gmask, weighted, replace, seed, stream, picks, take);
-    if (replace && row.deg > k) take = k;
 #pragma unroll
     for (int c = 0; c < MAXC; ++c) {
       const int j = c * G + gl;

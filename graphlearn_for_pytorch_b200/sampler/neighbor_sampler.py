@@ -46,11 +46,21 @@ class NeighborSampler(BaseSampler):
     device: sampling device (defaults to the graph's placement).
     with_edge: also return global edge ids.
     with_neg: create negative samplers for link sampling.
-    with_weight: weighted (edge-weight proportional) neighbour sampling.
+    with_weight: draw neighbours in proportion to the edge weights instead of uniformly.
     strategy: 'random' (only strategy, as in the reference).
     edge_dir: 'out' samples out-neighbours from CSR, 'in' samples in-neighbours from CSC.
     seed: Philox seed; together with the internal batch counter it determines every draw.
-    replace: sample with replacement (reference CPU behaviour) instead of without.
+    replace: sample with replacement (the reference's CPU behaviour) instead of without.
+
+  What a row of degree d > k draws, on CPU and GPU alike (a row with d <= k returns all its neighbours):
+    uniform, no replacement    a uniform k-subset (Floyd);
+    uniform, replacement       k independent uniform draws;
+    weighted, no replacement   a weighted k-subset: successive draws in proportion to the weights of the neighbours
+                               not yet drawn (exponential race); zero-weight neighbours only fill the places that
+                               positive weights cannot, in position order;
+    weighted, replacement      k independent draws, each neighbour with probability w / sum(w); a row whose weights
+                               are all 0 returns no neighbours.
+  Without replacement the picks of a row are a set: their order within the row is not random.
   """
 
   def __init__(self, graph: Union[Graph, Dict[EdgeType, Graph]], num_neighbors: Optional[NumNeighbors] = None,
@@ -190,7 +200,7 @@ class NeighborSampler(BaseSampler):
       if self.with_weight and topo.edge_weights is not None and req_num >= 0:
         nbr, num, eid = self._nat.cpu_sample_neighbors_weighted(
           topo.indptr, topo.indices, topo.edge_ids, topo.edge_weights, seeds, int(req_num),
-          self.with_edge, self.seed, stream)
+          self.with_edge, self.seed, stream, self.replace)
       else:
         nbr, num, eid = self._nat.cpu_sample_neighbors(
           topo.indptr, topo.indices, topo.edge_ids, seeds, int(req_num), self.with_edge,
