@@ -14,7 +14,7 @@ Arms:
           under bf16 autocast with torch.optim.Adam
 
 ms_per_step is device-timed (CUDA events around --steps steps), the median over --rounds rounds.  Launches per step:
-the engine's exact tally; for the eager arm, the CUDA kernels (and memcpy / memset operations) torch.profiler records
+the kernel, memset and memcpy nodes of the engine's captured step; for the eager arm, the CUDA kernels (and memcpy / memset operations) torch.profiler records
 over --steps steps, divided by --steps.  `--profile` prints the engine's per-kernel device times to stderr.  The card
 name and power limit are read in the same run.  One JSON line is printed.
 """

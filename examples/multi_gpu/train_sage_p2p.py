@@ -1,5 +1,5 @@
 """Multi-GPU GraphSAGE on one NVSwitch box: graph + features range-partitioned over the GPUs,
-sampling and layer-1 gather read peer HBM in-kernel, gradients all-reduced with NCCL.
+sampling and layer-1 gather read peer HBM in-kernel, gradients all-reduced over NVLink inside the Adam kernel.
 
 Counterpart of the reference's examples/multi_gpu/train_sage_ogbn_papers100m.py (which shares one
 Dataset over spawned processes by IPC and shards a 15%-hot feature cache over NVLink groups).

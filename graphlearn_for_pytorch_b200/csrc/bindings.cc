@@ -1091,9 +1091,8 @@ static void sage_gather_bwd(const Tensor& dA, int64_t d, SamplerArena& ar, int64
   check_cuda_err("sage_gather_bwd");
 }
 
-// Returns the number of kernels launched (2 when the bias gradient takes a separate column-sum pass).
-static int64_t relu_bwd_cast(const Tensor& dH, const Tensor& Z, const Tensor& counters, int64_t n_hops,
-                             Tensor dPre, const c10::optional<Tensor>& colsum, bool prezeroed, double gscale, bool relu) {
+static void relu_bwd_cast(const Tensor& dH, const Tensor& Z, const Tensor& counters, int64_t n_hops,
+                          Tensor dPre, const c10::optional<Tensor>& colsum, bool prezeroed, double gscale, bool relu) {
   c10::cuda::CUDAGuard guard(dH.device());
   const int64_t d = dPre.dim() == 2 ? dPre.size(1) : 0;
   TORCH_CHECK(d % 8 == 0, "relu_bwd_cast: width must be a multiple of 8");
@@ -1103,11 +1102,9 @@ static int64_t relu_bwd_cast(const Tensor& dH, const Tensor& Z, const Tensor& co
   TORCH_CHECK(dPre.size(0) <= dH.size(0) && dPre.size(0) <= Z.size(0), "relu_bwd_cast: dH / Z have fewer rows than dPre");
   check_counters(counters, n_hops, "relu_bwd_cast: counters must be int32 [> n_hops] on the device");
   if (has(colsum)) check_vec(*colsum, torch::kFloat32, d, "relu_bwd_cast: colsum must be fp32 [d]");
-  const int n = launch_relu_bwd_cast(dH.data_ptr<float>(), Z.data_ptr(), counters.data_ptr<int32_t>(), n_hops,
-                                     dPre.size(0), d, dPre.data_ptr(), opt_ptr<float>(colsum), cur_stream(),
-                                     prezeroed, static_cast<float>(gscale), relu);
+  launch_relu_bwd_cast(dH.data_ptr<float>(), Z.data_ptr(), counters.data_ptr<int32_t>(), n_hops, dPre.size(0), d,
+                       dPre.data_ptr(), opt_ptr<float>(colsum), cur_stream(), prezeroed, static_cast<float>(gscale), relu);
   check_cuda_err("relu_bwd_cast");
-  return n;
 }
 
 // ---- relational GAT (cuda/gat.cu) -------------------------------------------------------------------------------
@@ -2036,8 +2033,7 @@ static void dropout_bf16(Tensor Z, const Tensor& counters, int64_t n_hops, doubl
   check_cuda_err("dropout_bf16");
 }
 
-// Returns the number of kernels launched (2 when the bias gradient takes a separate column-sum pass).
-static int64_t softmax_nll(const Tensor& logits, int64_t C, const c10::optional<Tensor>& y,
+static void softmax_nll(const Tensor& logits, int64_t C, const c10::optional<Tensor>& y,
                         const c10::optional<Tensor>& labels_all, const c10::optional<Tensor>& nodes,
                         const Tensor& counters, Tensor loss, Tensor dlogits,
                         const c10::optional<Tensor>& correct, const c10::optional<Tensor>& colsum, bool prezeroed) {
@@ -2060,14 +2056,31 @@ static int64_t softmax_nll(const Tensor& logits, int64_t C, const c10::optional<
               "softmax_nll: loss must be fp32 [>= 1] on the device");
   if (has(correct)) check_counters(*correct, 0, "softmax_nll: correct must be int32 [>= 1] on the device");
   if (has(colsum)) check_vec(*colsum, torch::kFloat32, logits.size(1), "softmax_nll: colsum must be fp32 [ld]");
-  const int n = launch_softmax_nll(logits.data_ptr(), logits.size(1), C, direct ? y->data_ptr<int64_t>() : nullptr,
-                                   direct ? nullptr : labels_all->data_ptr<int64_t>(),
-                                   direct ? nullptr : nodes->data_ptr<int64_t>(),
-                                   counters.data_ptr<int32_t>(), logits.size(0), loss.data_ptr<float>(),
-                                   dlogits.data_ptr(), opt_ptr<int32_t>(correct), opt_ptr<float>(colsum), cur_stream(),
-                                   prezeroed);
+  launch_softmax_nll(logits.data_ptr(), logits.size(1), C, direct ? y->data_ptr<int64_t>() : nullptr,
+                     direct ? nullptr : labels_all->data_ptr<int64_t>(), direct ? nullptr : nodes->data_ptr<int64_t>(),
+                     counters.data_ptr<int32_t>(), logits.size(0), loss.data_ptr<float>(), dlogits.data_ptr(),
+                     opt_ptr<int32_t>(correct), opt_ptr<float>(colsum), cur_stream(), prezeroed);
   check_cuda_err("softmax_nll");
-  return n;
+}
+
+// (kernel, memset, memcpy) node counts of a captured CUDA graph: the launches one replay makes.  `raw_graph` is the
+// cudaGraph_t of torch.cuda.CUDAGraph(keep_graph=True).raw_cuda_graph().
+static std::tuple<int64_t, int64_t, int64_t> graph_node_counts(int64_t raw_graph) {
+  TORCH_CHECK(raw_graph != 0, "graph_node_counts: null graph (capture with keep_graph=True)");
+  cudaGraph_t graph = reinterpret_cast<cudaGraph_t>(static_cast<uintptr_t>(raw_graph));
+  size_t n = 0;
+  C10_CUDA_CHECK(cudaGraphGetNodes(graph, nullptr, &n));
+  std::vector<cudaGraphNode_t> nodes(n);
+  if (n > 0) C10_CUDA_CHECK(cudaGraphGetNodes(graph, nodes.data(), &n));
+  int64_t kernels = 0, memsets = 0, memcpys = 0;
+  for (cudaGraphNode_t node : nodes) {
+    cudaGraphNodeType type;
+    C10_CUDA_CHECK(cudaGraphNodeGetType(node, &type));
+    kernels += type == cudaGraphNodeTypeKernel;
+    memsets += type == cudaGraphNodeTypeMemset;
+    memcpys += type == cudaGraphNodeTypeMemcpy;
+  }
+  return {kernels, memsets, memcpys};
 }
 
 static void zero_grads(Tensor g, const c10::optional<Tensor>& loss, const c10::optional<Tensor>& correct) {
@@ -2627,6 +2640,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("seed"), py::arg("layer"), py::arg("step_dev") = py::none());
   m.def("zero_grads", &zero_grads);
   m.def("set_pdl", [](bool on) { return set_pdl(on ? 1 : 0) != 0; });
+  m.def("graph_node_counts", &graph_node_counts, py::arg("raw_graph"));
   m.def("sage_gather_bwd", &sage_gather_bwd, py::arg("dA"), py::arg("d"), py::arg("arena"), py::arg("n_hops_targets"),
         py::arg("Z"), py::arg("dPre"), py::arg("colsum"), py::arg("prezeroed") = false, py::arg("gscale") = 1.0);
   m.def("gat_scores", &gat_scores, py::arg("P0"), py::arg("att0"), py::arg("out0"), py::arg("counters0"),

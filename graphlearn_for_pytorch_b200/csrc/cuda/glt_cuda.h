@@ -284,10 +284,10 @@ void launch_sage_gather_bwd(const SageGatherBwdArgs& a, cudaStream_t s);
 
 // dPre = (Z > 0) ? bf16(dH) : 0 for rows < cum[n_hops]; 0 beyond.  relu = false: dPre = bf16(dH), Z is not read.
 // colsum (optional, fp32 [d]): bias gradient = column sums of the bf16 dPre, any d (multiple of 8): fused into the
-// cast when d divides 2048, a second column-sum kernel otherwise.  Returns the number of kernels launched.
-int launch_relu_bwd_cast(const float* dH, const void* Z, const int32_t* cum, int n_hops, int cap,
-                         int d, void* dPre, float* colsum, cudaStream_t s, bool prezeroed = false,
-                         float gscale = 1.f, bool relu = true);
+// cast when d divides 2048, a second column-sum kernel otherwise.
+void launch_relu_bwd_cast(const float* dH, const void* Z, const int32_t* cum, int n_hops, int cap,
+                          int d, void* dPre, float* colsum, cudaStream_t s, bool prezeroed = false,
+                          float gscale = 1.f, bool relu = true);
 // In-place inverted dropout (keep prob 1-p, kept values scaled by 1/(1-p)) on rows < cum[n_hops] of bf16 Z[cap, d];
 // mask = Philox(seed, layer, *step_dev, element).  Backward: launch_relu_bwd_cast(..., gscale = 1/(1-p)) on the
 // post-dropout Z.
@@ -299,10 +299,10 @@ void launch_zero_grads(float* g, int64_t n, float* loss, int32_t* correct, cudaS
 // loss = mean NLL(log_softmax(logits[:n0, :C]), y); dlogits = (softmax - onehot)/n0
 // labels come from y[r], or (labels_all != nullptr) from labels_all[nodes[r]].
 // colsum (optional, fp32 [ld]): bias gradient = column sums of the bf16 dlogits, any ld (multiple of 8): fused into
-// the loss kernel for ld <= 256, a second column-sum kernel otherwise.  Returns the number of kernels launched.
-int launch_softmax_nll(const void* logits, int ld, int C, const int64_t* y, const int64_t* labels_all,
-                       const int64_t* nodes, const int32_t* cum, int cap, float* loss, void* dlogits,
-                       int32_t* correct, float* colsum, cudaStream_t s, bool prezeroed = false);
+// the loss kernel for ld <= 256, a second column-sum kernel otherwise.
+void launch_softmax_nll(const void* logits, int ld, int C, const int64_t* y, const int64_t* labels_all,
+                        const int64_t* nodes, const int32_t* cum, int cap, float* loss, void* dlogits,
+                        int32_t* correct, float* colsum, cudaStream_t s, bool prezeroed = false);
 // out[c] = sum over valid rows of X[:, c]  (d multiple of 8)
 void launch_colsum_bf16(const void* X, const int32_t* cum, int n_hops, int cap, int d, float* out,
                         cudaStream_t s);

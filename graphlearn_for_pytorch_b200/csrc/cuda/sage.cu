@@ -459,8 +459,8 @@ static void launch_colsum_accum(const void* X, const int32_t* cum, int n_hops, i
            reinterpret_cast<const __nv_bfloat16*>(X), cum, n_hops, cap, d, out);
 }
 
-int launch_relu_bwd_cast(const float* dH, const void* Z, const int32_t* cum, int n_hops, int cap,
-                         int d, void* dPre, float* colsum, cudaStream_t s, bool prezeroed, float gscale, bool relu) {
+void launch_relu_bwd_cast(const float* dH, const void* Z, const int32_t* cum, int n_hops, int cap,
+                          int d, void* dPre, float* colsum, cudaStream_t s, bool prezeroed, float gscale, bool relu) {
   // the fused column sum needs d | 2048 (a thread keeps its 8 columns across grid-stride iterations); other widths
   // sum the bf16 dPre in a second pass
   const bool fused = colsum && 2048 % d == 0;
@@ -468,14 +468,12 @@ int launch_relu_bwd_cast(const float* dH, const void* Z, const int32_t* cum, int
   launch_k(k_relu_bwd_cast, dim3(grid_for(static_cast<int64_t>(cap) * d / 8, 256 * 2, 132 * 4)), dim3(256), 0, s,
            dH, reinterpret_cast<const __nv_bfloat16*>(Z), cum, n_hops, cap, d,
            reinterpret_cast<__nv_bfloat16*>(dPre), fused ? colsum : nullptr, gscale, relu ? 1 : 0);
-  if (colsum == nullptr || fused) return 1;
-  launch_colsum_accum(dPre, cum, n_hops, cap, d, colsum, s);
-  return 2;
+  if (colsum && !fused) launch_colsum_accum(dPre, cum, n_hops, cap, d, colsum, s);
 }
 
-int launch_softmax_nll(const void* logits, int ld, int C, const int64_t* y, const int64_t* labels_all,
-                       const int64_t* nodes, const int32_t* cum, int cap, float* loss, void* dlogits,
-                       int32_t* correct, float* colsum, cudaStream_t s, bool prezeroed) {
+void launch_softmax_nll(const void* logits, int ld, int C, const int64_t* y, const int64_t* labels_all,
+                        const int64_t* nodes, const int32_t* cum, int cap, float* loss, void* dlogits,
+                        int32_t* correct, float* colsum, cudaStream_t s, bool prezeroed) {
   // the loss kernel sums the bias gradient in registers for ld <= 256; wider rows sum the bf16 dlogits in a second
   // pass over the n0 = cum[1] seed rows
   const bool fused = colsum && ld <= 256;
@@ -487,9 +485,7 @@ int launch_softmax_nll(const void* logits, int ld, int C, const int64_t* y, cons
   launch_k(k_softmax_nll, dim3(grid_for(cap, 8)), dim3(256), 0, s, reinterpret_cast<const __nv_bfloat16*>(logits), ld,
            C, y, labels_all, nodes, cum, cap, loss, reinterpret_cast<__nv_bfloat16*>(dlogits), correct,
            fused ? colsum : nullptr);
-  if (colsum == nullptr || fused) return 1;
-  launch_colsum_accum(dlogits, cum, 1, cap, ld, colsum, s);
-  return 2;
+  if (colsum && !fused) launch_colsum_accum(dlogits, cum, 1, cap, ld, colsum, s);
 }
 
 void launch_adam(float* p, const float* g, float* m, float* v, void* p_bf16, int64_t n, float lr,

@@ -318,17 +318,11 @@ class HeteroSageEngine(object):
     self.step_idx, self.seed = s['step_idx'], s['seed']
 
   # ------------------------------------------------------------------ step pieces
-  _tally = 0
-
-  def _k(self, n=1):
-    self._tally += n
-
   def _rel_ell(self, r: int, nh: int):
     return [self.arena.ell_of(r, h) for h in range(nh)], [max(self.fan[r][h], 1) for h in range(nh)]
 
   def _sample(self):
     self.arena.sample([self.tid[self.seed_type]], [self._seeds], self.L * len(self.edge_types))
-    self._k(3 + 3 * self.L)
 
   def _plan(self, kind: str, l: int, t: int):
     key = (kind, l, t)
@@ -376,7 +370,6 @@ class HeteroSageEngine(object):
     """Layer-1 input of the attention engines: the feature rows of every sampled node of type u into X0[u]."""
     n = min(self.X0[u].shape[0], self.cap_nodes[u])
     self._gather_feat(u, self.arena.nodes_of(u)[:n], self._ctr[u][self.L + 1:self.L + 2], self.X0[u][:n])
-    self._k()
 
   def _loss(self, logits: torch.Tensor, dlogits: torch.Tensor, bias_grad: torch.Tensor):
     """Forward tail: clear the gradients, then the fused log-softmax / NLL of the seed rows of `logits`, writing
@@ -384,10 +377,9 @@ class HeteroSageEngine(object):
     nat, st = self.nat, self.tid[self.seed_type]
     if self.peer_group is not None:
       self.peer_group.barrier(1)            # peers finished reading last step's gradients
-      self._k()
     nat.zero_grads(self.g32, self.loss, self.correct)
-    self._k(1 + nat.softmax_nll(logits, self.C, None, self.labels, self.arena.nodes_of(st), self._ctr[st], self.loss,
-                                dlogits, self.correct, bias_grad, True))
+    nat.softmax_nll(logits, self.C, None, self.labels, self.arena.nodes_of(st), self._ctr[st], self.loss, dlogits,
+                    self.correct, bias_grad, True)
 
   def _forward(self):
     nat, ar = self.nat, self.arena
@@ -406,7 +398,6 @@ class HeteroSageEngine(object):
           else:
             nat.sage_aggregate_block(None, None, self.Z[l - 1][s], d, self._ctr[t], nh, ell, ks, ar.deg_of(r), A,
                                      offs[j])
-          self._k()
         d = self._width_in(l, t)
         blk = A[:, self_col:self_col + d]
         if l == 1:
@@ -414,9 +405,7 @@ class HeteroSageEngine(object):
           self._gather_feat(t, ar.nodes_of(t)[:n], self._ctr[t][nh:nh + 1], blk)
         else:
           blk.copy_(self.Z[l - 1][t][:A.shape[0]])
-        self._k()
         self._plan('fwd', l, t).run()
-        self._k()
     st = self.tid[self.seed_type]
     self._loss(self.Z[self.L][st], self.dPre[self.L][st], self.param(('b', self.L, st), True))
 
@@ -426,36 +415,30 @@ class HeteroSageEngine(object):
       nh = self.L - l + 1
       for t in self.targets[l]:
         self._plan('bwd', l, t).run()
-        self._k()
       if l == 1:
         break
       H = self.hidden
       for s in self.targets[l - 1]:
         nat.zero_rows(self.dH[l - 1][s], self._ctr[s], nh + 1)
-        self._k()
       for t in self.targets[l]:
         offs, self_col = self.col[l][t]
         for j, r in enumerate(self.in_rel[l][t]):
           ell, ks = self._rel_ell(r, nh)
           nat.sage_scatter_block(self.dA[l][t], H, offs[j], self._ctr[t], nh, ell, ks, ar.deg_of(r),
                                  self.dH[l - 1][self.nt[r]])
-          self._k()
         nat.add_block_f32(self.dA[l][t], self_col, H, self._ctr[t], nh, self.dH[l - 1][t])
-        self._k()
       for s in self.targets[l - 1]:
-        self._k(nat.relu_bwd_cast(self.dH[l - 1][s], self.Z[l - 1][s], self._ctr[s], nh + 1, self.dPre[l - 1][s],
-                                  self.param(('b', l - 1, s), True), True))
+        nat.relu_bwd_cast(self.dH[l - 1][s], self.Z[l - 1][s], self._ctr[s], nh + 1, self.dPre[l - 1][s],
+                          self.param(('b', l - 1, s), True), True)
 
   def _optimizer(self):
     if self.peer_group is not None:
       self.peer_group.barrier(0)            # every rank finished writing its gradients
       self.peer_group.adam(self.p32, self.m, self.v, self.p16, self.lr, 0.9, 0.999, 1e-8, self.wd, self.step_dev,
                            1.0 / self.world)
-      self._k(2)
       return
     self.nat.adam_step(self.p32, self.g32, self.m, self.v, self.p16, self.lr, 0.9, 0.999, 1e-8, self.wd,
                        self.step_dev, 1.0)
-    self._k()
 
   def _step_eager(self):
     self._sample()
@@ -465,26 +448,28 @@ class HeteroSageEngine(object):
 
   # ------------------------------------------------------------------ public API
   def warmup_and_capture(self, n_eager: int = 2):
+    """Run a few eager steps (lazy inits, GEMM plans), then capture the step into one CUDA graph and set
+    `kernels_per_step` to its kernel, memset and memcpy nodes.  Engines built with use_cuda_graph=False capture the
+    step only to count it, and keep running eagerly."""
     with torch.cuda.device(self.device):
       saved = self.state_dict()
       side = torch.cuda.Stream()
       side.wait_stream(torch.cuda.current_stream())
       with torch.cuda.stream(side):
         for _ in range(n_eager):
-          self._tally = 0
           self._step_eager()
-          self.kernels_per_step = self._tally
       torch.cuda.current_stream().wait_stream(side)
       torch.cuda.synchronize()
       self.load_state_dict(saved)
-      if not self.use_cuda_graph:
-        return
-      g = torch.cuda.CUDAGraph()
+      g = torch.cuda.CUDAGraph(keep_graph=True)
       with torch.cuda.graph(g):
         self._step_eager()
+      self.kernels_per_step = sum(self.nat.graph_node_counts(g.raw_cuda_graph()))
+      if self.use_cuda_graph:
+        g.instantiate()
       torch.cuda.synchronize()
       self.load_state_dict(saved)
-      self._graph = g
+      self._graph = g if self.use_cuda_graph else None
 
   def train_step(self, seeds: torch.Tensor) -> torch.Tensor:
     """One training step on a batch of seed ids of `seed_type` (host-pinned or device tensor); returns the device

@@ -195,11 +195,9 @@ class HeteroGatEngine(HeteroSageEngine):
           s = self.nt[r]
           ns, ntr, Ps, Pd = self._views(l, r)
           self._gat_plan('proj', l, r).run()
-          self._k()
           nat.gat_scores(Ps, self.param(('att_src', l, r)), self.as_[r][:ns], self._ctr[s], nh + 1,
                          Pd if Pd is not None else Ps[:ntr], self.param(('att_dst', l, r)), self.ad_[r][:ntr],
                          self._ctr[t], nh, zero=self.dsrc[(l, r)], heads=hd)
-          self._k()
           ell, ks = self._rel_ell(r, nh)
           last = j == len(rels) - 1
           nat.gat_aggregate(Ps, self.as_[r][:ns], self.ad_[r][:ntr], hd, self._ctr[t], nh, ell, ks, ar.deg_of(r),
@@ -207,24 +205,19 @@ class HeteroGatEngine(HeteroSageEngine):
                             last=last, bias=self._rel_params('bias', l, t) if last else None, act=l < self.L,
                             p=p if l < self.L else 0.0, seed=self.seed, layer=l, step_dev=self.step_dev,
                             Z=self.Z[l][t] if last else None)
-          self._k()
     self._head_plan().run()
-    self._k()
     self._loss(self.logits, self.dlogits, self.param(('head_b',), True))
 
   def _backward(self):
     nat, ar, hd, H = self.nat, self.arena, self.heads, self.hidden
     st = self.tid[self.seed_type]
     self._head_plan(self.G[self.L][st]).run()
-    self._k()
     nat.gat_act_bwd(None, None, self.G[self.L][st], self._ctr[st], 1, bias_g=self._rel_params('bias', self.L, st, True))
-    self._k()
     for l in range(self.L, 0, -1):
       nh = self.L - l + 1
       if l > 1:
         for u in self.targets[l - 1]:
           nat.zero_rows(self.dH[l - 1][u], self._ctr[u], nh + 1)
-          self._k()
       for t in self.targets[l]:
         for r in self.in_rel[l][t]:
           s = self.nt[r]
@@ -232,28 +225,22 @@ class HeteroGatEngine(HeteroSageEngine):
           ell, ks = self._rel_ell(r, nh)
           nat.gat_backward(self.G[l][t], Ps, hd, self._ctr[t], nh, ell, ks, ar.deg_of(r), self.alpha[(l, r)],
                            self.dal[r][:nh], self.dP32[r][:ns], self.dsrc[(l, r)], self.dadst[r][:ntr])
-          self._k()
           nat.gat_score_bwd(Ps, self.dP32[r][:ns], self.dsrc[(l, r)], self.param(('att_src', l, r)),
                             self.param(('att_src', l, r), True), self.dPs[r][:ns], self._ctr[s], nh + 1,
                             self.dadst[r][:ntr], self.param(('att_dst', l, r)), self.param(('att_dst', l, r), True),
                             self._ctr[t], nh, P_dst=Pd, dPb_dst=self.dPd[r][:ntr] if Pd is not None else None,
                             heads=hd)
-          self._k()
           self._gat_plan('wgrad', l, r).run()
-          self._k()
           if l > 1:
             self._gat_plan('dgrad', l, r).run()
             nat.add_block_f32(self.dX[s][:ns], 0, H, self._ctr[s], nh + 1, self.dH[l - 1][s])
-            self._k(2)
             if Pd is not None:
               nat.add_block_f32(self.dX[t][:ntr], 0, H, self._ctr[t], nh, self.dH[l - 1][t])
-              self._k()
       if l > 1:
         for u in self.targets[l - 1]:
           nat.gat_act_bwd(self.dH[l - 1][u], self.Z[l - 1][u], self.G[l - 1][u], self._ctr[u], nh + 1,
                           p=self.dropout, seed=self.seed, layer=l - 1, step_dev=self.step_dev,
                           bias_g=self._rel_params('bias', l - 1, u, True))
-          self._k()
 
   # ------------------------------------------------------------------ full-neighbourhood inference
   def _infer_chunk_row_bytes(self) -> int:

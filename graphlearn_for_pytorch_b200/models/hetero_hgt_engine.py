@@ -236,16 +236,13 @@ class HeteroHgtEngine(HeteroSageEngine):
     for u in self.in_types:
       self._gather_input(u)
       self._hgt_plan('in_fwd', 0, u).run()
-      self._k()
     for l in range(1, L + 1):
       nh = L - l + 1
       for t in self.targets[l]:
         nat.hgt_blocks(self._blocks('att', l, t), self._blocks('msg', l, t), self.att_img[(l, t)],
                        self.msg_img[(l, t)])
-        self._k()
       for u in self.kqv_types[l]:
         self._hgt_plan('kqv_fwd', l, u).run()
-        self._k()
       for t in self.targets[l]:
         c = self._ctr[t]
         self._hgt_plan('qq_fwd', l, t).run()
@@ -255,21 +252,17 @@ class HeteroHgtEngine(HeteroSageEngine):
         nat.hgt_gelu(self.AGG[l][t], self.GE[l][t], c, nh)
         self._hgt_plan('a_fwd', l, t).run()
         nat.hgt_gate(self.A[l][t], self.Z[l - 1][t][:self._rows(l, t)], self.Z[l][t], self._p32(('skip', l, t)), c, nh)
-        self._k(6)
     self._head_plan().run()
-    self._k()
     self._loss(self.logits, self.dlogits, self.param(('head_b',), True))
 
   def _backward(self):
     nat, L, H = self.nat, self.L, self.hidden
     self._head_plan(self.dZL).run()
-    self._k()
     for l in range(L, 0, -1):
       nh = L - l + 1
       below = self.dH[l - 1]
       for u in below:
         nat.zero_rows(below[u], self._ctr[u], nh + 1)
-        self._k()
       for t in self.targets[l]:
         c, n, R = self._ctr[t], self._rows(l, t), len(self.in_rel[l][t])
         dZ = self.dZL if l == L else self.dH[l][t]
@@ -289,7 +282,6 @@ class HeteroHgtEngine(HeteroSageEngine):
         nat.hgt_blocks(self._blocks('att', l, t), self._blocks('msg', l, t), self.att_img[(l, t)],
                        self.msg_img[(l, t)], att_dense=self.g_att[t][:R * H * H], msg_dense=self.g_msg[t][:R * H * H],
                        att_g=self._blocks('att', l, t, True), msg_g=self._blocks('msg', l, t, True))
-        self._k(8)
       for u in self.kqv_types[l]:
         n = self._rows(l - 1, u)
         is_t = u in self.targets[l]
@@ -297,12 +289,10 @@ class HeteroHgtEngine(HeteroSageEngine):
                          self._p32(('kqv_b', l, u), True), self._ctr[u], nh + 1, nh)
         self._hgt_plan('kqv_bwd', l, u).run()
         nat.add_block_f32(self.dX[u][:n], 0, H, self._ctr[u], nh + 1, below[u])
-        self._k(3)
     for u in self.in_types:
-      self._k(nat.relu_bwd_cast(self.dH[0][u], self.Z[0][u], self._ctr[u], L + 1, self.dPre0[u],
-                                self.param(('in_b', u), True), True, 1.0, True))
+      nat.relu_bwd_cast(self.dH[0][u], self.Z[0][u], self._ctr[u], L + 1, self.dPre0[u],
+                        self.param(('in_b', u), True), True, 1.0, True)
       self._hgt_plan('in_bwd', 0, u).run()
-      self._k()
 
   # ------------------------------------------------------------------ full-neighbourhood inference
   def _infer_chunk_row_bytes(self) -> int:

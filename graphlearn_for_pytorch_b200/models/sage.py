@@ -9,7 +9,7 @@ fanout [15,10,5], batch 1024).  `GraphSAGE` below is the drop-in eager module fo
     -> layer 1: ONE wgmma kernel = peer/local HBM row gather + neighbour mean +
        [mean | self] x W1 + bias + ReLU (csrc/cuda/sage_tc.cu)
     -> layers 2..L: ELL aggregation kernel + wgmma GEMM (csrc/cuda/tc_gemm.cu)
-    -> fused log-softmax/NLL fwd+bwd -> hand-written backward -> NCCL all-reduce -> fused Adam
+    -> fused log-softmax/NLL fwd+bwd -> hand-written backward -> Adam (multi-GPU: fused with a peer-HBM all-reduce)
 
 with every extent read from device counters, so the whole step is a fixed launch sequence
 replayed from a CUDA graph.
@@ -98,7 +98,8 @@ class GraphSageEngine(object):
     fanouts / batch_size / hidden / num_classes: model + sampling config.  `hidden` is a multiple of 8 up to 1024
       (a multiple of 64 unless every hidden layer runs the fused kernel); see `_check_widths`.  Widths that no
       kernel supports raise ValueError here.
-    group: torch.distributed group for the gradient all-reduce (None = single process).
+    group: torch.distributed group of the data-parallel ranks (None = single process).  Every rank reads the
+      others' gradients and feature rows in place, so the GPUs of the group need peer access.
     use_fused: True = use the wgmma gather+GEMM kernel where the shape allows; 'auto' = time the
       fused and the unfused (aggregate kernel + wgmma GEMM) layer on real batches during warm-up and
       keep the faster one (remote-heavy multi-GPU runs can favour the unfused pair).
@@ -119,7 +120,6 @@ class GraphSageEngine(object):
                device: Optional[torch.device] = None, group=None, use_fused: bool = True,
                use_cuda_graph: bool = True, calibration_seeds: Optional[torch.Tensor] = None,
                calibration_margin: float = 1.3, calibration_batches: int = 16, pipeline: bool = False,
-               use_peer_allreduce: bool = True,
                check_every: int = 64, auto_regrow: bool = True, feature_format: str = 'bf16',
                deterministic_sampling: bool = False,
                dropout: float = 0.0, preaggregate_layer1: Optional[bool] = None):
@@ -143,7 +143,6 @@ class GraphSageEngine(object):
       use_fused = True
     self.pipeline = bool(pipeline)
     self.deterministic_sampling = bool(deterministic_sampling)
-    self.use_peer_allreduce = bool(use_peer_allreduce)
     self._preagg_opt = preaggregate_layer1 is None or bool(preaggregate_layer1)
     self.preaggregate = False         # resolved once the layer-1 variant is known (_resolve_preagg)
     self._tc_plans = {}
@@ -207,8 +206,6 @@ class GraphSageEngine(object):
       self._repack()
       self._resolve_preagg()
     self._graph_fb = None
-    self._graph_opt = None
-    self._graph_full = None
 
   def _fused_shape(self, l: int, d: int, n_out: int) -> bool:
     """Can the fused layer kernel run layer l (input width d, output width n_out)?  Its MXFP8 loader is written for
@@ -279,7 +276,7 @@ class GraphSageEngine(object):
                               for l in range(2, self.L + 1)]
     self._tc_plans = {}
     self._graphs = []
-    self._graph_fb = self._graph_opt = self._graph_full = None
+    self._graph_fb = None
 
   def regrow(self, factor: float = 1.5):
     """Enlarge the (calibrated) arena after neighbours were dropped by the capacity guard: new per-hop
@@ -294,7 +291,7 @@ class GraphSageEngine(object):
       del tmp
       caps = [self.bs] + [min(worst[h], (int(self.cap_rows[h] * factor) + 255) // 128 * 128)
                           for h in range(1, self.L + 1)]
-      had_graphs = bool(getattr(self, '_graphs', None))
+      had_graphs = bool(self._graphs)
       self._build_buffers(caps)
       for a, v in zip(self._arenas, steps):
         a.step.fill_(v)
@@ -427,7 +424,7 @@ class GraphSageEngine(object):
     self.p16 = self.p32.to(torch.bfloat16)
     self._g = [torch.zeros_like(self.p32)]
     self._peer_groups = []
-    if self.world > 1 and self.use_peer_allreduce:
+    if self.world > 1:
       # gradients live in a symmetric-heap segment: the optimizer kernel of every rank reads
       # all peers' gradients over NVLink (all-reduce fused into Adam, no NCCL in the step)
       import torch.distributed as dist
@@ -459,7 +456,6 @@ class GraphSageEngine(object):
     for l in range(1, self.L + 1):
       if self.fused_ok[l]:
         self.nat.pack_weight_into(self.W(l), self.w_packed[l])
-        self._k(1)
 
   def state_dict(self):
     return {'p32': self.p32.clone(), 'm': self.m.clone(), 'v': self.v.clone(),
@@ -479,11 +475,6 @@ class GraphSageEngine(object):
     self._repack()
 
   # ------------------------------------------------------------------ step pieces
-  def _k(self, n):
-    self._tally += n
-
-  _tally = 0
-
   def _ell(self, l):
     """ELL blocks + strides used by layer l: hops 0..L-l."""
     nh = self.L - l + 1
@@ -496,7 +487,6 @@ class GraphSageEngine(object):
     ar = self._arenas[which]
     # (the increment itself is folded into the first sampling kernel: step_inc)
     ar.sample(self.gh, self._seeds[which], None, self.seed, 0, False, False, True, len(self._arenas))
-    self._k(2 + 2 * self.L)  # table clear + init_seeds + (sample, relabel) per hop
     if self.preaggregate:
       self._aggregate_layer1(which)
 
@@ -507,7 +497,6 @@ class GraphSageEngine(object):
     nh = self.L
     self.nat.sage_aggregate(self.feat, ar.nodes, None, self.in_dim, ar.counters, nh, list(ar.ell[:nh]),
                             self.fanouts[:nh], ar.deg, self._A1[which])
-    self._k(1)
 
   def _forward(self, train: bool = True):
     nat, ar = self.nat, self.arena
@@ -520,7 +509,6 @@ class GraphSageEngine(object):
     if train and self.dropout > 0.0 and l < self.L:
       self.nat.dropout_bf16(self.Z[l], self.arena.counters, self.L - l + 1, self.dropout, self.seed, l,
                             self.step_dev)
-      self._k(1)
 
   def _forward_layer_nodrop(self, l: int):
     nat, ar = self.nat, self.arena
@@ -533,14 +521,11 @@ class GraphSageEngine(object):
     if self.fused_ok[l]:
       nat.sage_fused(feat, nodes, src_local, d, ar.counters, nh, ell, ks, ar.deg, self.w_packed[l],
                      self.b(l), relu, self.Z[l], self.A[l])
-      self._k(1)
     else:
       if not (l == 1 and self.preaggregate):     # pre-aggregated: _sample already wrote A1 of this arena
         nat.sage_aggregate(feat, nodes, src_local, d, ar.counters, nh, ell, ks, ar.deg, self._A(l))
-        self._k(1)
       # Z = act(A . W^T + b) on wgmma (TMA-fed, bias/ReLU in the register epilogue, rows from the device counter)
       self._plan('fwd', l).run()
-      self._k(1)
 
   def _forward_loss(self, train: bool = True):
     # labels[nodes[r]] is looked up inside the loss kernel (no gather launch)
@@ -549,8 +534,8 @@ class GraphSageEngine(object):
     if train:                      # evaluation must not take part in the cross-rank gradient protocol
       self._begin_grads()
     # the bias gradient of the last layer (column sums of dlogits) is produced by the loss kernel
-    self._k(nat.softmax_nll(self.Z[self.L], self.C, None, self.labels, ar.nodes, ar.counters, self.loss,
-                            self.dPre[self.L], self.correct, self.g32[boff:boff + n], train))
+    nat.softmax_nll(self.Z[self.L], self.C, None, self.labels, ar.nodes, ar.counters, self.loss, self.dPre[self.L],
+                    self.correct, self.g32[boff:boff + n], train)
 
   def _begin_grads(self):
     """Runs before the first kernel that writes into the flat gradient buffer (the loss kernel produces the
@@ -558,11 +543,9 @@ class GraphSageEngine(object):
     gradient kernels accumulate with red.add, so the buffer starts from zero."""
     if self.peer_group is not None and len(self._peer_groups) == 1:
       self.peer_group.barrier(1)          # peers finished reading last step's gradients
-      self._k(1)
     # one launch zeroes the flat gradient buffer, the loss and the #correct counter; the kernels that accumulate
     # into them then skip their own memsets (memset nodes would cut the programmatic-launch chain of the step)
     self.nat.zero_grads(self.g32, self.loss, self.correct)
-    self._k(1)
 
   def _plan(self, kind: str, l: int):
     """Cached TcGemm launch for layer l of the current arena / gradient parity (tensor maps are encoded once)."""
@@ -589,12 +572,10 @@ class GraphSageEngine(object):
     # bias gradients are fused into the kernels that produce dPre (loss / sage_gather_bwd)
     for l in range(self.L, 0, -1):
       self._plan('bwd', l).run()
-      self._k(1)
       if l > 1:
         pboff, pn = self._b_off[l - 2]
         self.nat.sage_gather_bwd(self.dA[l], self.dims_in[l - 1], self.arena, self.L - l + 1, self.Z[l - 1],
                                  self.dPre[l - 1], self.g32[pboff:pboff + pn], True, 1.0 / (1.0 - self.dropout))
-        self._k(1)
 
   def _optimizer(self):
     # Adam's step counter is advanced by the kernel itself (last block to finish)
@@ -603,17 +584,16 @@ class GraphSageEngine(object):
       pg.barrier(0)                       # every rank finished writing its gradients
       pg.adam(self.p32, self.m, self.v, self.p16, self.lr, 0.9, 0.999, 1e-8, self.wd,
                            self.step_dev, 1.0 / self.world)
-      self._k(2)
     else:
       self.nat.adam_step(self.p32, self.g32, self.m, self.v, self.p16, self.lr, 0.9, 0.999, 1e-8, self.wd,
                          self.step_dev, 1.0 / self.world)
-      self._k(1)
     self._repack()
 
-  def _allreduce(self):
-    if self.world > 1 and self.peer_group is None:
-      import torch.distributed as dist
-      dist.all_reduce(self.g32, group=self.group)
+  def _train(self):
+    """Forward, backward and optimizer update of the batch in the current arena."""
+    self._forward()
+    self._backward()
+    self._optimizer()
 
   def _pipelined_body(self, cur: int):
     """train(batch in arena[cur])  ||  sample(next batch into arena[1-cur])."""
@@ -622,8 +602,7 @@ class GraphSageEngine(object):
     self._side.wait_stream(main)                       # fork
     with torch.cuda.stream(self._side):
       self._sample(1 - cur)
-    self._forward()
-    self._backward()
+    self._train()
     main.wait_stream(self._side)                        # join
 
   def _step_eager(self):
@@ -631,10 +610,7 @@ class GraphSageEngine(object):
       self._pipelined_body(self._cur)
     else:
       self._sample()
-      self._forward()
-      self._backward()
-    self._allreduce()
-    self._optimizer()
+      self._train()
 
   def _autotune(self, iters: int = 5):
     """Pick fused vs unfused per layer from device timings on the current batch."""
@@ -663,9 +639,9 @@ class GraphSageEngine(object):
 
   # ------------------------------------------------------------------ public API
   def warmup_and_capture(self, n_eager: int = 2):
-    """Run a few eager steps (lazy inits, GEMM plans), then capture the CUDA graphs.
-    Pipelined engines capture one graph per buffer parity."""
-    import os
+    """Run a few eager steps (lazy inits, GEMM plans), then capture the step into a CUDA graph, one per buffer parity
+    in pipelined engines, and set `kernels_per_step` to the kernel, memset and memcpy nodes of the parity-0 graph.
+    Engines built with use_cuda_graph=False capture one step only to count it, and keep running eagerly."""
     with torch.cuda.device(self.device):
       saved = self.state_dict()
       side = torch.cuda.Stream()
@@ -674,9 +650,7 @@ class GraphSageEngine(object):
         if self.pipeline:
           self._sample(0)
         for _ in range(n_eager):
-          self._tally = 0
           self._step_eager()
-          self.kernels_per_step = self._tally
           if self.pipeline:
             self._cur ^= 1
       torch.cuda.current_stream().wait_stream(side)
@@ -688,60 +662,40 @@ class GraphSageEngine(object):
         self._resolve_preagg()
         if self.pipeline:
           self._sample(0)
-        self._tally = 0
-        self._step_eager()                      # re-count kernels with the chosen variants
-        self.kernels_per_step = self._tally
+        self._step_eager()                      # builds the GEMM plans of the chosen variants outside the capture
         torch.cuda.synchronize()
         self._cur = 0
       self.load_state_dict(saved)
       self._cur, self._primed = 0, False
       self._graphs = []
-      if not self.use_cuda_graph:
-        return
       # programmatic dependent launch helps single-stream chains and costs ~2 % when the sampling and training
       # streams interleave (measured, csrc/cuda/launch_utils.h): captured without it in pipelined mode
       prev_pdl = self.nat.set_pdl(not self.pipeline)
-      # capturing NCCL collectives works but makes process-group teardown hang on this stack
-      # (measured: bench exit blocked until the timeout), so it is opt-in for world > 1
-      single = self.world == 1 or self.peer_group is not None or \
-          os.environ.get('GLT_B200_CAPTURE_NCCL', '0') == '1'
-      g_opt = None
-      for parity in range(2 if self.pipeline else 1):
-        g = torch.cuda.CUDAGraph()
+      for parity in range(2 if self.pipeline and self.use_cuda_graph else 1):
+        g = torch.cuda.CUDAGraph(keep_graph=True)
+        self._cur = parity
         with torch.cuda.graph(g):
-          if self.pipeline:
-            self._pipelined_body(parity)
-          else:
-            self._sample()
-            self._forward()
-            self._backward()
-          if single:
-            self._allreduce()
-            self._optimizer()
-        if not single and g_opt is None:
-          g_opt = torch.cuda.CUDAGraph()
-          with torch.cuda.graph(g_opt):
-            self._optimizer()
-        self._graphs.append((g, None if single else g_opt))
+          self._step_eager()
+        if parity == 0:
+          self.kernels_per_step = sum(self.nat.graph_node_counts(g.raw_cuda_graph()))
+        if self.use_cuda_graph:
+          g.instantiate()
+          self._graphs.append(g)
       torch.cuda.synchronize()
       self.nat.set_pdl(prev_pdl)
       self.load_state_dict(saved)
       self._cur, self._primed = 0, False
-      self._graph_fb = self._graphs[0][0]
+      self._graph_fb = self._graphs[0] if self._graphs else None
 
   def close(self):
     """Drop the captured graphs (call before destroying the process group)."""
     torch.cuda.synchronize(self.device)
     self._graphs = []
-    self._graph_full = self._graph_fb = self._graph_opt = None
+    self._graph_fb = None
 
   def _run_captured_or_eager(self, parity: int):
-    if getattr(self, '_graphs', None):
-      g, g_opt = self._graphs[parity]
-      g.replay()
-      if g_opt is not None:
-        self._allreduce()
-        g_opt.replay()
+    if self._graphs:
+      self._graphs[parity].replay()
     else:
       self._cur = parity
       self._step_eager()
@@ -786,10 +740,7 @@ class GraphSageEngine(object):
     """Pipelined mode: train the batch that was sampled by the last train_step() call."""
     if not self.pipeline or not self._primed:
       return None
-    self._forward()
-    self._backward()
-    self._allreduce()
-    self._optimizer()
+    self._train()
     self._primed = False
     self.step_idx += 1
     return self.loss
@@ -813,7 +764,7 @@ class GraphSageEngine(object):
       for l in range(2, self.L + 1):
         self._forward_layer(l)
       self._forward_loss(); ev[3].record()
-      self._backward(); self._allreduce(); ev[4].record()
+      self._backward(); ev[4].record()
       self._optimizer(); ev[5].record()
       torch.cuda.synchronize()
       if it >= 2:
@@ -873,10 +824,7 @@ class GraphSageEngine(object):
           # a pipelined step runs it on the sampling stream, outside the training chain
           self._aggregate_layer1(0)
           log[-1] = ('sage_aggregate (layer 1, sampling stream)',) + log[-1][1:]
-        self._forward()
-        self._backward()
-        self._allreduce()
-        self._optimizer()
+        self._train()
         torch.cuda.synchronize()
         if it >= 2:
           if acc is None:

@@ -97,7 +97,6 @@ class GraphSageLinkEngine(GraphSageEngine):
     # reads ar.step before the arena's first kernel advances it (same stream)
     self.nat.link_seeds(self.gh, self._pos[which], self._num_nodes, self.neg_ratio, self.seed, ar.step,
                         self._seeds[which], self._n_pairs[which])
-    self._k(1)
     super()._sample(which)
 
   def _forward_loss(self, train: bool = True):
@@ -105,18 +104,16 @@ class GraphSageLinkEngine(GraphSageEngine):
     if train:
       self._begin_grads()
       nat.zero_rows(self._dZ32, ar.counters, 1)
-      self._k(1)
     else:
       self.loss.zero_()
       self.correct.zero_()
     nat.link_bce(self.Z[L], self.C, ar.seed_local, self.P, self.pos_bs, self._n_pairs[self._cur], self.loss,
                  self.correct, self._dZ32 if train else None)
-    self._k(1)
     if not train:
       return
     boff, n = self._b_off[L - 1]
-    self._k(nat.relu_bwd_cast(self._dZ32, self.Z[L], ar.counters, 1, self.dPre[L], self.g32[boff:boff + n], True, 1.0,
-                              relu=False))
+    nat.relu_bwd_cast(self._dZ32, self.Z[L], ar.counters, 1, self.dPre[L], self.g32[boff:boff + n], True, 1.0,
+                      relu=False)
 
   @torch.no_grad()
   def evaluate_batch(self, pairs: torch.Tensor):

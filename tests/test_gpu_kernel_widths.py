@@ -252,21 +252,30 @@ def test_colsum_bf16_matches_fp64(native, d):
 
 
 # --------------------------------------------------------------------------- limits and launch counts
-def test_bias_gradient_launches(native):
+def _captured_kernels(native, fn, *args):
+  """Kernel nodes of a CUDA graph holding the one call fn(*args)."""
+  g = torch.cuda.CUDAGraph(keep_graph=True)
+  with torch.cuda.graph(g):
+    fn(*args)
+  return native.graph_node_counts(g.raw_cuda_graph())[0]
+
+
+def test_bias_gradient_kernel_nodes(native):
   """The bias gradient is fused into the cast / loss kernel where it can be (d | 2048, ld <= 256) and takes one extra
-  column-sum kernel elsewhere; the bindings report the number of kernels they launched."""
+  column-sum kernel elsewhere, counted on the kernel nodes of the captured call."""
   ctr = _counters([0, 10])
   for d in (64, 96, 256, 320, 2048):
     dH = torch.zeros(16, d, device=DEV)
     Z = torch.zeros(16, d, dtype=torch.bfloat16, device=DEV)
-    n = native.relu_bwd_cast(dH, Z, ctr, 1, Z.clone(), torch.zeros(d, device=DEV), False, 1.0)
+    n = _captured_kernels(native, native.relu_bwd_cast, dH, Z, ctr, 1, Z.clone(), torch.zeros(d, device=DEV), False,
+                          1.0)
     assert n == (1 if 2048 % d == 0 else 2), (d, n)
-    assert native.relu_bwd_cast(dH, Z, ctr, 1, Z.clone(), None, False, 1.0) == 1
+    assert _captured_kernels(native, native.relu_bwd_cast, dH, Z, ctr, 1, Z.clone(), None, False, 1.0) == 1
   for ld in (64, 256, 320, 3008):
     lg = torch.zeros(16, ld, dtype=torch.bfloat16, device=DEV)
     y = torch.zeros(16, dtype=torch.int64, device=DEV)
-    n = native.softmax_nll(lg, ld - 5, y, None, None, ctr, torch.zeros(1, device=DEV), lg.clone(), None,
-                           torch.zeros(ld, device=DEV), False)
+    n = _captured_kernels(native, native.softmax_nll, lg, ld - 5, y, None, None, ctr, torch.zeros(1, device=DEV),
+                          lg.clone(), None, torch.zeros(ld, device=DEV), False)
     assert n == (1 if ld <= 256 else 2), (ld, n)
 
 
