@@ -67,8 +67,11 @@ __global__ void __launch_bounds__(256) k_adam_peer(PeerPtrs p, float* param, flo
   // skipped on every rank that saw the timeout; the host raises at its next health check (models/sage.py)
   if (err && *reinterpret_cast<const volatile int32_t*>(err) != 0) return;
   // t = steps so far + 1; the last block to finish publishes it (see k_adam)
-  const float t = static_cast<float>(*reinterpret_cast<volatile int32_t*>(step_dev) + 1);
-  const float c1 = 1.f - __powf(b1, t), c2 = 1.f - __powf(b2, t);
+  const int t = *reinterpret_cast<volatile int32_t*>(step_dev) + 1;
+  // bias corrections in double, as k_sparse_adam: 1 - b2^t cancels most of b2^t's bits at small t, which left the
+  // error of __powf's approximate log2 in the update at dozens of times its fp32 rounding error
+  const float c1 = static_cast<float>(1.0 - pow(static_cast<double>(b1), t));
+  const float c2 = static_cast<float>(1.0 - pow(static_cast<double>(b2), t));
   const int64_t n4 = n >> 2;
   for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < n4;
        i += static_cast<int64_t>(gridDim.x) * blockDim.x) {

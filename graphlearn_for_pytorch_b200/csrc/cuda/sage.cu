@@ -266,8 +266,11 @@ __global__ void k_adam(float* p, const float* g, float* m, float* v, __nv_bfloat
                        float lr, float b1, float b2, float eps, float wd, int32_t* step_dev,
                        float gscale) {
   pdl_enter();
-  const float t = static_cast<float>(*reinterpret_cast<volatile int32_t*>(step_dev) + 1);
-  const float c1 = 1.f - __powf(b1, t), c2 = 1.f - __powf(b2, t);
+  const int t = *reinterpret_cast<volatile int32_t*>(step_dev) + 1;
+  // bias corrections in double, as k_sparse_adam: 1 - b2^t cancels most of b2^t's bits at small t, which left the
+  // error of __powf's approximate log2 in the update at dozens of times its fp32 rounding error
+  const float c1 = static_cast<float>(1.0 - pow(static_cast<double>(b1), t));
+  const float c2 = static_cast<float>(1.0 - pow(static_cast<double>(b2), t));
   for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < n;
        i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
     float gi = g[i] * gscale + wd * p[i];

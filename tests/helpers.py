@@ -50,6 +50,62 @@ def gemm_bound(ref: torch.Tensor, absprod: torch.Tensor, k: int, bf16_out: bool 
   return b + bf16_ulp(ref) if bf16_out else b
 
 
+EPS32 = 2.0 ** -23
+
+
+def sum_bound(n, abs_sum: torch.Tensor) -> torch.Tensor:
+  """Largest error of an fp32 sum of n terms (in any order, each term rounded once): (n + 1) * 2^-23 * sum|terms|."""
+  n = n.double() if torch.is_tensor(n) else float(n)
+  return (n + 1) * EPS32 * abs_sum.double()
+
+
+def mean_ref(X: torch.Tensor, tgt: torch.Tensor, src: torch.Tensor, deg: torch.Tensor):
+  """float64 mean aggregation sum_{edges t <- s} X[s] / deg[t] over the T = deg.numel() targets, and its error bound:
+  one bf16 ulp of the mean, plus the fp32 sum of deg rows and the multiplication by the fp32 1/deg; rows of degree 0
+  must be exactly 0."""
+  Xd = X.double()
+  T, d = deg.numel(), X.shape[1]
+  s = torch.zeros(T, d, dtype=torch.float64, device=X.device).index_add_(0, tgt, Xd[src])
+  a = torch.zeros(T, d, dtype=torch.float64, device=X.device).index_add_(0, tgt, Xd[src].abs())
+  dg = deg.to(X.device).double().unsqueeze(1)
+  ref = s / dg.clamp(min=1)
+  bound = torch.where(dg > 0, bf16_ulp(ref) + (dg + 2) * EPS32 * a / dg.clamp(min=1), torch.zeros_like(ref))
+  return ref, bound
+
+
+def gather_ref(dA, d, Z, tgt, src, deg, T, S, cap_src, gscale):
+  """float64 dPre of sage_gather_bwd (dPre[s] = relu'(Z[s]) * gscale * (dA[s, d:] if s < T + sum_{t <- s} dA[t, :d] /
+  deg[t])) and its error bound, from the exact bf16 operands and the edges (tgt, src) of the layer's hops; the bound is
+  0 (exact) on masked elements and on rows in [S, cap_src)."""
+  dev = dA.device
+  keep = (tgt < T) & (src < S)
+  tgt, src = tgt[keep], src[keep]
+  inv = (1.0 / deg.float()).double()                   # fp32 1/deg, as the kernel computes it
+  dAd = dA.double()
+  terms = dAd[tgt, :d] * inv[tgt].unsqueeze(1)
+  ref = torch.zeros(cap_src, d, dtype=torch.float64, device=dev)
+  ab = torch.zeros_like(ref)
+  m = min(T, S)
+  ref[:m] = dAd[:m, d:]
+  ab[:m] = dAd[:m, d:].abs()
+  ref.index_add_(0, src, terms)
+  ab.index_add_(0, src, terms.abs())
+  n = torch.bincount(src, minlength=cap_src).double()
+  n[:m] += 1
+  g = float(torch.tensor(gscale, dtype=torch.float32))
+  live = (torch.arange(cap_src, device=dev) < S).unsqueeze(1)
+  mask = live & (Z[:cap_src] > 0) if Z is not None else live.expand(cap_src, d)
+  ref = torch.where(mask, ref * g, torch.zeros_like(ref))
+  bound = torch.where(mask, bf16_ulp(ref) + g * sum_bound((n + 2).unsqueeze(1), ab),torch.zeros_like(ref))
+  return ref, bound
+
+
+def colsum_ratio(colsum: torch.Tensor, X: torch.Tensor, S: int, init: float = 0.0) -> float:
+  """Error / bound of fp32 column sums (bias gradients) of the first S rows of X accumulated onto `init`."""
+  x = X[:S].double()
+  return bound_ratio(colsum, x.sum(0) + init, sum_bound(S, x.abs().sum(0) + abs(init)))
+
+
 def bound_ratio(got: torch.Tensor, ref: torch.Tensor, bound: torch.Tensor) -> float:
   """max |got - ref| / bound over all elements (<= 1 when every element lies within its bound; 0-bound elements
   must match exactly)."""

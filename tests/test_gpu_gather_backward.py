@@ -23,13 +23,12 @@ import torch
 import graphlearn_for_pytorch_b200 as glt
 from graphlearn_for_pytorch_b200.models import GraphSageEngine
 from graphlearn_for_pytorch_b200.utils.synthetic import rmat_edges
-from helpers import bf16_ulp, bound_ratio
+from helpers import bound_ratio, colsum_ratio, gather_ref
 from test_gpu_kernel_widths import AGG_WIDTHS
 
 pytestmark = pytest.mark.gpu
 DEV = torch.device('cuda', 0)
 SENTINEL = 7.0
-EPS32 = 2.0 ** -23
 
 
 # --------------------------------------------------------------------------- hand-built batches
@@ -208,38 +207,6 @@ def gather_batch(native):
   torch.cuda.empty_cache()
 
 
-def _gather_ref(dA, d, Z, tgt, src, deg, T, S, cap_src, gscale):
-  """float64 dPre of sage_gather_bwd and its error bound from the exact bf16 operands and the edges of the layer's
-  hops; the bound is 0 (exact) on masked elements and on rows in [S, cap_src)."""
-  keep = (tgt < T) & (src < S)
-  tgt, src = tgt[keep], src[keep]
-  inv = (1.0 / deg.float()).double()                   # fp32 1/deg, as the kernel computes it
-  dAd = dA.double()
-  terms = dAd[tgt, :d] * inv[tgt].unsqueeze(1)
-  ref = torch.zeros(cap_src, d, dtype=torch.float64, device=DEV)
-  ab = torch.zeros_like(ref)
-  m = min(T, S)
-  ref[:m] = dAd[:m, d:]
-  ab[:m] = dAd[:m, d:].abs()
-  ref.index_add_(0, src, terms)
-  ab.index_add_(0, src, terms.abs())
-  n = torch.bincount(src, minlength=cap_src).double()
-  n[:m] += 1
-  g = float(torch.tensor(gscale, dtype=torch.float32))
-  live = (torch.arange(cap_src, device=DEV) < S).unsqueeze(1)
-  mask = live & (Z[:cap_src] > 0) if Z is not None else live.expand(cap_src, d)
-  ref = torch.where(mask, ref * g, torch.zeros_like(ref))
-  bound = torch.where(mask, bf16_ulp(ref) + (n + 3).unsqueeze(1) * EPS32 * g * ab, torch.zeros_like(ref))
-  return ref, bound
-
-
-def _colsum_ratio(colsum, dPre, S, init):
-  x = dPre[:S].double()
-  ref = x.sum(0) + init
-  bound = (S + 1) * EPS32 * (x.abs().sum(0) + abs(init))
-  return bound_ratio(colsum, ref, bound)
-
-
 @pytest.mark.parametrize('d', AGG_WIDTHS)
 def test_sage_gather_bwd_matches_fp64(native, gather_batch, d):
   ar, hop, tgt, src = gather_batch
@@ -264,14 +231,14 @@ def test_sage_gather_bwd_matches_fp64(native, gather_batch, d):
     native.sage_gather_bwd(dA, d, ar, n_hops, Z, dPre, colsum, bias == 'prezeroed', gscale)
     torch.cuda.synchronize()
     sel = hop < n_hops
-    ref, bound = _gather_ref(dA, d, Z, tgt[sel], src[sel], ar.deg, T, S, cap_src, gscale)
+    ref, bound = gather_ref(dA, d, Z, tgt[sel], src[sel], ar.deg, T, S, cap_src, gscale)
     case = (d, n_hops, rows_dA, cap_src, with_z, round(gscale, 4), bias)
     r = bound_ratio(dPre, ref, bound)
     assert r <= 1.0, f'dPre off its float64 reference {case}: error / bound = {r}'
     assert bool((full[cap_src:] == SENTINEL).all()), f'rows past dPre must stay untouched {case}'
     rc = 0.0
     if bias:
-      rc = _colsum_ratio(colsum, dPre, S, init if bias == 'prezeroed' else 0.0)
+      rc = colsum_ratio(colsum, dPre, S, init if bias == 'prezeroed' else 0.0)
       assert rc <= 1.0, f'bias column sums off {case}: error / bound = {rc}'
       assert bool((cbuf[d:] == init).all()), f'columns past d must stay untouched {case}'
     ratios.append((n_hops, r, rc))
@@ -347,11 +314,11 @@ def test_engine_gather_backward_matches_fp64(native, fanouts, hidden, dropout, p
       dA, Z, dPre = eng.dA[l], eng.Z[l - 1], eng.dPre[l - 1]
       T, S = min(c[n], dA.shape[0]), min(c[n + 1], dPre.shape[0])
       _, tgt, src = _edges(c, _arena_hops(ar, c, n), ar.cap_rows, ar.cap_nodes)
-      ref, bound = _gather_ref(dA, hidden, Z, tgt.to(DEV), src.to(DEV), ar.deg, T, S, dPre.shape[0], gscale)
+      ref, bound = gather_ref(dA, hidden, Z, tgt.to(DEV), src.to(DEV), ar.deg, T, S, dPre.shape[0], gscale)
       r = bound_ratio(dPre, ref, bound)
       assert r <= 1.0, f'layer {l} (parity {parity}): dPre[{l - 1}] error / bound = {r}'
       boff, bn = eng._b_off[l - 2]
-      rc = _colsum_ratio(eng.g32[boff:boff + bn], dPre, S, 0.0)
+      rc = colsum_ratio(eng.g32[boff:boff + bn], dPre, S, 0.0)
       assert rc <= 1.0, f'layer {l} (parity {parity}): bias gradient of layer {l - 1} error / bound = {rc}'
       out.append(f'l={l}/p{parity}: {r:.3f} {rc:.2e}')
   print(f'engine fanouts={fanouts} hidden={hidden} dropout={dropout} pipeline={pipeline} calibrated={calibrated} '

@@ -14,12 +14,11 @@ import torch
 import torch.nn.functional as F
 
 import graphlearn_for_pytorch_b200 as glt
-from helpers import bf16_ulp, bound_ratio
+from helpers import bf16_ulp, bound_ratio, mean_ref, sum_bound
 
 pytestmark = pytest.mark.gpu
 DEV = torch.device('cuda', 0)
 SENTINEL = 7.0
-EPS32 = 2.0 ** -23
 
 # both sides of every lane-group boundary of GLT_DISPATCH_WIDTH (8 columns = one 16-byte vector)
 AGG_WIDTHS = [8, 32, 40, 64, 72, 128, 136, 256, 264, 512, 520, 1024]
@@ -94,7 +93,6 @@ def test_sage_aggregate_matches_fp64_mean(native, d, table, block):
   X, ut, nodes = _sources(600, d, seed=d + 1, table=table)
   feat = ut._table() if table else None
   src_local = None if table else X
-  Xd = X.double()
   ratio = 0.0
   # spare rows above the batch, then counters above the capacity (the kernel clamps to the buffer's rows)
   for cap, total in ((cum[-1] + 37, None), (cum[-1] - 20, cum[-1] + 1000)):
@@ -108,12 +106,7 @@ def test_sage_aggregate_matches_fp64_mean(native, d, table, block):
       native.sage_aggregate(feat, nodes, src_local, d, ctr, 3, ell, ks, deg_d, out)
     torch.cuda.synchronize()
     tg, sr = _edges(cum, deg, ells, T)
-    s = torch.zeros(T, d, dtype=torch.float64, device=DEV).index_add_(0, tg, Xd[sr])
-    a = torch.zeros(T, d, dtype=torch.float64, device=DEV).index_add_(0, tg, Xd[sr].abs())
-    dg = deg[:T].to(DEV).double().unsqueeze(1)
-    ref = s / dg.clamp(min=1)
-    # one bf16 ulp of the mean, plus the fp32 sum of dg rows and the multiplication by the fp32 1/dg
-    bound = torch.where(dg > 0, bf16_ulp(ref) + (dg + 2) * EPS32 * a / dg.clamp(min=1), torch.zeros_like(ref))
+    ref, bound = mean_ref(X, tg, sr, deg[:T])
     r = bound_ratio(out[:T, mcol:mcol + d], ref, bound)
     assert r <= 1.0, (d, table, block, cap, r)
     ratio = max(ratio, r)
@@ -159,7 +152,7 @@ def test_sage_scatter_matches_fp64_sum(native, d, layout):
     n[:T] += 1
     n += torch.bincount(sr, minlength=n_src).double()
     # fp32 summation of n terms (the initial value, the self term and one term per edge), each rounded once
-    bound = (n + 1).unsqueeze(1) * EPS32 * a
+    bound = sum_bound(n.unsqueeze(1), a)
     r = bound_ratio(dH, ref, bound)
     assert r <= 1.0, (d, layout, cap, r)
     ratio = max(ratio, r)
@@ -188,7 +181,7 @@ def test_relu_bwd_cast_bits_and_bias_gradient(native, d, relu, prezeroed):
   assert bool((dPre[T:] == 0).all()), 'rows in [T, cap) must be zero'
   x = dPre[:T].double()
   ref = x.sum(0)
-  bound = (T + 1) * EPS32 * x.abs().sum(0)
+  bound = sum_bound(T, x.abs().sum(0))
   r = bound_ratio(colsum, ref, bound)
   print(f'relu_bwd_cast d={d} relu={relu} prezeroed={prezeroed}: bias gradient error / bound = {r:.3f}')
   assert r <= 1.0, f'bias gradient (column sums of dPre) wrong at d={d}: error / bound = {r}'
@@ -232,7 +225,7 @@ def test_softmax_nll_matches_fp64(native, C, via_nodes):
   first = torch.where(xs == mx, torch.arange(C, device=DEV), C).min(1).values
   assert int(correct.item()) == int((first == lab).sum()), 'correct counts first-index arg-max hits'
   db = dl[:n0].double()
-  rc = bound_ratio(colsum, db.sum(0), (n0 + 1) * EPS32 * db.abs().sum(0))
+  rc = bound_ratio(colsum, db.sum(0), sum_bound(n0, db.abs().sum(0)))
   print(f'softmax_nll C={C} via_nodes={via_nodes}: dlogits error / bound = {r:.3f}, bias gradient {rc:.3f}')
   assert rc <= 1.0, f'bias gradient (column sums of dlogits) wrong at C={C}: error / bound = {rc}'
 
@@ -246,7 +239,7 @@ def test_colsum_bf16_matches_fp64(native, d):
   native.colsum_bf16(X, _counters([0, 500, T]), 2, out)
   torch.cuda.synchronize()
   x = X[:T].double()
-  r = bound_ratio(out, x.sum(0), (T + 1) * EPS32 * x.abs().sum(0))
+  r = bound_ratio(out, x.sum(0), sum_bound(T, x.abs().sum(0)))
   print(f'colsum_bf16 d={d}: error / bound = {r:.3f}')
   assert r <= 1.0, (d, r)
 
