@@ -69,7 +69,10 @@ class HeteroGatEngine(HeteroSageEngine):
     self._check_attention_schema()
     z, f32 = self._zeros, torch.float32
     H, nhd = self.hidden, self.heads
-    self.X0 = {t: z(self._rows(0, t), self.dim_in[self.ntypes[t]]) for t in self.targets[1]}
+    # layer 1 reads the features of its targets and of its relations' sources (a source type can be sampled only at
+    # the deepest hop, outside targets[1])
+    self.in_types = sorted(set(self.targets[1]) | {self.nt[r] for t in self.targets[1] for r in self.in_rel[1][t]})
+    self.X0 = {t: z(self._rows(0, t), self.dim_in[self.ntypes[t]]) for t in self.in_types}
     self.Z, self.G, self.dH = [None], [None], [None]
     for l in range(1, self.L + 1):
       self.Z.append({t: z(self._rows(l, t), H) for t in self.targets[l]})
@@ -185,7 +188,7 @@ class HeteroGatEngine(HeteroSageEngine):
   def _forward(self):
     nat, ar, hd = self.nat, self.arena, self.heads
     p = self.dropout if self._training else 0.0
-    for t in self.targets[1]:
+    for t in self.in_types:
       self._gather_input(t)
     for l in range(1, self.L + 1):
       nh = self.L - l + 1

@@ -40,15 +40,14 @@ math): expf and erff are within 2 ulp and the division is correctly rounded, whi
 import pytest
 import torch
 
-from helpers import bf16_ulp, bound_ratio
+from helpers import (act_bwd_ref, bf16_ulp, block_grads, block_images, bound_ratio, colsum_bound, gate_da_ref,
+                     gate_dx_ref, gate_ref, gelu_bwd_ref, gelu_ref, skip_g_ref)
 
 pytestmark = pytest.mark.gpu
 DEV = torch.device('cuda', 0)
 SENTINEL = 7.0
 SPARE = 40                        # rows past the capacity the kernel is given; they must keep the sentinel
 EPS32 = 2.0 ** -23
-SIG_ERR = 2.0 ** -21
-ERF_ERR = 2.0 ** -21
 WIDTHS = list(range(64, 1025, 64))
 SMALL_T = (0, 1, 127, 128, 129)
 SEED = 0x1234_5678_9ABC           # both 32-bit halves of the Philox key are non-zero
@@ -83,9 +82,7 @@ def _check_tail(buf, T, z_end, what):
   assert bool((buf[z_end:] == SENTINEL).all()), f'{what}: rows from {z_end} on must not be written'
 
 
-def _sum_bound(x, s0, n):
-  """fp32 sum of n terms (the rows of x, float64) onto s0: (n + 2) EPS32 (sum |x| + |s0|), per column"""
-  return (n + 2) * EPS32 * (x.abs().sum(0) + s0.double().abs())
+_sum_bound = colsum_bound
 
 
 # --------------------------------------------------------------------------- gat_act_bwd
@@ -119,9 +116,9 @@ def _act_bwd(native, d, Tc, cap, p, step, layer, g):
   native.gat_act_bwd(dH, Z, buf[:cap], ctr, 3, p=p, seed=SEED, layer=layer, step_dev=step_dev, bias_g=bias)
   torch.cuda.synchronize()
   got = buf[:T]
-  ref = dH[:T].double() * torch.where(Z[:T] > 0, 1.0, 0.01).double() * keep.double() / (1.0 - p)
+  ref, bound = act_bwd_ref(dH[:T], Z[:T], keep, 1.0 / (1.0 - p))
   where = (d, Tc, cap, p, step, layer)
-  r = bound_ratio(got, ref, bf16_ulp(ref))
+  r = bound_ratio(got, ref, bound)
   assert r <= 1.0, ('dPre', where, r)
   assert torch.equal(got != 0, keep & (dH[:T] != 0)), ('the zeros of dPre are the dropped positions', where)
   _check_tail(buf, T, cap, 'dPre')
@@ -186,14 +183,6 @@ def _gelu_inputs(rows, d, g):
   return pool[torch.randint(0, len(pool), (rows, d), generator=g, device=DEV)].to(torch.bfloat16)
 
 
-def _gelu64(x):
-  return 0.5 * x * (1 + torch.erf(x / 2 ** 0.5))
-
-
-def _gelu_grad64(x):
-  return 0.5 * (1 + torch.erf(x / 2 ** 0.5)) + x * torch.exp(-0.5 * x * x) / (2 * torch.pi) ** 0.5
-
-
 @pytest.mark.parametrize('d', WIDTHS)
 def test_hgt_gelu_matches_fp64(native, d):
   g = torch.Generator(device=DEV).manual_seed(d + 2)
@@ -208,16 +197,13 @@ def test_hgt_gelu_matches_fp64(native, d):
     native.hgt_gelu(X, dX[:cap], ctr, 3, dY=dY)
     torch.cuda.synchronize()
     x = X[:T].double()
-    ref = _gelu64(x)
-    r0 = bound_ratio(Y[:T], ref, bf16_ulp(ref) + 2 * (0.5 * x.abs() * ERF_ERR + EPS32 * ref.abs()))
+    ref, bound = gelu_ref(x)
+    r0 = bound_ratio(Y[:T], ref, bound)
     assert r0 <= 1.0, ('gelu', d, Tc, cap, r0)
     _check_tail(Y, T, T, 'gelu')
     gy = dY[:T].double()
-    ref = gy * _gelu_grad64(x)
-    t1 = 0.5 * (1 + torch.erf(x / 2 ** 0.5))
-    t2 = (x * torch.exp(-0.5 * x * x)).abs() / (2 * torch.pi) ** 0.5
-    err = gy.abs() * (ERF_ERR / 2 + (0.5 * x * x + 7) * EPS32 / 2 * t2 + EPS32 * (t1 + t2))
-    r1 = bound_ratio(dX[:T], ref, bf16_ulp(ref) + 2 * err)
+    ref, bound = gelu_bwd_ref(x, gy)
+    r1 = bound_ratio(dX[:T], ref, bound)
     assert r1 <= 1.0, ('gelu backward', d, Tc, cap, r1)
     _check_tail(dX, T, min(cap, _round(T)), 'gelu backward')
     ratio = [max(ratio[0], r0), max(ratio[1], r1)]
@@ -242,9 +228,8 @@ def _gate(native, d, Tc, cap, skip, mode, g):
   if mode is None:
     native.hgt_gate(A, X, out[:cap], sk, ctr, 3)
     torch.cuda.synchronize()
-    ref = sg * a + (1 - sg) * x
-    r = bound_ratio(out[:T], ref, bf16_ulp(ref) + 2 * (SIG_ERR * (a.abs() + x.abs()) +
-                                                      EPS32 * (sg * a.abs() + (1 - sg) * x.abs())))
+    ref, bound = gate_ref(a, x, sg)
+    r = bound_ratio(out[:T], ref, bound)
     assert r <= 1.0, ('gate', where, r)
     _check_tail(out, T, T, 'gate')
     return dict(r=r)
@@ -260,22 +245,20 @@ def _gate(native, d, Tc, cap, skip, mode, g):
                   skip_g=skip_g if with_sg else None)
   torch.cuda.synchronize()
   gz = dZ[:T].double()
-  ref = sg * gz
-  r = bound_ratio(out[:T], ref, bf16_ulp(ref) + 2 * (SIG_ERR + EPS32 * sg) * gz.abs())
+  ref, bound = gate_da_ref(gz, sg)
+  r = bound_ratio(out[:T], ref, bound)
   assert r <= 1.0, ('gate dA', where, r)
   _check_tail(out, T, min(cap, _round(T)), 'gate dA')
   if with_dx:
-    ref = dX0[:T].double() + (1 - sg) * gz
-    bound = SIG_ERR * gz.abs() + 2 * EPS32 * (dX0[:T].double().abs() + 2 * (1 - sg) * gz.abs())
+    ref, bound = gate_dx_ref(dX0[:T].double(), gz, sg)
     rx = bound_ratio(dX[:T], ref, bound)
     assert rx <= 1.0, ('gate dX', where, rx)
     r = max(r, rx)
   assert torch.equal(dX[T:] if with_dx else dX, dX0[T:] if with_dx else dX0), 'dX rows >= T are untouched'
   t = gz * (a - x)
   dsg = sg * (1 - sg)
-  ref_s = s0.double() + dsg * t.sum()
   # fp32 sum of T d terms onto s0, and sigma'(skip) within 2^-20 (two factors within SIG_ERR)
-  bound_s = (T * d + 2) * EPS32 * (dsg * t.abs().sum() + s0.double().abs()) + 2 * SIG_ERR * t.abs().sum()
+  ref_s, bound_s = skip_g_ref(s0, sg, t, T * d)
   if with_sg:
     rs = bound_ratio(skip_g, ref_s, bound_s)
     assert rs <= 1.0, ('skip_g', where, rs)
@@ -317,8 +300,7 @@ def test_hgt_blocks_match_block_diag(native, H):
       torch.cuda.synchronize()
       where = (H, heads, D, R)
       # att_img rows r H .. (r + 1) H: block h is att[r, h];  msg_img columns r H ..: block h is msg[r, h]^T
-      ref_a = torch.cat([torch.block_diag(*att[r]) for r in range(R)], 0)
-      ref_m = torch.cat([torch.block_diag(*msg[r].transpose(1, 2)) for r in range(R)], 1)
+      ref_a, ref_m = block_images(att, msg)
       assert torch.equal(att_img.view(torch.int16), ref_a.view(torch.int16)), ('att image', where)
       assert torch.equal(msg_img.view(torch.int16), ref_m.view(torch.int16)), ('msg image', where)
 
@@ -327,8 +309,7 @@ def test_hgt_blocks_match_block_diag(native, H):
       msg_g0 = torch.randn(R, heads, D, D, generator=g, device=DEV)
       att_d = torch.randn(R * H, H, generator=g, device=DEV)
       msg_d = torch.randn(H, R * H, generator=g, device=DEV)
-      blk_a = torch.diagonal(att_d.view(R, heads, D, heads, D), dim1=1, dim2=3).permute(0, 3, 1, 2)
-      blk_m = torch.diagonal(msg_d.view(heads, D, R, heads, D), dim1=0, dim2=3).permute(1, 3, 2, 0)
+      blk_a, blk_m = block_grads(att_d, msg_d, R, heads, D)
       exp_a, exp_m = att_g0 + blk_a, msg_g0 + blk_m               # one fp32 add, as in the kernel
       att_g, msg_g = att_g0.clone(), msg_g0.clone()
       att_img.fill_(SENTINEL)

@@ -16,7 +16,8 @@ import torch
 import torch.nn.functional as F
 
 import graphlearn_for_pytorch_b200 as glt
-from helpers import bf16_ulp, bound_ratio
+from helpers import (GAT_ISOLATED_EDGES, add_isolated_papers, bf16_ulp, bound_ratio, colsum_bound, gat_alpha_bound,
+                     gat_dscore_tol, gat_score_bound, score_bwd_bound, softmax_seg, weighted_sum_bound)
 
 pytestmark = pytest.mark.gpu
 DEV = torch.device('cuda', 0)
@@ -58,16 +59,6 @@ def _counters(vals):
   c = torch.zeros(16, dtype=torch.int32)
   c[:len(vals)] = torch.tensor(vals, dtype=torch.int32)
   return c.to(DEV)
-
-
-def _softmax_ref(e, tg, T):
-  """Segment softmax of e [E, heads] over the targets tg (float64)."""
-  heads = e.shape[1]
-  m = torch.full((T, heads), -float('inf'), dtype=e.dtype, device=DEV)
-  m = m.scatter_reduce(0, tg.unsqueeze(1).expand(-1, heads), e, 'amax', include_self=True)
-  ex = torch.exp(e - m[tg])
-  den = torch.zeros(T, heads, dtype=e.dtype, device=DEV).index_add_(0, tg, ex)
-  return ex / den[tg]
 
 
 # (heads, C): H = heads * C from 64 to 1024, C in {8, 16, 24, 48, 128, 256}.  Up to 8 heads a lane owns at most one
@@ -116,10 +107,10 @@ def test_gat_kernels_match_fp64(native, heads, C, scores):
   # scores: fp32 dot of C terms
   for got, ref, P, att in ((as_, a_s, Psd, asd_), (ad[:T], a_d, Pdd, add_)):
     ab = (P.detach().abs().view(-1, heads, C) * att.detach().abs().view(heads, C)).sum(-1)
-    assert bound_ratio(got, ref.detach(), (C + 2) * EPS32 * ab + 1e-30) <= 1.0
+    assert bound_ratio(got, ref.detach(), gat_score_bound(ab, C)) <= 1.0
   raw = a_s[sr] + a_d[tg]
   e = F.leaky_relu(raw, 0.2)
-  al = _softmax_ref(e, tg, T)
+  al = softmax_seg(e, tg, T)
   out = torch.zeros(T, H, dtype=torch.float64, device=DEV).index_add_(
       0, tg, (al.unsqueeze(-1) * Psd[sr].view(-1, heads, C)).view(-1, H))
   # alpha: relative error of the fp32 exp of (score - max), |score| * 2^-22 with margin
@@ -127,13 +118,13 @@ def test_gat_kernels_match_fp64(native, heads, C, scores):
            for h, (rows, k) in enumerate(HOPS)]
   ga = torch.cat([alpha[h].view(rows, k, heads)[kmask[h].to(DEV)] for h, (rows, k) in enumerate(HOPS)], 0)
   emax = float(e.detach().abs().max()) + 1.0
-  assert bound_ratio(ga.abs(), al.detach(), 64 * EPS32 * emax * al.detach() + 1e-30) <= 1.0
+  assert bound_ratio(ga.abs(), al.detach(), gat_alpha_bound(al.detach(), emax)) <= 1.0
   assert bool(((ga < 0) | ((ga == 0) & torch.signbit(ga))).eq(raw.detach() <= 0).all()), 'sign bit of alpha'
   # output: one bf16 rounding of an fp32 sum of deg weighted terms
   ab = torch.zeros(T, H, dtype=torch.float64, device=DEV).index_add_(
       0, tg, (al.detach().unsqueeze(-1) * Psd.detach()[sr].abs().view(-1, heads, C)).view(-1, H))
   kd = deg.to(DEV).double().unsqueeze(1)
-  bound = bf16_ulp(out.detach()) + (kd + 2 + 64 * emax) * EPS32 * ab
+  bound = weighted_sum_bound(out.detach(), ab, kd, arel=64 * EPS32 * emax)
   assert bound_ratio(Z[:T], out.detach(), bound) <= 1.0
   assert bool((Z[0] == 0).all())                          # degree-0 row without bias: exactly zero
 
@@ -159,7 +150,7 @@ def test_gat_kernels_match_fp64(native, heads, C, scores):
   dalpha_abs = (Gd[tg].abs().view(-1, heads, C) * Psd.detach()[sr].abs().view(-1, heads, C)).sum(-1)
   sabs = torch.zeros(T, heads, dtype=torch.float64, device=DEV).index_add_(0, tg, al.detach() * dalpha_abs)
   term = al.detach() * (dalpha_abs + sabs[tg])
-  tol = (C + 64 * emax + 600) * EPS32
+  tol = gat_dscore_tol(C, emax, 600)
   ds_abs_src = torch.zeros(N_SRC, heads, dtype=torch.float64, device=DEV).index_add_(0, sr, term)
   ds_abs_dst = torch.zeros(T, heads, dtype=torch.float64, device=DEV).index_add_(0, tg, term)
   assert bound_ratio(da_src_k, a_s.grad, tol * ds_abs_src + 1e-30) <= 1.0
@@ -205,12 +196,13 @@ def test_gat_score_bwd_folded_destination(native, heads, C):
   torch.cuda.synchronize()
   terms = dP.double().abs() + (da_s.double().abs().unsqueeze(-1) * att_s.double().abs().view(heads, C)).view(n, H)
   terms[:T] += (da_d.double().abs().unsqueeze(-1) * att_d.double().abs().view(heads, C)).view(T, H)
-  assert bound_ratio(out[:n], ref, bf16_ulp(ref) + 4 * EPS32 * terms + 1e-30) <= 1.0
+  assert bound_ratio(out[:n], ref, score_bwd_bound(ref, terms)) <= 1.0
   assert bool((out[n:] == 0).all())
   ab_s = (da_s.double().abs().unsqueeze(-1) * P.double().abs().view(n, heads, C)).view(n, H).sum(0)
   ab_d = (da_d.double().abs().unsqueeze(-1) * P[:T].double().abs().view(T, heads, C)).view(T, H).sum(0)
-  assert bound_ratio(g_as, gs, (n + 2) * EPS32 * ab_s + 1e-30) <= 1.0
-  assert bound_ratio(g_ad, gd, (T + 2) * EPS32 * ab_d + 1e-30) <= 1.0
+  zero = torch.zeros(H, device=DEV)
+  assert bound_ratio(g_as, gs, colsum_bound(ab_s.unsqueeze(0), zero, n) + 1e-30) <= 1.0
+  assert bound_ratio(g_ad, gd, colsum_bound(ab_d.unsqueeze(0), zero, T) + 1e-30) <= 1.0
 
 
 @pytest.mark.parametrize('H,heads', [(64, 1), (192, 4), (1024, 8)])
@@ -241,13 +233,7 @@ def _build(feat_dim=64, hidden=64, heads=4, classes=19, dropout=0.0, fan=(4, 3, 
   from graphlearn_for_pytorch_b200.models import HeteroGatEngine
   edges, feats, labels, sizes = synthetic_igbh(papers, papers // 2, 50, 30, feat_dim=64, num_classes=classes, seed=2)
   g = torch.Generator().manual_seed(3)
-  n_old = sizes['paper']
-  new = torch.arange(n_old, n_old + ISOLATED)
-  cites_new = torch.stack([new.repeat_interleave(4), torch.randint(0, n_old, (4 * ISOLATED,), generator=g)])
-  wrote_new = torch.stack([new.repeat_interleave(3), torch.randint(0, sizes['author'], (3 * ISOLATED,), generator=g)])
-  edges[('paper', 'cites', 'paper')] = torch.cat([edges[('paper', 'cites', 'paper')], cites_new], 1)
-  edges[('paper', 'written_by', 'author')] = torch.cat([edges[('paper', 'written_by', 'author')], wrote_new], 1)
-  sizes['paper'] = n_old + ISOLATED
+  add_isolated_papers(edges, sizes, ISOLATED, g, GAT_ISOLATED_EDGES)
   labels = {'paper': torch.cat([labels['paper'], torch.randint(0, classes, (ISOLATED,), generator=g)])}
   dims = feat_dim if isinstance(feat_dim, dict) else {t: feat_dim for t in sizes}
   feats = {t: torch.randn(sizes[t], dims[t], generator=g) for t in sizes}

@@ -19,7 +19,8 @@ import torch
 import torch.nn.functional as F
 
 import graphlearn_for_pytorch_b200 as glt
-from helpers import bf16_ulp, bound_ratio
+from helpers import (add_isolated_papers, bf16_ulp, bound_ratio, hgt_alpha_rel, hgt_bwd_tol, hgt_score_err,
+                     weighted_sum_bound)
 
 pytestmark = pytest.mark.gpu
 DEV = torch.device('cuda', 0)
@@ -157,13 +158,10 @@ def _attention_case(native, heads, D, R, scores):
     slot = E[r][2]
     ga.append(torch.cat([alpha[r][h].view(rows, FANS[r][h], heads)[slot[h].to(DEV)] for h, rows in enumerate(ROWS)]))
   ga = torch.cat(ga)
-  emax = float(s_all.detach().abs().max()) + 1.0
   # score error: an fp32 dot of D terms times prior / sqrt(D), relative to the sum of |terms|
   pr_abs = torch.cat([pd[r].detach().abs().expand(len(tgs[r]), heads) for r in range(R)])
-  serr = (D + 4) * EPS32 * torch.cat(cabs) * pr_abs + 4 * EPS32 * s_all.detach().abs()
-  serr_row = torch.zeros(T, heads, dtype=torch.float64, device=DEV).scatter_reduce(
-      0, tg_all.unsqueeze(1).expand(-1, heads), serr, 'amax', include_self=True)
-  arel = 64 * EPS32 * emax + 2 * serr_row[tg_all]
+  serr = hgt_score_err(torch.cat(cabs), pr_abs, s_all.detach(), D)
+  arel = hgt_alpha_rel(s_all.detach(), serr, tg_all, T)
   assert bound_ratio(ga, al.detach(), arel * al.detach() + 1e-30) <= 1.0
   # the softmax spans every relation: alpha sums to one per (row, head) over all of them (zero for isolated rows)
   tot = torch.zeros(T, heads, dtype=torch.float64, device=DEV).index_add(0, tg_all, ga.double())
@@ -187,7 +185,7 @@ def _attention_case(native, heads, D, R, scores):
   arel_col = arel_row.repeat_interleave(D, 1).repeat(1, R)
   # (+ 2^-120 kd max|v|: alphas below fp32's normal range lose their precision, the float64 reference keeps it)
   vmax = max(float(x[:, 2 * H:].abs().max()) for x in kv)
-  bound = bf16_ulp(out.detach()) + ((kd + 2) * EPS32 + arel_col) * ab + 2.0 ** -120 * kd * vmax
+  bound = weighted_sum_bound(out.detach(), ab, kd, arel=arel_col, floor=2.0 ** -120 * kd * vmax)
   assert bound_ratio(U[:T], out.detach(), bound) <= 1.0
   assert bool((U[:T][~covered] == 0).all()), 'a row without any neighbour aggregates nothing'
 
@@ -212,7 +210,7 @@ def _attention_case(native, heads, D, R, scores):
   dabs = torch.cat(dabs)
   sabs = torch.zeros(T, heads, dtype=torch.float64, device=DEV).index_add(0, tg_all, al.detach() * dabs)
   term = al.detach() * (dabs + sabs[tg_all])
-  tol = (kd.max().item() + D + 600) * EPS32 + float(arel.max())
+  tol = hgt_bwd_tol(D, kd.max().item() + 600, float(arel.max()))
   terms = list(torch.split(term, [len(t) for t in tgs]))
   for r in range(R):
     tg, sr, _ = E[r]
@@ -265,14 +263,7 @@ def _build(schema='mag', feat_dim=64, hidden=64, heads=2, classes=20, fan=(4, 3)
   else:
     edges, _, labels, sizes = synthetic_igbh(papers, papers // 2, 50, 30, feat_dim=8, num_classes=classes, seed=2)
   g = torch.Generator().manual_seed(3)
-  n_old = sizes['paper']
-  new = torch.arange(n_old, n_old + ISOLATED)
-  for et in list(edges):
-    if et[0] == 'paper':
-      n_dst = n_old if et[2] == 'paper' else sizes[et[2]]
-      extra = torch.stack([new.repeat_interleave(3), torch.randint(0, n_dst, (3 * ISOLATED,), generator=g)])
-      edges[et] = torch.cat([edges[et], extra], 1)
-  sizes['paper'] = n_old + ISOLATED
+  add_isolated_papers(edges, sizes, ISOLATED, g, {et: 3 for et in edges if et[0] == 'paper'})
   labels = torch.randint(0, classes, (sizes['paper'],), generator=g)
   dims = feat_dim if isinstance(feat_dim, dict) else {t: feat_dim for t in sizes}
   feats = {t: torch.randn(sizes[t], dims[t], generator=g) for t in sizes}

@@ -30,150 +30,14 @@ import graphlearn_for_pytorch_b200 as glt
 from graphlearn_for_pytorch_b200.data import dequantize_mxfp8, quantize_mxfp8
 from graphlearn_for_pytorch_b200.models import GraphSageEngine, GraphSageLinkEngine, HeteroSageEngine
 from graphlearn_for_pytorch_b200.utils.synthetic import rmat_edges
-from helpers import bf16_ulp, bound_ratio, colsum_ratio, gather_ref, gemm_bound, mean_ref, sum_bound
+from helpers import (Ratios, _batches, _check_adam, _check_grads, _check_linear, _check_softmax, _ell_edges, _f32,
+                     _snapshot, _table, _wgrad_ratio, bound_ratio, colsum_ratio, gather_ref, mean_ref, sum_bound)
 
 pytestmark = pytest.mark.gpu
 DEV = torch.device('cuda', 0)
-U = 2.0 ** -24
-
-
-class Ratios(object):
-  """Worst error / bound per stage of one step; `check` asserts each ratio <= 1 as it is recorded."""
-
-  def __init__(self, tag):
-    self.tag, self.r = tag, {}
-
-  def check(self, stage, ratio):
-    self.r[stage] = max(self.r.get(stage, 0.0), ratio)
-    assert ratio <= 1.0, f'{self.tag}: {stage} error / bound = {ratio}'
-
-  def exact(self, stage, ok):
-    self.check(stage, 0.0 if ok else float('inf'))
-
-  def show(self):
-    print(f'{self.tag}: ' + ', '.join(f'{k} {v:.3f}' for k, v in self.r.items()))
-
-
-def _f32(x):
-  return float(torch.tensor(x, dtype=torch.float32))
-
-
-def _batches(bs, N, g):
-  """Seed batches of bs, about bs / 3, 1 and bs nodes (the small ones padded with -1 by train_step)."""
-  return [torch.randperm(N, generator=g)[:n].to(DEV) for n in (bs, max(1, bs // 3), 1, bs)]
-
-
-def _ell_edges(ell_of, deg, ctr, nh, caps, ks):
-  """(target, source) of the ELL hops 0..nh-1: frontier rows of hop h are [ctr[h], ctr[h+1]) clamped to the hop's
-  capacity, slots inside the row's degree, sources >= 0.  A hop of fan-out 0 has no ELL block; its rows must have
-  degree 0."""
-  tg, sr = [], []
-  for h in range(nh):
-    k = ks[h]
-    n = max(0, min(ctr[h + 1] - ctr[h], caps[h]))
-    if n == 0:
-      continue
-    if k == 0:
-      assert not bool(deg[ctr[h]:ctr[h] + n].any()), f'rows of hop {h} (fan-out 0) must have degree 0'
-      continue
-    e = ell_of(h).view(-1, k)[:n].long()
-    m = (torch.arange(k, device=DEV).unsqueeze(0) < deg[ctr[h]:ctr[h] + n].long().unsqueeze(1)) & (e >= 0)
-    tg.append((torch.arange(n, device=DEV).unsqueeze(1) + ctr[h]).expand(n, k)[m])
-    sr.append(e[m])
-  empty = torch.zeros(0, dtype=torch.int64, device=DEV)
-  return torch.cat(tg + [empty]), torch.cat(sr + [empty])
 
 
 # --------------------------------------------------------------------------- stages shared by the engines
-def _check_linear(R, stage, A, W, b, Z, T, relu, keep=None, scale=1.0):
-  """Z[:T] against bf16(act(A W^T + b)) (then inverted dropout with mask `keep`)."""
-  Ad, Wd = A[:T].double(), W.double()
-  ref = Ad @ Wd.t() + b.double()
-  bound = gemm_bound(ref, Ad.abs() @ Wd.abs().t() + b.double().abs(), A.shape[1])
-  if relu:
-    ref = ref.clamp(min=0)
-  if keep is not None:
-    ref = torch.where(keep, ref * scale, torch.zeros_like(ref))
-    bound = torch.where(keep, bound * scale + bf16_ulp(ref), torch.zeros_like(ref))
-  R.check(stage, bound_ratio(Z[:T], ref, bound))
-
-
-def _wgrad_ratio(gW, dPre, A, T):
-  Pd, Ad = dPre[:T].double(), A[:T].double()
-  return bound_ratio(gW, Pd.t() @ Ad, gemm_bound(None, Pd.abs().t() @ Ad.abs(), T, bf16_out=False))
-
-
-def _check_grads(R, stage, gW, dPre, A, W, dA, T):
-  """dW = dPre[:T]^T A[:T] (split-K fp32) and, when dA is given, dA[:T] = bf16(dPre[:T] W)."""
-  R.check(f'dW{stage}', _wgrad_ratio(gW, dPre, A, T))
-  if dA is not None:
-    Pd, Wd = dPre[:T].double(), W.double()
-    ref = Pd @ Wd
-    R.check(f'dA{stage}', bound_ratio(dA[:T], ref, gemm_bound(ref, Pd.abs() @ Wd.abs(), W.shape[0])))
-
-
-def _check_softmax(R, Z, C, labels, nodes, n0, dPre, bias_grad, loss, correct):
-  xs = Z[:n0, :C].double()
-  lab = labels[nodes[:n0]]
-  ref_loss = F.cross_entropy(xs, lab)
-  R.check('loss', abs(loss.item() - ref_loss.item()) / (1e-4 * max(1.0, ref_loss.item())))
-  mx = xs.max(1, keepdim=True).values
-  first = torch.where(xs == mx, torch.arange(C, device=DEV), C).min(1).values
-  R.exact('correct', int(correct.item()) == int((first == lab).sum()))
-  ref = (torch.softmax(xs, 1) - F.one_hot(lab, C).double()) / n0
-  R.check('dlogits', bound_ratio(dPre[:n0, :C], ref, bf16_ulp(ref) + 1e-4 / n0))
-  R.exact('dlogits pad', bool((dPre[:n0, C:] == 0).all()))
-  R.check('db_last', colsum_ratio(bias_grad, dPre, n0))
-
-
-def _adam_ref(p, g, m, v, t, lr, wd, b1=0.9, b2=0.999, eps=1e-8):
-  """float64 torch.optim.Adam(weight_decay=wd) update from fp32 state, with the fp32 constants the kernel receives,
-  and the bounds of its fp32 evaluation: 2u per rounded sum of products, one u for each bias correction."""
-  lr, wd, b1, b2, eps = (_f32(x) for x in (lr, wd, b1, b2, eps))
-  p, g, m, v = p.double(), g.double(), m.double(), v.double()
-  gi = g + wd * p
-  e_g = 2 * U * (g.abs() + (wd * p).abs())
-  m1 = b1 * m + (1 - b1) * gi
-  v1 = b2 * v + (1 - b2) * gi * gi
-  e_m = 2 * U * (b1 * m.abs() + (1 - b1) * gi.abs()) + (1 - b1) * e_g
-  e_v = 3 * U * (b2 * v + (1 - b2) * gi * gi) + (1 - b2) * 2 * gi.abs() * e_g
-  c1, c2 = 1 - b1 ** t, 1 - b2 ** t
-  M, V = m1 / c1, v1 / c2
-  dM = e_m / c1 + M.abs() * 2 * U
-  dV = e_v / c2 + V * 2 * U
-  S = V.sqrt()
-  dS = torch.minimum(dV.sqrt(), dV / (2 * S).clamp(min=1e-300)) + U * S
-  D = S + eps
-  upd = M / D
-  dU = dM / D + M.abs() * (dS + U * D) / (D * D) + U * upd.abs()
-  p1 = p - lr * upd
-  dP = lr * dU + 2 * U * (lr * upd.abs() + p1.abs())
-  return (p1, m1, v1), (dP, e_m, e_v)
-
-
-def _check_adam(R, eng, snap, wd, controls=False):
-  t = int(snap['step'][0]) + 1
-  (p1, m1, v1), (bp, bm, bv) = _adam_ref(snap['p32'], eng.g32, snap['m'], snap['v'], t, eng.lr, wd)
-  R.check('adam p', bound_ratio(eng.p32, p1, bp))
-  R.check('adam m', bound_ratio(eng.m, m1, bm))
-  R.check('adam v', bound_ratio(eng.v, v1, bv))
-  R.exact('p16', torch.equal(eng.p16.view(torch.int16), eng.p32.to(torch.bfloat16).view(torch.int16)))
-  R.exact('step_dev', eng.step_dev.tolist() == [t, 0])
-  if controls:
-    # the same check rejects Adam without weight decay and Adam with t off by one
-    (q, _, _), _ = _adam_ref(snap['p32'], eng.g32, snap['m'], snap['v'], t, eng.lr, 0.0)
-    assert bound_ratio(q.float(), p1, bp) > 1.0, 'the Adam check must reject an update without weight decay'
-    (q, _, _), _ = _adam_ref(snap['p32'], eng.g32, snap['m'], snap['v'], t + 1, eng.lr, wd)
-    assert bound_ratio(q.float(), p1, bp) > 1.0, 'the Adam check must reject an update with t off by one'
-
-
-def _snapshot(eng, dpre):
-  s = {k: getattr(eng, k).clone() for k in ('p32', 'p16', 'm', 'v')}
-  s['step'] = eng.step_dev.clone()
-  s['dPre'] = dpre()
-  return s
-
-
 # --------------------------------------------------------------------------- GraphSageEngine / GraphSageLinkEngine
 def _sage_stages(R, eng, snap, parity, X, Xself, labels, controls):
   """Every stage of the step that trained arena `parity`.  X: fp32/bf16 feature table indexed by global id (the
@@ -283,12 +147,6 @@ def _sage_graph(N, E, seed):
   ei = torch.cat([ei, ei.flip(0)], 1)
   topo = glt.data.Topology(ei, layout='CSR', num_nodes=N)
   return topo, glt.data.Graph(topo, 'CUDA', 0)
-
-
-def _table(x):
-  ut = glt.data.UnifiedTensor(0, x.dtype)
-  ut.append_shared_tensor(x)
-  return ut
 
 
 SAGE_CASES = {
