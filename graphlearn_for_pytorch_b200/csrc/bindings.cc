@@ -2063,6 +2063,31 @@ static void softmax_nll(const Tensor& logits, int64_t C, const c10::optional<Ten
   check_cuda_err("softmax_nll");
 }
 
+static void sigmoid_bce(const Tensor& logits, int64_t T, const Tensor& label_bits, const Tensor& nodes,
+                        const Tensor& counters, Tensor loss, Tensor dlogits, const c10::optional<Tensor>& counts,
+                        const c10::optional<Tensor>& colsum, bool prezeroed) {
+  c10::cuda::CUDAGuard guard(logits.device());
+  TORCH_CHECK(logits.dim() == 2 && logits.size(1) % 8 == 0 && 1 <= T && T <= logits.size(1),
+              "sigmoid_bce: logits must be [rows, ld] with ld a multiple of 8 and 1 <= T <= ld");
+  check_rows(logits, torch::kBFloat16, logits.size(1), "sigmoid_bce: logits must be contiguous bf16 [rows, ld]");
+  check_rows(dlogits, torch::kBFloat16, logits.size(1), "sigmoid_bce: dlogits must be contiguous bf16 of logits' shape");
+  TORCH_CHECK(dlogits.size(0) == logits.size(0), "sigmoid_bce: dlogits must be contiguous bf16 of logits' shape");
+  TORCH_CHECK(on_dev(label_bits) && label_bits.scalar_type() == torch::kUInt32 && label_bits.dim() == 2 &&
+                  label_bits.size(1) == (T + 31) / 32 && label_bits.is_contiguous(),
+              "sigmoid_bce: label_bits must be contiguous uint32 [num_nodes, ceil(T / 32)] on the device");
+  check_ids(nodes, "sigmoid_bce: nodes must be contiguous int64 on the device");
+  TORCH_CHECK(nodes.numel() >= logits.size(0), "sigmoid_bce: nodes must hold an id for every row of logits");
+  check_counters(counters, 1, "sigmoid_bce: counters must be int32 [> 1] on the device");
+  TORCH_CHECK(on_dev(loss) && loss.scalar_type() == torch::kFloat32 && loss.numel() >= 1,
+              "sigmoid_bce: loss must be fp32 [>= 1] on the device");
+  if (has(counts)) check_counters(*counts, 2, "sigmoid_bce: counts must be int32 [>= 3] on the device");
+  if (has(colsum)) check_vec(*colsum, torch::kFloat32, logits.size(1), "sigmoid_bce: colsum must be fp32 [ld]");
+  launch_sigmoid_bce(logits.data_ptr(), logits.size(1), T, static_cast<const uint32_t*>(label_bits.data_ptr()), label_bits.size(0),
+                     nodes.data_ptr<int64_t>(), counters.data_ptr<int32_t>(), logits.size(0), loss.data_ptr<float>(),
+                     dlogits.data_ptr(), opt_ptr<int32_t>(counts), opt_ptr<float>(colsum), cur_stream(), prezeroed);
+  check_cuda_err("sigmoid_bce");
+}
+
 // (kernel, memset, memcpy) node counts of a captured CUDA graph: the launches one replay makes.  `raw_graph` is the
 // cudaGraph_t of torch.cuda.CUDAGraph(keep_graph=True).raw_cuda_graph().
 static std::tuple<int64_t, int64_t, int64_t> graph_node_counts(int64_t raw_graph) {
@@ -2684,6 +2709,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("softmax_nll", &softmax_nll, py::arg("logits"), py::arg("C"), py::arg("y"), py::arg("labels_all"),
         py::arg("nodes"), py::arg("counters"), py::arg("loss"), py::arg("dlogits"), py::arg("correct"),
         py::arg("colsum"), py::arg("prezeroed") = false);
+  m.def("sigmoid_bce", &sigmoid_bce, py::arg("logits"), py::arg("T"), py::arg("label_bits"), py::arg("nodes"),
+        py::arg("counters"), py::arg("loss"), py::arg("dlogits"), py::arg("counts") = py::none(),
+        py::arg("colsum") = py::none(), py::arg("prezeroed") = false);
   m.def("adam_step", &adam_step);
   m.def("colsum_bf16", &colsum_bf16);
   m.def("zero_rows", &zero_rows);

@@ -306,11 +306,24 @@ void launch_softmax_nll(const void* logits, int ld, int C, const int64_t* y, con
 // out[c] = sum over valid rows of X[:, c]  (d multiple of 8)
 void launch_colsum_bf16(const void* X, const int32_t* cum, int n_hops, int cap, int d, float* out,
                         cudaStream_t s);
+// launch_colsum_bf16 without the memset: accumulates onto `out`
+void launch_colsum_accum(const void* X, const int32_t* cum, int n_hops, int cap, int d, float* out,
+                         cudaStream_t s);
 void launch_zero_rows(float* p, const int32_t* cum, int n_hops, int cap, int d, cudaStream_t s);
 // flat fp32 Adam over [n] with bf16 shadow copy refresh.
 void launch_adam(float* p, const float* g, float* m, float* v, void* p_bf16, int64_t n, float lr,
                  float b1, float b2, float eps, float wd, int32_t* step_dev, float gscale,
                  cudaStream_t s);
+
+// ---- multilabel.cu (multi-label node classification loss) --------------------------------------------------------
+// loss = mean over rows r < n0 = min(cum[1], cap) and tasks c < T of BCE-with-logits(logits[r, c], y[r, c]), with
+// y[r, c] = bit c & 31 of bits[nodes[r] * W + (c >> 5)], W = ceil(T / 32) (an id outside [0, n_nodes): all zeros);
+// dlogits = (sigmoid - y) / (n0 T), zero in columns [T, ld) and rows [n0, cap).  counts (optional, int32 [3]) +=
+// (TP, FP, FN) at logit 0.  colsum (optional, fp32 [ld]): bias gradient = column sums of the bf16 dlogits, fused for
+// ld <= 256, a second column-sum kernel otherwise.  prezeroed: loss, counts and colsum were zeroed by the caller.
+void launch_sigmoid_bce(const void* logits, int ld, int T, const uint32_t* bits, int64_t n_nodes,
+                        const int64_t* nodes, const int32_t* cum, int cap, float* loss, void* dlogits,
+                        int32_t* counts, float* colsum, cudaStream_t s, bool prezeroed = false);
 
 // ---- link.cu (link-prediction step: in-graph negatives + fused edge loss) --------
 // pos: int64 [2, B] positive pairs (-1 = padding).  Writes seeds [2P], P = (1 + k) B: seeds[p] = source and

@@ -453,8 +453,8 @@ void launch_dropout_bf16(void* Z, const int32_t* cum, int n_hops, int cap, int d
 }
 
 // Accumulates the column sums of the first min(cum[n_hops], cap) rows of X into `out` (not zeroed here).
-static void launch_colsum_accum(const void* X, const int32_t* cum, int n_hops, int cap, int d, float* out,
-                                cudaStream_t s) {
+void launch_colsum_accum(const void* X, const int32_t* cum, int n_hops, int cap, int d, float* out,
+                         cudaStream_t s) {
   const int groups = d / 8;
   const int rpb = 256 / groups > 0 ? 256 / groups : 1;
   const size_t smem = groups <= 256 ? sizeof(float) * rpb * d : 0;

@@ -1,6 +1,7 @@
 from .sage import SAGEConv, GraphSAGE, GraphSageEngine
 from .sage_link import GraphSageLinkEngine, link_auc
-from .trainer import GraphSageTrainer, GraphSageLinkTrainer
+from .sage_multilabel import GraphSageMultiLabelEngine, multilabel_auc, multilabel_f1, pack_label_bits
+from .trainer import GraphSageTrainer, GraphSageMultiLabelTrainer, GraphSageLinkTrainer
 from .rgnn import RGNN, RelSAGEConv, RelGCNConv, RelGATConv
 from .seal import drnl_node_labeling, DGCNN
 from .hgt import HGT, HGTConv

@@ -1,5 +1,5 @@
-"""`GraphSageTrainer` / `GraphSageLinkTrainer`: the device-agnostic counterparts of `GraphSageEngine` /
-`GraphSageLinkEngine`.
+"""`GraphSageTrainer` / `GraphSageMultiLabelTrainer` / `GraphSageLinkTrainer`: the device-agnostic counterparts of
+`GraphSageEngine` / `GraphSageMultiLabelEngine` / `GraphSageLinkEngine`.
 
 Same step-level API (`train_step(seeds)`, `evaluate_batch(seeds)`, `state_dict()` / `load_state_dict()`), built
 from the public pieces -- `NeighborSampler`, `Feature`, the eager `GraphSAGE` module and `torch.optim.Adam` -- so it
@@ -17,6 +17,7 @@ import torch.nn.functional as F
 
 from ..sampler import EdgeSamplerInput, NegativeSampling, NeighborSampler, NodeSamplerInput
 from .sage import GraphSAGE
+from .sage_multilabel import check_multilabel
 
 
 @torch.no_grad()
@@ -73,13 +74,16 @@ class GraphSageTrainer(object):
     self.model.train()
     x, ei, nn_, ne_, y, n = self._batch(seeds)
     logits = self.model(x, ei, nn_, ne_)[:n]
-    loss = F.cross_entropy(logits, y)
+    loss = self._loss(logits, y)
     self.opt.zero_grad(set_to_none=True)
     loss.backward()
     self.opt.step()
     self.step_idx += 1
     self.loss = loss.detach()
     return self.loss
+
+  def _loss(self, logits: torch.Tensor, y: torch.Tensor) -> torch.Tensor:
+    return F.cross_entropy(logits, y)
 
   @torch.no_grad()
   def evaluate_batch(self, seeds: torch.Tensor):
@@ -114,6 +118,32 @@ class GraphSageTrainer(object):
     self.step_idx = int(s.get('step', 0))
     if 'sampler' in s and hasattr(self.sampler, 'load_state_dict'):
       self.sampler.load_state_dict(s['sampler'])
+
+
+class GraphSageMultiLabelTrainer(GraphSageTrainer):
+  """Device-agnostic counterpart of `GraphSageMultiLabelEngine` (same step-level API): `labels` is a [N, T] tensor of
+  0/1 values, the loss the mean `F.binary_cross_entropy_with_logits` over the batch's seeds and tasks.  Runs on a CPU as
+  well as on any GPU, and is the semantic reference of the engine."""
+
+  def __init__(self, graph, features, labels: torch.Tensor, in_dim: int, fanouts: List[int] = (15, 10, 5),
+               hidden: int = 256, lr: float = 3e-3, weight_decay: float = 0.0, seed: int = 0,
+               device: Optional[torch.device] = None):
+    T = check_multilabel(labels)
+    super().__init__(graph, features, labels.float(), in_dim, fanouts=fanouts, hidden=hidden, num_classes=T, lr=lr,
+                     weight_decay=weight_decay, seed=seed, device=device)
+
+  def _loss(self, logits: torch.Tensor, y: torch.Tensor) -> torch.Tensor:
+    return F.binary_cross_entropy_with_logits(logits, y)
+
+  @torch.no_grad()
+  def evaluate_batch(self, seeds: torch.Tensor):
+    """(loss, TP, FP, FN, #seeds) without updating parameters, as GraphSageMultiLabelEngine.evaluate_batch."""
+    self.model.eval()
+    x, ei, nn_, ne_, y, n = self._batch(seeds)
+    logits = self.model(x, ei, nn_, ne_)[:n]
+    pred, yb = logits > 0, y.bool()
+    return (float(self._loss(logits, y)), int((pred & yb).sum()), int((pred & ~yb).sum()), int((~pred & yb).sum()),
+            int(n))
 
 
 class GraphSageLinkTrainer(object):

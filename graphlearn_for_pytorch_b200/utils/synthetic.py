@@ -55,6 +55,23 @@ def id_features(num_nodes: int, dim: int = 16, dtype=torch.float32) -> torch.Ten
   return torch.arange(num_nodes, dtype=dtype).unsqueeze(1).repeat(1, dim)
 
 
+def multilabel_targets(edge_index: torch.Tensor, x: torch.Tensor, num_tasks: int, seed: int = 0) -> torch.Tensor:
+  """Learnable multi-label targets, bool [N, num_tasks]: task t of node v is positive when a random projection w_t of
+  the mean feature row of v's neighbours (edge_index[1] of the edges out of v) is in its top r_t fraction, r_t uniform
+  in [0.1, 0.5).  A node without neighbours averages to zero."""
+  n = x.shape[0]
+  g = torch.Generator().manual_seed(seed)
+  src, dst = edge_index[0].long(), edge_index[1].long()
+  xf = x.float()
+  agg = torch.zeros_like(xf).index_add_(0, src, xf[dst])
+  deg = torch.bincount(src, minlength=n).clamp(min=1).to(xf.dtype)
+  proj = (agg / deg.unsqueeze(1)) @ torch.randn(x.shape[1], num_tasks, generator=g).to(x.device)
+  rate = 0.1 + 0.4 * torch.rand(num_tasks, generator=g).to(x.device)
+  k = ((1 - rate) * (n - 1)).long()
+  thresh = proj.sort(0).values.gather(0, k.unsqueeze(0))
+  return proj > thresh
+
+
 def synthetic_dataset_tensors(name: str = 'tiny', seed: int = 0, device='cpu',
                               feat_dtype=torch.float32, pad_to: Optional[int] = None,
                               scale_edges: float = 1.0):
