@@ -696,10 +696,10 @@ size_t tc_gemm_smem_bytes();
 // ---- hetero_infer.cu (full-neighbourhood attention of the heterogeneous engines' layer-wise inference) ----------
 // Both kernels walk the COMPLETE CSR row of every target r in [r0, r1) (global ids of the destination type; rows of the
 // relation graph are targets, columns are global source ids, ids outside [0, n_src) are skipped).  A row is reduced by
-// one lane group, or, above kHeteroHubDeg neighbours (HGT: summed over its relations), by the whole CTA with per-group
-// partials merged in group order.  The path depends on the degree alone, so every row has one fixed reduction order:
-// no floating-point atomics, bitwise identical for any chunking.  Every exp is of a score minus its row maximum.
-constexpr int kHeteroHubDeg = 256;
+// one lane group, or, above kFullRowHubDeg neighbours (full_rows.cuh; HGT: summed over its relations), by the whole CTA
+// with per-group partials merged in group order.  The path depends on the degree alone, so every row has one fixed
+// reduction order: no floating-point atomics, bitwise identical for any chunking.  Every exp is of a score minus its row
+// maximum.
 
 // R-GAT, one relation r = (s -> t):  e_ij,h = leaky_relu(as[j, h] + ad[i, h], 0.2),  alpha = softmax over i's complete
 // in-row per head,  out_i = concat_h sum_j alpha_ij,h P[j, h-block]  (fp32).  first / last as in GatAggArgs:

@@ -3,22 +3,17 @@
 // sampled kernels in gat.cu / hgt.cu), for a chunk [r0, r1) of global target ids.
 //
 // Lane-group layout of the sampled siblings: LPR lanes per row, a lane owns VPL 16-byte vectors (columns c * 8 ..
-// c * 8 + 7, c = v * LPR + lane) of an H-wide row.  Degrees are power-law, so a row above kHeteroHubDeg neighbours is
-// not walked by one group while the rest of the GPU idles: the whole CTA splits it (group g takes neighbours g, g + G,
-// ...) and the G partials are merged in group order in shared memory.  Which path a row takes depends on its degree
-// alone, and no floating-point atomics are used, so every row has one fixed reduction order: results are bitwise
-// identical from call to call and for any chunking.  No exp is ever taken of a score that is not shifted by the
-// maximum it is normalised against.
+// c * 8 + 7, c = v * LPR + lane) of an H-wide row.  Rows follow the schedule of full_rows.cuh (hub rows split over the
+// CTA, partials merged in group order), so every row has one fixed reduction order: results are bitwise identical from
+// call to call and for any chunking.  No exp is ever taken of a score that is not shifted by the maximum it is
+// normalised against.
 #include <cmath>
 
-#include "device_utils.cuh"
-#include "launch_utils.h"
+#include "full_rows.cuh"
 
 namespace glt {
 
 namespace {
-
-constexpr int kThreads = 256;
 
 // ------------------------------------------------------------------------------------------------------ R-GAT
 // Scores are per node (as, ad), so both passes over a row read scalars; only pass 2 reads the projection rows.
@@ -108,23 +103,19 @@ struct GatFull {
   }
 };
 
-// One row per lane group (G = 256 / LPR rows per CTA); rows above kHeteroHubDeg are queued and reduced by the CTA.
+// One row per lane group (G = 256 / LPR rows per CTA); hub rows are reduced by the whole CTA.
 // Shared memory: [G][H] partial sums and [G][nvec] partial statistics of a hub row.
 template <int LPR, int VPL>
-__global__ void __launch_bounds__(kThreads, 2) k_gat_full_aggregate(GatFullAggArgs a) {
+__global__ void __launch_bounds__(kFullRowThreads, 2) k_gat_full_aggregate(GatFullAggArgs a) {
   using K = GatFull<LPR, VPL>;
-  constexpr int G = kThreads / LPR;
+  constexpr int G = kFullRowThreads / LPR;
   extern __shared__ float smem[];
   float* s_part = smem;                         // [G][H]
   float* s_stat = smem + G * a.H;               // [G][nvec]
-  __shared__ int64_t s_hub[G];
-  __shared__ int s_nhub;
   pdl_enter();
   const int gl = (threadIdx.x & 31) % LPR;
   const int g = threadIdx.x / LPR;
   const int nvec = a.H >> 3;
-  if (threadIdx.x == 0) s_nhub = 0;
-  __syncthreads();
   float ad[VPL], m[VPL], s[VPL], acc[VPL][8];
   auto reset = [&]() {
 #pragma unroll
@@ -134,71 +125,41 @@ __global__ void __launch_bounds__(kThreads, 2) k_gat_full_aggregate(GatFullAggAr
       for (int q = 0; q < 8; ++q) acc[v][q] = 0.f;
     }
   };
-  const int64_t r = a.r0 + static_cast<int64_t>(blockIdx.x) * G + g;
-  if (r < a.r1) {
-    const RowRef rr = load_row(a.g, r);
-    if (rr.deg > kHeteroHubDeg) {
-      if (gl == 0) s_hub[atomicAdd(&s_nhub, 1)] = r;
-    } else {
-      reset();
-      K::adh(a, r, gl, ad);
-      K::max_pass(a, rr, 0, 1, gl, ad, m);
-      K::sum_pass(a, rr, 0, 1, gl, ad, m, s, acc);
-      K::epilogue(a, r, gl, s, acc);
-    }
-  }
-  __syncthreads();
-  const int nhub = s_nhub;
-  for (int h = 0; h < nhub; ++h) {
-    const int64_t hr = s_hub[h];
-    const RowRef rr = load_row(a.g, hr);
-    reset();
-    K::adh(a, hr, gl, ad);
-    K::max_pass(a, rr, g, G, gl, ad, m);
+  RowRef rr;
+  full_rows<G>(
+      a.r0, a.r1, g, gl, [&](int64_t r) { rr = load_row(a.g, r); return rr.deg; },
+      [&](int64_t r) {
+        reset();
+        K::adh(a, r, gl, ad);
+        K::max_pass(a, rr, 0, 1, gl, ad, m);
+        K::sum_pass(a, rr, 0, 1, gl, ad, m, s, acc);
+        K::epilogue(a, r, gl, s, acc);
+      },
+      [&](int64_t hr) {
+        const RowRef hb = load_row(a.g, hr);
+        reset();
+        K::adh(a, hr, gl, ad);
+        K::max_pass(a, hb, g, G, gl, ad, m);
+        put_partials<LPR>(s_stat, nvec, g, gl, m);
+        __syncthreads();
 #pragma unroll
-    for (int v = 0; v < VPL; ++v) {
-      const int c = v * LPR + gl;
-      if (c < nvec) s_stat[g * nvec + c] = m[v];
-    }
-    __syncthreads();
-#pragma unroll
-    for (int v = 0; v < VPL; ++v) {
-      const int c = v * LPR + gl;
-      if (c < nvec)
+        for (int v = 0; v < VPL; ++v) {
+          const int c = v * LPR + gl;
+          if (c < nvec)
 #pragma unroll 1
-        for (int q = 0; q < G; ++q) m[v] = fmaxf(m[v], s_stat[q * nvec + c]);
-    }
-    __syncthreads();
-    K::sum_pass(a, rr, g, G, gl, ad, m, s, acc);
-#pragma unroll
-    for (int v = 0; v < VPL; ++v) {
-      const int c = v * LPR + gl;
-      if (c >= nvec) continue;
-      s_stat[g * nvec + c] = s[v];
-#pragma unroll
-      for (int q = 0; q < 8; ++q) s_part[g * a.H + c * 8 + q] = acc[v][q];
-    }
-    __syncthreads();
-    if (g == 0) {
-#pragma unroll
-      for (int v = 0; v < VPL; ++v) {
-        const int c = v * LPR + gl;
-        if (c >= nvec) continue;
-        float ss = 0.f, o[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-#pragma unroll 1
-        for (int q = 0; q < G; ++q) {
-          ss += s_stat[q * nvec + c];
-#pragma unroll
-          for (int e = 0; e < 8; ++e) o[e] += s_part[q * a.H + c * 8 + e];
+            for (int q = 0; q < G; ++q) m[v] = fmaxf(m[v], s_stat[q * nvec + c]);
         }
-        s[v] = ss;
-#pragma unroll
-        for (int e = 0; e < 8; ++e) acc[v][e] = o[e];
-      }
-      K::epilogue(a, hr, gl, s, acc);
-    }
-    __syncthreads();
-  }
+        __syncthreads();
+        K::sum_pass(a, hb, g, G, gl, ad, m, s, acc);
+        put_partials<LPR>(s_stat, nvec, g, gl, s);
+        put_partials<LPR>(s_part, a.H, g, gl, acc);
+        __syncthreads();
+        if (g == 0) {
+          sum_partials<G, LPR>(s_stat, nvec, gl, s);
+          sum_partials<G, LPR>(s_part, a.H, gl, acc);
+          K::epilogue(a, hr, gl, s, acc);
+        }
+      });
 }
 
 // ------------------------------------------------------------------------------------------------------ HGT
@@ -350,17 +311,15 @@ struct HgtFull {
 // Shared memory: per group a dot row [LPR * VPL] and an alpha row [heads]; for hub rows [G][2 heads] statistics and
 // [G][H] partial sums.
 template <int LPR, int VPL>
-__global__ void __launch_bounds__(kThreads, 2) k_hgt_full_attention(HgtFullAttnArgs a) {
+__global__ void __launch_bounds__(kFullRowThreads, 2) k_hgt_full_attention(HgtFullAttnArgs a) {
   using K = HgtFull<LPR, VPL>;
-  constexpr int G = kThreads / LPR;
+  constexpr int G = kFullRowThreads / LPR;
   extern __shared__ float smem[];
-  const int heads = a.heads, nvec = a.H >> 3;
+  const int heads = a.heads;
   float* s_dot = smem;                                  // [G][LPR * VPL]
   float* s_al = s_dot + G * LPR * VPL;                  // [G][heads]
   float* s_stat = s_al + G * heads;                     // [G][2 heads]
   float* s_part = s_stat + G * 2 * heads;               // [G][H]
-  __shared__ int64_t s_hub[G];
-  __shared__ int s_nhub;
   pdl_enter();
   const int lane = threadIdx.x & 31;
   const int gl = lane % LPR;
@@ -370,116 +329,83 @@ __global__ void __launch_bounds__(kThreads, 2) k_hgt_full_attention(HgtFullAttnA
   x.al = s_al + g * heads;
   x.gl = gl;
   x.gmask = (LPR == 32) ? 0xffffffffu : (((1u << LPR) - 1u) << ((lane / LPR) * LPR));
-  if (threadIdx.x == 0) s_nhub = 0;
-  __syncthreads();
   float m[VPL], s[VPL], inv[VPL], acc[VPL][8];
 #pragma unroll
   for (int q = 0; q < VPL; ++q) { m[q] = -INFINITY; s[q] = 0.f; }
-  const int64_t row = a.r0 + static_cast<int64_t>(blockIdx.x) * G + g;
-  if (row < a.r1) {
-    int total = 0;
+  full_rows<G>(
+      a.r0, a.r1, g, gl,
+      [&](int64_t row) {   // the row's neighbours over all its relations
+        int total = 0;
 #pragma unroll 1
-    for (int r = 0; r < a.n_rel; ++r) total += load_row(a.g[r], row).deg;
-    if (total > kHeteroHubDeg) {
-      if (gl == 0) s_hub[atomicAdd(&s_nhub, 1)] = row;
-    } else {
-      K::stats_pass(a, row, 0, 1, x, m, s);
+        for (int r = 0; r < a.n_rel; ++r) total += load_row(a.g[r], row).deg;
+        return total;
+      },
+      [&](int64_t row) {
+        K::stats_pass(a, row, 0, 1, x, m, s);
 #pragma unroll
-      for (int q = 0; q < VPL; ++q) inv[q] = s[q] > 0.f ? __fdividef(1.f, s[q]) : 0.f;
+        for (int q = 0; q < VPL; ++q) inv[q] = s[q] > 0.f ? __fdividef(1.f, s[q]) : 0.f;
 #pragma unroll 1
-      for (int r = 0; r < a.n_rel; ++r) {
-        K::value_pass(a, r, row, 0, 1, x, m, inv, acc);
-        K::store_u(a, r, row, gl, acc);
-      }
-    }
-  }
-  __syncthreads();
-  const int nhub = s_nhub;
-  for (int hb = 0; hb < nhub; ++hb) {
-    const int64_t hr = s_hub[hb];
-#pragma unroll
-    for (int q = 0; q < VPL; ++q) { m[q] = -INFINITY; s[q] = 0.f; }
-    K::stats_pass(a, hr, g, G, x, m, s);
-#pragma unroll
-    for (int q = 0; q < VPL; ++q) {
-      const int h = gl + q * LPR;
-      if (h < heads) { s_stat[(g * heads + h) * 2] = m[q]; s_stat[(g * heads + h) * 2 + 1] = s[q]; }
-    }
-    __syncthreads();
-    // merge the groups' (max, sum) in group order; every group computes the same result
-#pragma unroll
-    for (int q = 0; q < VPL; ++q) {
-      const int h = gl + q * LPR;
-      float M = -INFINITY, S = 0.f;
-      if (h < heads) {
-#pragma unroll 1
-        for (int p = 0; p < G; ++p) {
-          const float mq = s_stat[(p * heads + h) * 2], sq = s_stat[(p * heads + h) * 2 + 1];
-          if (!(sq > 0.f)) continue;
-          if (mq > M) { S = S * expf(M - mq) + sq; M = mq; }
-          else S += sq * expf(mq - M);
+        for (int r = 0; r < a.n_rel; ++r) {
+          K::value_pass(a, r, row, 0, 1, x, m, inv, acc);
+          K::store_u(a, r, row, gl, acc);
         }
-      }
-      m[q] = M;
-      inv[q] = S > 0.f ? __fdividef(1.f, S) : 0.f;
-    }
+      },
+      [&](int64_t hr) {
+#pragma unroll
+        for (int q = 0; q < VPL; ++q) { m[q] = -INFINITY; s[q] = 0.f; }
+        K::stats_pass(a, hr, g, G, x, m, s);
+#pragma unroll
+        for (int q = 0; q < VPL; ++q) {
+          const int h = gl + q * LPR;
+          if (h < heads) { s_stat[(g * heads + h) * 2] = m[q]; s_stat[(g * heads + h) * 2 + 1] = s[q]; }
+        }
+        __syncthreads();
+        // merge the groups' (max, sum) in group order; every group computes the same result
+#pragma unroll
+        for (int q = 0; q < VPL; ++q) {
+          const int h = gl + q * LPR;
+          float M = -INFINITY, S = 0.f;
+          if (h < heads) {
 #pragma unroll 1
-    for (int r = 0; r < a.n_rel; ++r) {
-      K::value_pass(a, r, hr, g, G, x, m, inv, acc);
-#pragma unroll
-      for (int v = 0; v < VPL; ++v) {
-        const int c = v * LPR + gl;
-        if (c < nvec)
-#pragma unroll
-          for (int e = 0; e < 8; ++e) s_part[g * a.H + c * 8 + e] = acc[v][e];
-      }
-      __syncthreads();
-      if (g == 0) {
-#pragma unroll
-        for (int v = 0; v < VPL; ++v) {
-          const int c = v * LPR + gl;
-          if (c >= nvec) continue;
-#pragma unroll
-          for (int e = 0; e < 8; ++e) {
-            float t = 0.f;
+            for (int p = 0; p < G; ++p) {
+              const float mq = s_stat[(p * heads + h) * 2], sq = s_stat[(p * heads + h) * 2 + 1];
+              if (!(sq > 0.f)) continue;
+              if (mq > M) { S = S * expf(M - mq) + sq; M = mq; }
+              else S += sq * expf(mq - M);
+            }
+          }
+          m[q] = M;
+          inv[q] = S > 0.f ? __fdividef(1.f, S) : 0.f;
+        }
 #pragma unroll 1
-            for (int p = 0; p < G; ++p) t += s_part[p * a.H + c * 8 + e];
-            acc[v][e] = t;
+        for (int r = 0; r < a.n_rel; ++r) {
+          if (r > 0) __syncthreads();   // group 0 has summed the previous relation's partials
+          K::value_pass(a, r, hr, g, G, x, m, inv, acc);
+          put_partials<LPR>(s_part, a.H, g, gl, acc);
+          __syncthreads();
+          if (g == 0) {
+            sum_partials<G, LPR>(s_part, a.H, gl, acc);
+            K::store_u(a, r, hr, gl, acc);
           }
         }
-        K::store_u(a, r, hr, gl, acc);
-      }
-      __syncthreads();
-    }
-  }
+      });
 }
 
 }  // namespace
 
 // lane-group shape from the row width H (a multiple of 64 in [64, 1024]: 8 .. 128 vectors)
 void launch_gat_full_aggregate(const GatFullAggArgs& a, cudaStream_t s) {
-  if (a.r1 <= a.r0) return;
   dispatch_lanes<8, 4>(a.H / 8, [&](auto lpr, auto vpl) {
-    constexpr int LPR = decltype(lpr)::value, VPL = decltype(vpl)::value;
-    constexpr int G = kThreads / LPR;
-    const int64_t blocks = (a.r1 - a.r0 + G - 1) / G;
-    const size_t smem = sizeof(float) * G * (a.H + a.H / 8);
-    cudaFuncSetAttribute(k_gat_full_aggregate<LPR, VPL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                         static_cast<int>(smem));
-    launch_k(k_gat_full_aggregate<LPR, VPL>, dim3(static_cast<unsigned>(blocks)), dim3(kThreads), smem, s, a);
+    constexpr int LPR = decltype(lpr)::value;
+    launch_full_rows<LPR>(k_gat_full_aggregate<LPR, decltype(vpl)::value>, a, a.H + a.H / 8, s);
   });
 }
 
 void launch_hgt_full_attention(const HgtFullAttnArgs& a, cudaStream_t s) {
-  if (a.r1 <= a.r0) return;
   dispatch_lanes<8, 4>(a.H / 8, [&](auto lpr, auto vpl) {
     constexpr int LPR = decltype(lpr)::value, VPL = decltype(vpl)::value;
-    constexpr int G = kThreads / LPR;
-    const int64_t blocks = (a.r1 - a.r0 + G - 1) / G;
-    const size_t smem = sizeof(float) * G * (LPR * VPL + 3 * a.heads + a.H);   // up to 48 KB (H = 1024, D = 8)
-    cudaFuncSetAttribute(k_hgt_full_attention<LPR, VPL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                         static_cast<int>(smem));
-    launch_k(k_hgt_full_attention<LPR, VPL>, dim3(static_cast<unsigned>(blocks)), dim3(kThreads), smem, s, a);
+    // up to 48 KB (H = 1024, D = 8)
+    launch_full_rows<LPR>(k_hgt_full_attention<LPR, VPL>, a, LPR * VPL + 3 * a.heads + a.H, s);
   });
 }
 

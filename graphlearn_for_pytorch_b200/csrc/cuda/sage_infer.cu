@@ -1,20 +1,14 @@
 // Exact layer-wise GraphSAGE inference: the neighbour mean over a node's FULL CSR row (the `fanout >= degree` limit of
 // the sampler, which takes every neighbour of a row with d <= k), for a chunk [r0, r1) of global node ids.
 //
-// Rows are reduced in a fixed order with fp32 accumulators and rounded once, without floating-point atomics, so the
-// result is bitwise identical from call to call and for any chunking.  Degrees are power-law: a row above kHubDeg is
-// not walked by one lane group while the rest of the GPU idles -- the whole CTA splits it (group g takes neighbours
-// g, g + G, ...) and the G partial sums are added in group order in shared memory.  Whether a row takes that path
-// depends on its degree alone, so the summation order of every row is fixed.
-#include "device_utils.cuh"
-#include "launch_utils.h"
+// Rows are reduced in a fixed order with fp32 accumulators and rounded once (the row schedule of full_rows.cuh: hub rows
+// are split over the CTA and their partial sums added in group order), so the result is bitwise identical from call to
+// call and for any chunking.
+#include "full_rows.cuh"
 
 namespace glt {
 
 namespace {
-
-constexpr int kHubDeg = 256;
-constexpr int kInferThreads = 256;
 
 // Source row of global node u: the dense bf16 table at column src_col, or the feature table (layer 1).
 __device__ __forceinline__ const uint8_t* full_src_row(const SageFullAggArgs& a, int64_t u) {
@@ -133,87 +127,53 @@ struct FullAgg {
   }
 };
 
-// One row per lane group (G = 256 / LPR rows per CTA); rows above kHubDeg are queued and reduced by the whole CTA.
+// One row per lane group (G = 256 / LPR rows per CTA); hub rows are reduced by the whole CTA.
 template <int LPR, int VPL, bool FP8>
-__global__ void __launch_bounds__(kInferThreads) k_sage_full_aggregate(SageFullAggArgs a) {
+__global__ void __launch_bounds__(kFullRowThreads) k_sage_full_aggregate(SageFullAggArgs a) {
   using K = FullAgg<LPR, VPL, FP8>;
-  constexpr int EPV = K::EPV;
-  constexpr int G = kInferThreads / LPR;
+  constexpr int G = kFullRowThreads / LPR;
   extern __shared__ float s_part[];    // [G][d] partial sums of a hub row
-  __shared__ int64_t s_hub[G];
-  __shared__ int s_nhub;
   pdl_enter();
   const int lane = threadIdx.x & 31;
   const int gl = lane % LPR;
   const int g = threadIdx.x / LPR;
   const unsigned gmask = (LPR == 32) ? 0xffffffffu : (((1u << LPR) - 1u) << ((lane / LPR) * LPR));
-  if (threadIdx.x == 0) s_nhub = 0;
-  __syncthreads();
-
-  const int64_t r = a.r0 + static_cast<int64_t>(blockIdx.x) * G + g;
-  float acc[VPL][EPV];
-#pragma unroll
-  for (int v = 0; v < VPL; ++v)
-#pragma unroll
-    for (int i = 0; i < EPV; ++i) acc[v][i] = 0.f;
-  if (r < a.r1) {
-    const RowRef rr = load_row(a.g, r);
-    if (rr.deg > kHubDeg) {
-      if (gl == 0) s_hub[atomicAdd(&s_nhub, 1)] = r;
-    } else {
-      if (rr.deg > 0) K::accumulate(a, rr.part, rr.start, rr.deg, 0, 1, gl, gmask, acc);
-      K::epilogue(a, r, rr.deg, gl, acc);
-    }
-  }
-  __syncthreads();
-  const int nhub = s_nhub;
-  for (int h = 0; h < nhub; ++h) {
-    const int64_t hr = s_hub[h];
-    const RowRef rr = load_row(a.g, hr);
+  float acc[VPL][K::EPV];
+  auto zero = [&]() {
 #pragma unroll
     for (int v = 0; v < VPL; ++v)
 #pragma unroll
-      for (int i = 0; i < EPV; ++i) acc[v][i] = 0.f;
-    K::accumulate(a, rr.part, rr.start, rr.deg, g, G, gl, gmask, acc);
-#pragma unroll
-    for (int v = 0; v < VPL; ++v) {
-      const int col = (v * LPR + gl) * EPV;
-      if (col < a.d)
-#pragma unroll
-        for (int i = 0; i < EPV; ++i) s_part[g * a.d + col + i] = acc[v][i];
-    }
-    __syncthreads();
-    if (g == 0) {
-#pragma unroll
-      for (int v = 0; v < VPL; ++v) {
-        const int col = (v * LPR + gl) * EPV;
-        if (col >= a.d) continue;
-#pragma unroll
-        for (int i = 0; i < EPV; ++i) {
-          float s = 0.f;
-#pragma unroll 1
-          for (int q = 0; q < G; ++q) s += s_part[q * a.d + col + i];
-          acc[v][i] = s;
+      for (int i = 0; i < K::EPV; ++i) acc[v][i] = 0.f;
+  };
+  RowRef rr;
+  zero();
+  full_rows<G>(
+      a.r0, a.r1, g, gl, [&](int64_t r) { rr = load_row(a.g, r); return rr.deg; },
+      [&](int64_t r) {
+        if (rr.deg > 0) K::accumulate(a, rr.part, rr.start, rr.deg, 0, 1, gl, gmask, acc);
+        K::epilogue(a, r, rr.deg, gl, acc);
+      },
+      [&](int64_t hr) {
+        const RowRef hb = load_row(a.g, hr);
+        zero();
+        K::accumulate(a, hb.part, hb.start, hb.deg, g, G, gl, gmask, acc);
+        put_partials<LPR>(s_part, a.d, g, gl, acc);
+        __syncthreads();
+        if (g == 0) {
+          sum_partials<G, LPR>(s_part, a.d, gl, acc);
+          K::epilogue(a, hr, hb.deg, gl, acc);
         }
-      }
-      K::epilogue(a, hr, rr.deg, gl, acc);
-    }
-    __syncthreads();
-  }
+      });
 }
 
 template <int LPR, int VPL, bool FP8>
 void launch_full(const SageFullAggArgs& a, cudaStream_t s) {
-  constexpr int G = kInferThreads / LPR;
-  const int64_t blocks = (a.r1 - a.r0 + G - 1) / G;
-  launch_k(k_sage_full_aggregate<LPR, VPL, FP8>, dim3(static_cast<unsigned>(blocks)), dim3(kInferThreads),
-           sizeof(float) * G * a.d, s, a);
+  launch_full_rows<LPR>(k_sage_full_aggregate<LPR, VPL, FP8>, a, a.d, s);
 }
 
 }  // namespace
 
 void launch_sage_full_aggregate(const SageFullAggArgs& a, cudaStream_t s) {
-  if (a.r1 <= a.r0) return;
   if (a.feat_fp8) {   // d / 16 vectors of 16 e4m3 elements; d = 128 is <8, 1, true>
     dispatch_lanes<2, 2>(a.d / 16, [&](auto lpr, auto vpl) {
       launch_full<decltype(lpr)::value, decltype(vpl)::value, true>(a, s);

@@ -28,6 +28,7 @@ import torch
 
 from ..data.quantize import mxfp8_row_bytes
 from ..ops import require_native
+from .sage import infer_chunk_rows, infer_chunks, infer_gemm
 
 EdgeType = Tuple[str, str, str]
 
@@ -521,10 +522,7 @@ class HeteroSageEngine(object):
     dev, L = self.device, self.L
     st = self.tid[self.seed_type]
     with torch.cuda.device(dev):
-      if chunk_rows is None:
-        free, _ = torch.cuda.mem_get_info(dev)
-        chunk_rows = max(4096, min(1 << 19, free // 4 // self._infer_chunk_row_bytes()))
-      chunk_rows = max(1, min(int(chunk_rows), max(self._n_nodes)))
+      chunk_rows = infer_chunk_rows(chunk_rows, max(self._n_nodes), self._infer_chunk_row_bytes(), dev)
       # TcGemm / elementwise row counts read on the device: [0] one chunk, [1 + t] every node of type t
       self._rows_dev = torch.tensor([chunk_rows] + self._n_nodes, dtype=torch.int32, device=dev)
       self._ids = torch.arange(max(self._n_nodes), dtype=torch.int64, device=dev)
@@ -537,10 +535,6 @@ class HeteroSageEngine(object):
       out = self._infer_head(X[st])
       self._rows_dev = self._ids = None
       return out[:, :self.C].contiguous()
-
-  def _chunks(self, n: int, chunk_rows: int):
-    for r0 in range(0, n, chunk_rows):
-      yield r0, min(n, r0 + chunk_rows)
 
   def _gh(self, r: int):
     return self.graphs[self.edge_types[r]].graph_handler
@@ -571,9 +565,7 @@ class HeteroSageEngine(object):
     return x
 
   def _gemm(self, A, W, b, relu, out, idx):
-    g = self.nat.TcGemm(self.device.index)
-    g.add_forward(A, W, b, relu, out, self._rows_dev, idx)
-    g.run()
+    infer_gemm(self.nat, A, W, b, relu, out, self._rows_dev, idx)
 
   def _infer_layer(self, l: int, X, Z, chunk_rows: int):
     """R-SAGE layer l: A_t = [mean_r1 | ... | mean_rk | self] per chunk (sage_full_aggregate, mean-only blocks), then
@@ -585,7 +577,7 @@ class HeteroSageEngine(object):
       offs, self_col = self.col[l][t]
       d_t = self._width_in(l, t)
       K = self_col + d_t
-      for r0, r1 in self._chunks(self._n_nodes[t], chunk_rows):
+      for r0, r1 in infer_chunks(self._n_nodes[t], chunk_rows):
         a = buf[:(r1 - r0) * K].view(r1 - r0, K)
         for j, r in enumerate(self.in_rel[l][t]):
           s = self.nt[r]

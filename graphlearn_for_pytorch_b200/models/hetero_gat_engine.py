@@ -33,6 +33,7 @@ from typing import Dict, Optional, Sequence, Union
 import torch
 
 from .hetero_engine import HeteroSageEngine, EdgeType
+from .sage import infer_chunks
 
 
 class HeteroGatEngine(HeteroSageEngine):
@@ -257,7 +258,7 @@ class HeteroGatEngine(HeteroSageEngine):
     if l > 1:
       self._gemm(X[s], W, None, False, P, 1 + s)
       return P
-    for r0, r1 in self._chunks(self._n_nodes[s], chunk_rows):
+    for r0, r1 in infer_chunks(self._n_nodes[s], chunk_rows):
       self._gemm(self._gather_chunk(s, r0, r1, buf), W, None, False, P[r0:r1], 0)
     return P
 
@@ -282,7 +283,7 @@ class HeteroGatEngine(HeteroSageEngine):
         del Pd
         ops.append((r, Ps, as_, ad))
       acc = torch.empty(chunk_rows, H, dtype=torch.float32, device=dev) if len(rels) > 1 else None
-      for r0, r1 in self._chunks(self._n_nodes[t], chunk_rows):
+      for r0, r1 in infer_chunks(self._n_nodes[t], chunk_rows):
         for j, (r, Ps, as_, ad) in enumerate(ops):
           last = j == len(ops) - 1
           nat.gat_full_aggregate(self._gh(r), Ps, as_, ad, hd, r0, r1, acc=acc[:r1 - r0] if acc is not None else None,

@@ -38,6 +38,7 @@ from typing import Dict, Optional, Sequence, Union
 import torch
 
 from .hetero_engine import HeteroSageEngine, EdgeType
+from .sage import infer_chunks
 
 MAX_RELATIONS = 8      # incoming relations of one destination type that the attention kernels take
 
@@ -308,7 +309,7 @@ class HeteroHgtEngine(HeteroSageEngine):
     X = {}
     for u in self.in_types:
       X[u] = torch.empty(self._n_nodes[u], self.hidden, dtype=torch.bfloat16, device=dev)
-      for r0, r1 in self._chunks(self._n_nodes[u], chunk_rows):
+      for r0, r1 in infer_chunks(self._n_nodes[u], chunk_rows):
         self._gemm(self._gather_chunk(u, r0, r1, buf), self.param(('in_W', u)), self.param(('in_b', u)), True,
                    X[u][r0:r1], 0)
     return X
@@ -335,7 +336,7 @@ class HeteroHgtEngine(HeteroSageEngine):
       graphs = [self._gh(r) for r in rels]
       kv = [KQV[self.nt[r]] for r in rels]
       prior = [self._p32(('prior', l, r)) for r in rels]
-      for r0, r1 in self._chunks(self._n_nodes[t], chunk_rows):
+      for r0, r1 in infer_chunks(self._n_nodes[t], chunk_rows):
         n = r1 - r0
         self._gemm(KQV[t][r0:r1, H:2 * H], att_img, None, False, qq[:n], 0)
         nat.hgt_full_attention(graphs, qq[:n], U[:n], hd, r0, r1, kv, prior)

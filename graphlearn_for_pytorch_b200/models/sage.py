@@ -84,6 +84,29 @@ def _round_up(x, m):
   return (x + m - 1) // m * m
 
 
+# The chunking of the engines' exact layer-wise inference (GraphSageEngine, HeteroSageEngine and its subclasses).
+def infer_chunk_rows(chunk_rows: Optional[int], n: int, row_bytes: int, device) -> int:
+  """Target rows per chunk, clamped to [1, n]; None: a quarter of the free device memory at row_bytes per row, at
+  least 4096 and at most 512 k rows."""
+  if chunk_rows is None:
+    free, _ = torch.cuda.mem_get_info(device)
+    chunk_rows = max(4096, min(1 << 19, free // 4 // row_bytes))
+  return max(1, min(int(chunk_rows), n))
+
+
+def infer_chunks(n: int, chunk_rows: int):
+  """[r0, r1) of n rows, chunk_rows at a time."""
+  for r0 in range(0, n, chunk_rows):
+    yield r0, min(n, r0 + chunk_rows)
+
+
+def infer_gemm(nat, A, W, b, relu, out, rows_dev, idx):
+  """out = act(A W^T + b) by a single-use TcGemm forward over rows_dev[idx] rows."""
+  g = nat.TcGemm(A.device.index)
+  g.add_forward(A, W, b, relu, out, rows_dev, idx)
+  g.run()
+
+
 class GraphSageEngine(object):
   """Static-shape, CUDA-graph-captured GraphSAGE training step.
 
@@ -876,10 +899,7 @@ class GraphSageEngine(object):
       bufs = [torch.empty(N, wide, dtype=bf, device=dev) for _ in range(2 if L > 1 else 1)]
       agg_dims = [self.dims_in[l - 1] for l in range(1, L + 1) if not self._project_first(l)]
       a_row = 2 * max(agg_dims)
-      if chunk_rows is None:
-        free, _ = torch.cuda.mem_get_info(dev)
-        chunk_rows = max(4096, min(1 << 19, free // 4 // (a_row * 2)))
-      chunk_rows = max(1, min(int(chunk_rows), N))
+      chunk_rows = infer_chunk_rows(chunk_rows, N, a_row * 2, dev)
       A = torch.empty(chunk_rows, a_row, dtype=bf, device=dev)
       rows_dev = torch.tensor([chunk_rows, N], dtype=torch.int32, device=dev)   # TcGemm row counts (device-side)
       H = None
@@ -898,17 +918,11 @@ class GraphSageEngine(object):
     if self._project_first(l):
       W = self.W(l)
       P = torch.empty(N, 2 * n, dtype=torch.bfloat16, device=self.device)
-      g = nat.TcGemm(self.device.index)
-      g.add_forward(H, torch.cat([W[:, :d], W[:, d:]], 0), None, False, P, rows_dev, 1)
-      g.run()
-      for r0 in range(0, N, chunk_rows):
-        r1 = min(N, r0 + chunk_rows)
+      infer_gemm(nat, H, torch.cat([W[:, :d], W[:, d:]], 0), None, False, P, rows_dev, 1)
+      for r0, r1 in infer_chunks(N, chunk_rows):
         nat.sage_full_aggregate(self.gh, None, P, 0, n, n, r0, r1, True, self.b(l), relu, out[r0:r1])
       return
-    for r0 in range(0, N, chunk_rows):
-      r1 = min(N, r0 + chunk_rows)
+    for r0, r1 in infer_chunks(N, chunk_rows):
       a = A[:r1 - r0, :2 * d]
       nat.sage_full_aggregate(self.gh, self.feat if l == 1 else None, H, 0, 0, d, r0, r1, False, None, False, a)
-      g = nat.TcGemm(self.device.index)
-      g.add_forward(a, self.W(l), self.b(l), relu, out[r0:r1], rows_dev, 0)
-      g.run()
+      infer_gemm(nat, a, self.W(l), self.b(l), relu, out[r0:r1], rows_dev, 0)
