@@ -180,6 +180,7 @@ struct GraphHandle {
   // all neighbours; returns (nbrs [sum], counts [n] int64, eids)
   std::tuple<Tensor, Tensor, Tensor> full_neighbors(const Tensor& ids, bool with_edge) {
     c10::cuda::CUDAGuard guard(device);
+    TORCH_CHECK(!with_edge || has_eids, "graph has no edge ids");
     Tensor deg = lookup_degree(ids);
     Tensor offs = torch::zeros({ids.numel() + 1}, opts(torch::kInt64));
     if (ids.numel() > 0) offs.narrow(0, 1, ids.numel()).copy_(deg.cumsum(0));
@@ -212,9 +213,13 @@ struct GraphHandle {
                      int64_t stream) {
     c10::cuda::CUDAGuard guard(device);
     check_ids(starts, "random_walk: starts must be contiguous int64 on the graph's device");
+    TORCH_CHECK(walk_len >= 0 && walk_len < INT32_MAX, "random_walk: walk_length must be in [0, 2^31 - 1)");
+    Node2VecWeights w;
+    const char* bad = node2vec_weights(p, q, &w);
+    TORCH_CHECK(bad == nullptr, fmt("random_walk: %s", bad));
     Tensor out = torch::empty({starts.numel(), walk_len + 1}, opts(torch::kInt64));
-    launch_random_walk(tbl, starts.data_ptr<int64_t>(), starts.numel(), walk_len, p, q, seed, stream,
-                       out.data_ptr<int64_t>(), cur_stream());
+    launch_random_walk(tbl, starts.data_ptr<int64_t>(), starts.numel(), static_cast<int>(walk_len),
+                       !(p == 1.0 && q == 1.0), w, seed, stream, out.data_ptr<int64_t>(), cur_stream());
     check_cuda_err("random_walk");
     return out;
   }
@@ -307,6 +312,8 @@ struct DeviceTable {
   // induced subgraph of `g` on the table's current node set (n = size())
   std::tuple<Tensor, Tensor, Tensor> subgraph(GraphHandle& g, int64_t n, bool with_edge) {
     c10::cuda::CUDAGuard guard(device);
+    TORCH_CHECK(n >= 0 && n <= cap_nodes, "DeviceTable.subgraph: n must be in [0, capacity]");
+    TORCH_CHECK(!with_edge || g.has_eids, "graph has no edge ids");
     auto o64 = torch::TensorOptions().dtype(torch::kInt64).device(torch::kCUDA, device);
     Tensor cnt = torch::zeros({n}, o64);
     launch_subgraph_count(g.tbl, ht, nodes.data_ptr<int64_t>(), n, cnt.data_ptr<int64_t>(), cur_stream());
@@ -1759,13 +1766,13 @@ static void metapath_walk(const MetaPath& mp, const Tensor& starts, int64_t walk
 }
 
 // node2vec's p / q walks of one step over a metapath of one relation from a type to itself; the same contract as
-// metapath_walk.  max(1, 1/p, 1/q) / min(1, 1/p, 1/q) <= 64 bounds the rejection sampler's expected proposals.
+// metapath_walk.  p and q pass node2vec_weights (philox.h): r <= 64 bounds the rejection sampler's proposals.
 static void node2vec_walk(const MetaPath& mp, const Tensor& starts, int64_t walks_per_node, int64_t context_size,
                           int64_t seed, const Tensor& step, Tensor walks, Tensor n_valid, double p, double q) {
   c10::cuda::CUDAGuard guard(mp.device);
-  TORCH_CHECK(std::isfinite(p) && std::isfinite(q) && p > 0 && q > 0, "node2vec_walk: p and q must be finite and > 0");
-  const double hi = std::max({1.0, 1.0 / p, 1.0 / q}), lo = std::min({1.0, 1.0 / p, 1.0 / q});
-  TORCH_CHECK(hi / lo <= 64.0, "node2vec_walk: max(1, 1/p, 1/q) / min(1, 1/p, 1/q) must be <= 64");
+  Node2VecWeights w;
+  const char* bad = node2vec_weights(p, q, &w);
+  TORCH_CHECK(bad == nullptr, fmt("node2vec_walk: %s", bad));
   TORCH_CHECK(mp.R == 1 && mp.types.off[0] == mp.types.off[1] && mp.types.n[0] == mp.types.n[1],
               "node2vec_walk: the metapath must be one relation from a node type to itself");
   check_ids(starts, "node2vec_walk: starts must be contiguous int64 on the metapath's device");
@@ -1780,7 +1787,7 @@ static void node2vec_walk(const MetaPath& mp, const Tensor& starts, int64_t walk
   if (n_walks == 0) return;
   launch_node2vec_walk(mp.dev_tables(), mp.types, starts.data_ptr<int64_t>(), static_cast<int>(n_walks),
                        static_cast<int>(walks_per_node), static_cast<int>(L), static_cast<int>(context_size),
-                       static_cast<float>(1.0 / p / hi), static_cast<float>(1.0 / hi), static_cast<float>(1.0 / q / hi),
+                       w.ret, w.in, w.out,
                        static_cast<uint64_t>(seed), step.data_ptr<int32_t>(), walks.data_ptr<int64_t>(),
                        n_valid.data_ptr<int32_t>(), cur_stream());
   check_cuda_err("node2vec_walk");

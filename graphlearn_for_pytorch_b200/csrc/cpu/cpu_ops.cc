@@ -636,15 +636,20 @@ std::tuple<Tensor, Tensor, Tensor, Tensor> cpu_node_subgraph(
 }
 
 // ----------------------------------------------------------------------------
-// Random walks (uniform / node2vec p,q by rejection).  New functionality: the
-// reference only declares SamplingType.RANDOM_WALK (sampler/base.py:335).
-// A walker on a node without out-edges stays in place.
+// Random walks (uniform / node2vec p,q by rejection, philox.h).  New functionality:
+// the reference only declares SamplingType.RANDOM_WALK (sampler/base.py:335).
+// Same draws and the same float accept test as k_random_walk, so the planes'
+// walks are bit-identical.  A walker on a node without out-edges stays in place.
 // ----------------------------------------------------------------------------
 Tensor cpu_random_walk(const Tensor& indptr, const Tensor& indices, const Tensor& starts,
                        int64_t walk_length, double p, double q, int64_t seed, int64_t stream) {
   check_i64(indptr, "indptr");
   check_i64(indices, "indices");
   check_i64(starts, "starts");
+  TORCH_CHECK(walk_length >= 0, "random_walk: walk_length must be >= 0");
+  Node2VecWeights nw;
+  const char* bad = node2vec_weights(p, q, &nw);
+  TORCH_CHECK(bad == nullptr, std::string("random_walk: ") + (bad ? bad : ""));
   const int64_t num_rows = indptr.numel() - 1;
   const int64_t* ip = indptr.data_ptr<int64_t>();
   const int64_t* ind = indices.data_ptr<int64_t>();
@@ -653,7 +658,6 @@ Tensor cpu_random_walk(const Tensor& indptr, const Tensor& indices, const Tensor
   Tensor out = torch::empty({n, walk_length + 1}, torch::kInt64);
   int64_t* o = out.data_ptr<int64_t>();
   const bool biased = !(p == 1.0 && q == 1.0);
-  const double maxw = std::max({1.0, 1.0 / p, 1.0 / q});
   glt::parallel_for(0, n, 512, [&](int64_t b, int64_t e) {
     for (int64_t i = b; i < e; ++i) {
       int64_t cur = st[i], prev = -1;
@@ -666,14 +670,13 @@ Tensor cpu_random_walk(const Tensor& indptr, const Tensor& indices, const Tensor
           if (!biased || prev < 0) {
             nxt = ind[ip[cur] + bounded(philox_draw(seed, stream, i, draw++), (uint32_t)d)];
           } else {
-            for (int tries = 0; tries < 64; ++tries) {
-              int64_t cand = ind[ip[cur] + bounded(philox_draw(seed, stream, i, draw++), (uint32_t)d)];
-              double w;
-              if (cand == prev) w = 1.0 / p;
-              else if (prev < num_rows && edge_in_row(ind, ip[prev], ip[prev + 1], cand, false)) w = 1.0;
-              else w = 1.0 / q;
-              nxt = cand;
-              if (u01(philox_draw(seed, stream, i, draw++)) * maxw <= w) break;
+            const int64_t pd = row_degree(ip, num_rows, prev);
+            for (int tries = 0; tries < kNode2VecMaxProposals; ++tries) {
+              nxt = ind[ip[cur] + bounded(philox_draw(seed, stream, i, draw++), (uint32_t)d)];
+              const float u = u01(philox_draw(seed, stream, i, draw++));
+              if (node2vec_accept(nw, nxt == prev, u,
+                                  [&] { return pd > 0 && edge_in_row(ind, ip[prev], ip[prev] + pd, nxt, false); }))
+                break;
             }
           }
         }

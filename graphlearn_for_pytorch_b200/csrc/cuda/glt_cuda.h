@@ -6,6 +6,8 @@
 
 #include <cstdint>
 
+#include "../philox.h"
+
 namespace glt {
 
 constexpr int kMaxParts = 16;  // 8 GPUs of one NVSwitch box + optional host tiers
@@ -141,7 +143,8 @@ void launch_subgraph_count(GraphTable g, HashTable t, const int64_t* nodes, int 
 void launch_subgraph_fill(GraphTable g, HashTable t, const int64_t* nodes, int n,
                           const int64_t* offs, int64_t* rows, int64_t* cols, int64_t* eids,
                           cudaStream_t s);
-void launch_random_walk(GraphTable g, const int64_t* starts, int n, int walk_len, float p, float q,
+// uniform steps when !biased, otherwise node2vec's second-order rule with weights w (philox.h)
+void launch_random_walk(GraphTable g, const int64_t* starts, int n, int walk_len, bool biased, Node2VecWeights w,
                         uint64_t seed, uint32_t stream, int64_t* out, cudaStream_t s);
 void launch_nbr_prob(GraphTable g, GraphTable nbr_g, const float* last, const float* nbr_last,
                      int64_t n, int64_t n_nbr, int k, float* cur, cudaStream_t s);
@@ -357,7 +360,6 @@ void launch_metapath_walk(const GraphTable* rel, int R, MetaPathTypes types, con
 // node2vec's second-order walk over one relation from a type to itself (column-sorted CSR rows): the same output and
 // dead-end contract as launch_metapath_walk.  w_ret / w_in / w_out are the unnormalised weights 1/p, 1 and 1/q divided
 // by their maximum; L <= kNode2VecMaxWalk keeps the draw counters from wrapping.
-constexpr int kNode2VecMaxProposals = 4096;
 constexpr int kNode2VecMaxWalk = 1 << 20;
 void launch_node2vec_walk(const GraphTable* rel, MetaPathTypes types, const int64_t* starts, int n_walks, int W, int L,
                           int C, float w_ret, float w_in, float w_out, uint64_t seed, const int32_t* step_dev,

@@ -88,11 +88,11 @@ __global__ void k_subgraph_fill(GraphTable g, HashTable t, const int64_t* nodes,
   }
 }
 
-// Random walk, thread per walker (new functionality; node2vec p/q by rejection).
-__global__ void k_random_walk(GraphTable g, const int64_t* starts, int n, int walk_len, float p,
-                              float q, uint64_t seed, uint32_t stream, int64_t* out) {
-  const bool biased = !(p == 1.f && q == 1.f);
-  const float maxw = fmaxf(1.f, fmaxf(1.f / p, 1.f / q));
+// Random walk, thread per walker (new functionality).  A step draws one Philox word for a uniform position, or runs
+// node2vec's rejection sampler (philox.h) with two words per proposal: the position, then the acceptance uniform.  A
+// walker on a node without out-edges (or outside every shard) stays in place.
+__global__ void k_random_walk(GraphTable g, const int64_t* starts, int n, int walk_len, bool biased,
+                              Node2VecWeights w, uint64_t seed, uint32_t stream, int64_t* out) {
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     int64_t cur = starts[i], prev = -1;
     out[static_cast<int64_t>(i) * (walk_len + 1)] = cur;
@@ -104,15 +104,10 @@ __global__ void k_random_walk(GraphTable g, const int64_t* starts, int n, int wa
         if (!biased || prev < 0) {
           nxt = load_col(g, row.part, row.start + bounded(philox_draw(seed, stream, i, draw++), row.deg));
         } else {
-          for (int tries = 0; tries < 64; ++tries) {
-            const int64_t cand =
-                load_col(g, row.part, row.start + bounded(philox_draw(seed, stream, i, draw++), row.deg));
-            float w;
-            if (cand == prev) w = 1.f / p;
-            else if (edge_exists(g, prev, cand)) w = 1.f;
-            else w = 1.f / q;
-            nxt = cand;
-            if (u01(philox_draw(seed, stream, i, draw++)) * maxw <= w) break;
+          for (int tries = 0; tries < kNode2VecMaxProposals; ++tries) {
+            nxt = load_col(g, row.part, row.start + bounded(philox_draw(seed, stream, i, draw++), row.deg));
+            const float u = u01(philox_draw(seed, stream, i, draw++));
+            if (node2vec_accept(w, nxt == prev, u, [&] { return edge_exists(g, prev, nxt); })) break;
           }
         }
       }
@@ -170,10 +165,10 @@ void launch_subgraph_fill(GraphTable g, HashTable t, const int64_t* nodes, int n
   k_subgraph_fill<<<grid_for(n, 8), 256, 0, s>>>(g, t, nodes, n, offs, rows, cols, eids);
 }
 
-void launch_random_walk(GraphTable g, const int64_t* starts, int n, int walk_len, float p, float q,
+void launch_random_walk(GraphTable g, const int64_t* starts, int n, int walk_len, bool biased, Node2VecWeights w,
                         uint64_t seed, uint32_t stream, int64_t* out, cudaStream_t s) {
   if (n <= 0) return;
-  k_random_walk<<<grid_for(n, 128), 128, 0, s>>>(g, starts, n, walk_len, p, q, seed, stream, out);
+  k_random_walk<<<grid_for(n, 128), 128, 0, s>>>(g, starts, n, walk_len, biased, w, seed, stream, out);
 }
 
 void launch_nbr_prob(GraphTable g, GraphTable nbr_g, const float* last, const float* nbr_last,

@@ -8,6 +8,7 @@
 // (reference: csrc/cuda/random_sampler.cu:236-241), which is neither
 // reproducible across devices nor checkpointable.
 #pragma once
+#include <algorithm>
 #include <cstdint>
 #include <cmath>
 
@@ -84,6 +85,43 @@ GLT_HD uint32_t floyd_candidate(uint64_t seed, uint32_t stream, uint64_t row,
                                 uint32_t i, uint32_t d, uint32_t k) {
   uint32_t j = d - k + i;
   return bounded(philox_draw(seed, stream, row, i), j + 1u);
+}
+
+// node2vec's second-order step, shared by every walk sampler on both planes.  At v with previous node t, entry x of
+// v's row weighs 1/p if x == t, 1 if t's row holds x, 1/q otherwise; the step proposes x uniformly over the row's
+// positions and accepts it with probability w(x) / max(1, 1/p, 1/q).  With r = max / min weight <= kNode2VecMaxRatio
+// a proposal is accepted with probability >= 1/64, so a step that still has none after kNode2VecMaxProposals takes its
+// last proposal with probability < (63/64)^4096 ~ 1e-28.
+constexpr int kNode2VecMaxProposals = 4096;
+constexpr double kNode2VecMaxRatio = 64.0;
+
+// The three weights divided by their maximum, rounded to float once on the host: every plane then decides a proposal
+// with the same float comparisons, so GPU and CPU walks agree bit for bit at any p and q.
+struct Node2VecWeights {
+  float ret, in, out;
+  float lo, hi;  // min / max of in and out: a uniform outside [lo, hi) decides x != t without t's row
+};
+
+// nullptr with *w filled, or why p and q are refused.
+inline const char* node2vec_weights(double p, double q, Node2VecWeights* w) {
+  if (!(std::isfinite(p) && std::isfinite(q) && p > 0 && q > 0)) return "p and q must be finite and > 0";
+  const double hi = std::max({1.0, 1.0 / p, 1.0 / q}), lo = std::min({1.0, 1.0 / p, 1.0 / q});
+  if (hi / lo > kNode2VecMaxRatio) return "max(1, 1/p, 1/q) / min(1, 1/p, 1/q) must be <= 64";
+  w->ret = static_cast<float>(1.0 / p / hi);
+  w->in = static_cast<float>(1.0 / hi);
+  w->out = static_cast<float>(1.0 / q / hi);
+  w->lo = std::min(w->in, w->out);
+  w->hi = std::max(w->in, w->out);
+  return nullptr;
+}
+
+// Accept proposal x, u = u01 of its acceptance draw.  in_prev_row() (is x in t's row?) runs only when it decides.
+template <class InPrevRow>
+GLT_HD bool node2vec_accept(const Node2VecWeights& w, bool is_prev, float u, InPrevRow in_prev_row) {
+  if (is_prev) return u < w.ret;
+  if (u < w.lo) return true;
+  if (u >= w.hi) return false;
+  return in_prev_row() ? u < w.in : u < w.out;
 }
 
 }  // namespace glt

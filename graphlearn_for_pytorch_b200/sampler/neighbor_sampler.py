@@ -621,7 +621,18 @@ class NeighborSampler(BaseSampler):
   def random_walk(self, starts: torch.Tensor, walk_length: int, p: float = 1.0, q: float = 1.0,
                   etype: Optional[EdgeType] = None) -> torch.Tensor:
     """[n, walk_length + 1] node ids; uniform (p=q=1) or node2vec-biased walks.
-    New functionality: the reference only declares SamplingType.RANDOM_WALK."""
+    New functionality: the reference only declares SamplingType.RANDOM_WALK.
+
+    A step of a biased walk weighs the previous node 1/p, its neighbours 1 and every other node 1/q, and samples
+    by rejection: p and q must be finite and > 0 with max(1, 1/p, 1/q) / min(1, 1/p, 1/q) <= 64."""
+    p, q, walk_length = float(p), float(q), int(walk_length)
+    if walk_length < 0:
+      raise ValueError(f'random_walk: walk_length must be >= 0, got {walk_length}')
+    if not (math.isfinite(p) and math.isfinite(q) and p > 0 and q > 0):
+      raise ValueError(f'random_walk: p and q must be finite and > 0, got p={p}, q={q}')
+    w = (1.0, 1.0 / p, 1.0 / q)
+    if max(w) / min(w) > 64.0:
+      raise ValueError(f'random_walk: max(1, 1/p, 1/q) / min(1, 1/p, 1/q) must be <= 64, got p={p}, q={q}')
     g = self._graph_of(etype)
     self.lazy_init_sampler()
     starts = starts.to(self.device, dtype=torch.int64).contiguous()
