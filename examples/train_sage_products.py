@@ -6,6 +6,10 @@ train_sage_prod_with_trim.py.  Two paths:
   --mode engine   fused CUDA-graph engine (wgmma layer 1, hand-written backward); train / valid / test accuracy
                   from exact layer-wise full-neighbourhood inference (`inference()`), the protocol of the reference
                   example and of published ogbn-products accuracies
+  --cs            (engine mode, also its CPU fallback) Correct & Smooth after inference: PyG's ogbn-products recipe
+                  (`CorrectAndSmooth`, 50 + 50 layers, alphas 1.0 / 0.8, no autoscale, scale 20; sym-normalised
+                  correction, row-normalised smoothing) on the softmax of the full-neighbourhood logits, with the
+                  train split as the mask; accuracies before and after
 """
 import argparse
 import time
@@ -23,6 +27,7 @@ p.add_argument('--epochs', type=int, default=2)
 p.add_argument('--batch', type=int, default=1024)
 p.add_argument('--dropout', type=float, default=0.5, help='hidden-layer dropout (engine mode and loader-mode model)')
 p.add_argument('--split-ratio', type=float, default=0.2, help='fraction of (hot) feature rows kept in HBM')
+p.add_argument('--cs', action='store_true', help='engine mode: Correct & Smooth the inference() predictions')
 args = p.parse_args()
 
 cuda = torch.cuda.is_available()
@@ -31,6 +36,22 @@ ei, x, y, split, num_nodes = load_homo(args)
 args.nodes = num_nodes
 n_cls = int(y.max()) + 1
 train_idx = split['train']
+
+
+def correct_and_smooth(logits, graph):
+  """PyG's ogbn-products C&S recipe on softmax(logits) over `graph`, the train split as the mask."""
+  from graphlearn_for_pytorch_b200.models import CorrectAndSmooth
+  t0 = time.time()
+  y_soft = logits.float().softmax(-1)
+  mask, y_train = train_idx.to(y_soft.device), y[train_idx].to(y_soft.device)
+  cs = CorrectAndSmooth(50, 1.0, 50, 0.8, autoscale=False, scale=20.0)
+  out = cs.correct(y_soft, y_train, mask, graph, norm='sym')
+  out = cs.smooth(out, y_train, mask, graph, norm='row')
+  if cuda:
+    torch.cuda.synchronize()
+  pred, yd = out.argmax(1), y.to(out.device)
+  print('  '.join(f'{k} acc {float((pred[split[k].to(out.device)] == yd[split[k].to(out.device)]).float().mean()):.4f}'
+                  for k in ('train', 'valid', 'test')) + f'  (after C&S, {time.time() - t0:.2f}s)')
 
 if args.mode == 'loader':
   ds = glt.data.Dataset()
@@ -79,9 +100,12 @@ elif not cuda:
     losses = [float(tr.train_step(train_idx[perm[i:i + args.batch]]))
               for i in range(0, perm.numel() - args.batch + 1, args.batch)]
     print(f'epoch {epoch}: loss {sum(losses) / max(len(losses), 1):.4f} time {time.time() - t0:.2f}s')
-  pred = tr.inference().argmax(1)
+  logits = tr.inference()
+  pred = logits.argmax(1)
   print('  '.join(f'{k} acc {float((pred[split[k]] == y[split[k]]).float().mean()):.4f}'
                   for k in ('train', 'valid', 'test')))
+  if args.cs:
+    correct_and_smooth(logits, ds.graph)
 else:
   in_dim = (x.shape[1] + 63) // 64 * 64
   feats = torch.zeros(args.nodes, in_dim, dtype=torch.bfloat16, device=device)
@@ -108,10 +132,13 @@ else:
     print(f'epoch {epoch}: loss {sum(losses) / max(len(losses), 1):.4f} eval-acc {c / n:.4f} '
           f'time {time.time() - t0:.2f}s ({perm.numel() / (time.time() - t0):.0f} seeds/s)')
   t0 = time.time()
-  pred = eng.inference().argmax(1)
+  logits = eng.inference()
+  pred = logits.argmax(1)
   torch.cuda.synchronize()
   y_dev = y.to(device)
   accs = {k: float((pred[split[k].to(device)] == y_dev[split[k].to(device)]).float().mean())
           for k in ('train', 'valid', 'test')}
   print('  '.join(f'{k} acc {a:.4f}' for k, a in accs.items()) + f'  (full-neighbourhood inference, '
         f'{time.time() - t0:.2f}s)')
+  if args.cs:
+    correct_and_smooth(logits, graph)

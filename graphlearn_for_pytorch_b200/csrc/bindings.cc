@@ -1043,6 +1043,57 @@ static void sage_full_aggregate(GraphHandle* graph, RowTableHandle* feat, const 
   check_cuda_err("sage_full_aggregate");
 }
 
+// num_layers iterations of label propagation over every row of the graph (csrc/cuda/label_prop.cu), from x_0 = base:
+//   x_{k+1} = post(alpha * A_norm x_k + (1 - alpha) * base),  post = clamp to [lo, hi], then base on the rows of fixed
+// A_norm is 'sym' (deg_i^-1/2 deg_j^-1/2) or 'row' (1 / deg_i) over the unweighted CSR.  base: fp32 [num_rows, cp]
+// holding c classes, cp = c rounded up to 4.  Returns a new [num_rows, cp] tensor whose columns >= c are 0 (a copy of
+// base when num_layers = 0).  The factors are computed once, two buffers ping-pong, and nothing waits for the device.
+static Tensor label_prop(GraphHandle* graph, const Tensor& base, int64_t c, int64_t num_layers, double alpha,
+                         const std::string& norm, double lo, double hi, const c10::optional<Tensor>& fixed) {
+  TORCH_CHECK(graph != nullptr && graph->tbl.num_parts > 0, "label_prop: graph has no shards");
+  c10::cuda::CUDAGuard guard(graph->device);
+  TORCH_CHECK(c >= 1 && c <= 512, fmt("label_prop: %lld classes, the kernel takes 1 to 512", static_cast<long long>(c)));
+  TORCH_CHECK(norm == "sym" || norm == "row", fmt("label_prop: norm must be 'sym' or 'row', not '%s'", norm.c_str()));
+  TORCH_CHECK(std::isfinite(alpha), "label_prop: alpha must be finite");
+  TORCH_CHECK(num_layers >= 0, "label_prop: num_layers must be >= 0");
+  TORCH_CHECK(!(lo > hi), "label_prop: clamp bounds need lo <= hi");
+  const int64_t n = graph->num_rows, cp = (c + 3) / 4 * 4;
+  check_rows(base, torch::kFloat32, cp, "label_prop: base must be contiguous, 16-byte aligned fp32 [rows, c rounded up "
+                                        "to 4] on the graph's device");
+  TORCH_CHECK(base.size(0) == n, fmt("label_prop: base has %lld rows, the graph %lld",
+                                     static_cast<long long>(base.size(0)), static_cast<long long>(n)));
+  if (has(fixed))
+    check_vec(*fixed, torch::kBool, n, "label_prop: fixed must be a contiguous bool [rows] mask on the graph's device");
+  if (num_layers == 0) return base.clone();
+  const auto f32 = base.options();
+  Tensor s = torch::empty({n}, f32);
+  Tensor t = norm == "sym" ? torch::empty({n}, f32) : Tensor();
+  launch_label_prop_factors(graph->tbl, n, norm == "sym", s.data_ptr<float>(), t.defined() ? t.data_ptr<float>() : nullptr,
+                            cur_stream());
+  check_cuda_err("label_prop_factors");
+  Tensor buf[2] = {torch::empty({n, cp}, f32), num_layers > 1 ? torch::empty({n, cp}, f32) : Tensor()};
+  LabelPropArgs a{};
+  a.g = graph->tbl;
+  a.n = n;
+  a.c = static_cast<int>(c);
+  a.cp = static_cast<int>(cp);
+  a.base = base.data_ptr<float>();
+  a.s = s.data_ptr<float>();
+  a.t = t.defined() ? t.data_ptr<float>() : nullptr;
+  a.alpha = static_cast<float>(alpha);
+  a.beta = static_cast<float>(1.0 - alpha);
+  a.lo = static_cast<float>(lo);
+  a.hi = static_cast<float>(hi);
+  a.fixed = has(fixed) ? reinterpret_cast<const uint8_t*>(fixed->data_ptr()) : nullptr;
+  for (int64_t k = 0; k < num_layers; ++k) {
+    a.x = k == 0 ? a.base : buf[(k - 1) & 1].data_ptr<float>();
+    a.out = buf[k & 1].data_ptr<float>();
+    launch_label_prop(a, cur_stream());
+    check_cuda_err("label_prop");
+  }
+  return buf[(num_layers - 1) & 1];
+}
+
 static void add_block_f32(const Tensor& dA, int64_t col, int64_t d, const Tensor& counters, int64_t n_hops, Tensor dH) {
   c10::cuda::CUDAGuard guard(dA.device());
   TORCH_CHECK(d % 8 == 0, "add_block_f32: d must be a multiple of 8");
@@ -2619,6 +2670,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("sage_full_aggregate", &sage_full_aggregate, py::arg("graph"), py::arg("feat"), py::arg("src"),
         py::arg("src_col"), py::arg("self_col"), py::arg("d"), py::arg("r0"), py::arg("r1"), py::arg("combine"),
         py::arg("bias"), py::arg("relu"), py::arg("out"), py::arg("mean_only") = false);
+  m.def("label_prop", &label_prop, py::arg("graph"), py::arg("base"), py::arg("c"), py::arg("num_layers"),
+        py::arg("alpha"), py::arg("norm"), py::arg("lo"), py::arg("hi"), py::arg("fixed") = py::none());
   m.def("sage_aggregate_block", &sage_aggregate_block);
   m.def("sage_scatter_block", &sage_scatter_block);
   m.def("add_block_f32", &add_block_f32);

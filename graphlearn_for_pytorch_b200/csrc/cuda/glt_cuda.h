@@ -219,6 +219,30 @@ struct SageFullAggArgs {
 };
 void launch_sage_full_aggregate(const SageFullAggArgs& a, cudaStream_t s);
 
+// ---- label_prop.cu (label propagation / Correct & Smooth over the full CSR) ------
+// One iteration over every row i of [0, n) (row i lists the nodes whose values flow into i; multi-edges count with
+// their multiplicity):
+//   out_i = alpha * s_i * sum_{j in row(i)} t_j x_j + beta * base_i, clamped to [lo, hi]; out_i = base_i where fixed[i]
+// x, base, out: fp32 [n, cp], cp a multiple of 4 in [4, 512], 16-byte aligned; columns >= c of out are written as 0.
+// Columns outside [0, n) read as zero rows.  t == nullptr: t_j = 1.
+struct LabelPropArgs {
+  GraphTable g;
+  int64_t n;
+  int c, cp;
+  const float* x;
+  const float* base;
+  const float* s;               // [n]
+  const float* t;               // [n] or nullptr
+  float alpha, beta;
+  float lo, hi;
+  const uint8_t* fixed;         // bool [n] or nullptr
+  float* out;
+  int64_t r0, r1;               // set by launch_label_prop: all rows [0, n)
+};
+void launch_label_prop(const LabelPropArgs& a, cudaStream_t s);
+// The per-row factors from row lengths: s = t = deg^-1/2 (sym), or s = 1 / deg (row; t not written); 0 where deg = 0.
+void launch_label_prop_factors(const GraphTable& g, int64_t n, bool sym, float* s, float* t, cudaStream_t st);
+
 // dH[s, :] += dA[t, mean_col : mean_col + d] / deg[t] for every sampled edge t <- s of the targets t < cum[n_hops]
 // (the mean block of one relation of a heterogeneous layer; its self block is added by launch_add_block_f32)
 struct SageScatterArgs {

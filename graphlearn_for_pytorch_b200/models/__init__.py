@@ -10,3 +10,4 @@ from .hetero_gat_engine import HeteroGatEngine
 from .hetero_hgt_engine import HeteroHgtEngine
 from .metapath2vec import MetaPath2VecEngine
 from .seal_engine import SealEngine
+from .label_prop import LabelPropagation, CorrectAndSmooth
