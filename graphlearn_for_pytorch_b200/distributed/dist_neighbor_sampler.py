@@ -9,18 +9,15 @@ with labels and features).  Data planes:
           their owners through RPC, partial results are stitched back in seed order.
 """
 import asyncio
-import math
 from typing import Dict, List, Optional, Tuple, Union
 
 import torch
 
 from ..channel import ChannelBase, SampleMessage
 from ..ops import require_native
-from ..ops.tables import IdTable
 from ..sampler import (EdgeSamplerInput, HeteroSamplerOutput, NegativeSampling, NeighborOutput, NeighborSampler,
                        NodeSamplerInput, SamplerOutput, SamplingConfig, SamplingType)
 from ..typing import EdgeType, NodeType, as_str, reverse_edge_type
-from ..utils.common import count_dict
 from .dist_dataset import DistDataset
 from .dist_feature import DistFeature
 from .dist_graph import DistGraph
@@ -187,163 +184,49 @@ class DistNeighborSampler(ConcurrentEventLoop):
       return out
     return await self._homo_from_seeds(seeds)
 
+  async def _drive(self, loop):
+    """Serve a NeighborSampler hop loop over the partitions: every request of a hop starts at once, then they are
+    awaited in order."""
+    outs = None
+    while True:
+      try:
+        reqs = loop.send(outs)
+      except StopIteration as done:
+        return done.value
+      tasks = [asyncio.ensure_future(self._sample_one_hop(*r)) for r in reqs]
+      outs = [await t for t in tasks]
+
   async def _homo_from_seeds(self, seeds: torch.Tensor) -> SamplerOutput:
     if not self._remote:
       return self.sampler._sample_from_nodes(seeds)
-    s = self.sampler
-    table = IdTable(self.device, s._max_sampled_nodes(seeds.numel()))
-    table.init(seeds)
-    n0 = table.size()
-    frontier = table.keys(0)
-    frontier_local = torch.arange(n0, dtype=torch.int64, device=self.device)
-    rows, cols, eids, nn, ne = [], [], [], [n0], []
-    stream = s._next_stream(len(self.num_neighbors))
-    for h, k in enumerate(self.num_neighbors):
-      out = await self._sample_one_hop(frontier, k, None, stream + h)
-      if out.nbr.numel() == 0:
-        break
-      before = table.size()
-      nbr_local = table.insert(out.nbr)
-      rows.append(nbr_local)
-      cols.append(torch.repeat_interleave(frontier_local, out.nbr_num.to(self.device)))
-      if out.edge is not None:
-        eids.append(out.edge)
-      after = table.size()
-      nn.append(after - before)
-      ne.append(int(out.nbr.numel()))
-      frontier = table.keys(before)
-      frontier_local = torch.arange(before, after, dtype=torch.int64, device=self.device)
-      if frontier.numel() == 0:
-        break
-    e = torch.empty(0, dtype=torch.int64, device=self.device)
-    node = table.keys(0)
-    return SamplerOutput(node=node, row=torch.cat(rows) if rows else e, col=torch.cat(cols) if cols else e.clone(),
-                         edge=(torch.cat(eids) if eids else e.clone()) if self.with_edge else None,
-                         batch=node[:n0], num_sampled_nodes=nn, num_sampled_edges=ne, device=self.device)
+    return await self._drive(self.sampler._homo_loop(seeds))
 
   async def _hetero_from_seeds(self, seeds_dict: Dict[NodeType, torch.Tensor]) -> HeteroSamplerOutput:
     if not self._remote:
       return self.sampler._hetero_sample_from_nodes(seeds_dict)
-    s = self.sampler
-    cap = s._hetero_table_cap(sum(v.numel() for v in seeds_dict.values()))
-    tables: Dict[NodeType, IdTable] = {}
-
-    n_seed_total = sum(v.numel() for v in seeds_dict.values())
-
-    def table_of(nt):
-      if nt not in tables:
-        # global node count of the type, when the partition book can tell (the local shard cannot)
-        pb = self.data.node_pb.get(nt) if isinstance(self.data.node_pb, dict) else None
-        total = None
-        if isinstance(pb, torch.Tensor):
-          total = pb.numel()
-        elif hasattr(pb, 'partition_bounds'):
-          total = int(pb.partition_bounds[-1])
-        elif hasattr(pb, '_ranges'):
-          total = int(pb._ranges[-1])
-        bound = s._hetero_type_bound(nt, n_seed_total, total) if total is not None else None
-        tables[nt] = IdTable(self.device, min(cap, bound) if bound else cap)
-      return tables[nt]
-    src_dict, src_local, num_nodes, num_edges = {}, {}, {}, {}
-    for nt, sd in seeds_dict.items():
-      t = table_of(nt)
-      t.init(sd)
-      src_dict[nt] = t.keys(0)
-      src_local[nt] = torch.arange(t.size(), dtype=torch.int64, device=self.device)
-    count_dict(src_dict, num_nodes, 1)
-    batch = {nt: v.clone() for nt, v in src_dict.items()}
-    rows, cols, eids = {}, {}, {}
-    n_et = max(1, len(s.edge_types))
-    stream = s._next_stream(s.num_hops * n_et)
-    for h in range(s.num_hops):
-      before = {nt: t.size() for nt, t in tables.items()}
-      tasks = []
-      for ei, etype in enumerate(s.edge_types):
-        src_t, nbr_t = s._etype_ends(etype)
-        src = src_dict.get(src_t)
-        if src is None or src.numel() == 0:
-          continue
-        tasks.append((etype, src_t, nbr_t,
-                      asyncio.ensure_future(self._sample_one_hop(src, s.num_neighbors[etype][h], etype,
-                                                                 stream + h * n_et + ei))))
-      hop_edges = {}
-      for etype, src_t, nbr_t, task in tasks:
-        out = await task
-        if out.nbr.numel() == 0:
-          continue
-        nbr_local = table_of(nbr_t).insert(out.nbr)
-        s_local = torch.repeat_interleave(src_local[src_t], out.nbr_num.to(self.device))
-        key = reverse_edge_type(etype) if self.edge_dir == 'out' else etype
-        rows.setdefault(key, []).append(nbr_local)
-        cols.setdefault(key, []).append(s_local)
-        if out.edge is not None:
-          eids.setdefault(key, []).append(out.edge)
-        hop_edges[key] = out.nbr
-      new_src, new_local = {}, {}
-      for nt, t in tables.items():
-        b = before.get(nt, 0)
-        if t.size() > b:
-          new_src[nt] = t.keys(b)
-          new_local[nt] = torch.arange(b, t.size(), dtype=torch.int64, device=self.device)
-      count_dict(new_src, num_nodes, h + 2)
-      count_dict(hop_edges, num_edges, h + 1)
-      src_dict, src_local = new_src, new_local
-      if not new_src:
-        break
-    out_types = [reverse_edge_type(et) if self.edge_dir == 'out' else et for et in s.edge_types]
-    return HeteroSamplerOutput(
-      node={nt: t.keys(0) for nt, t in tables.items()},
-      row={k: torch.cat(v) for k, v in rows.items()}, col={k: torch.cat(v) for k, v in cols.items()},
-      edge={k: torch.cat(v) for k, v in eids.items()} if self.with_edge else None, batch=batch,
-      num_sampled_nodes={k: torch.as_tensor(v, dtype=torch.int64) for k, v in num_nodes.items()},
-      num_sampled_edges={k: torch.as_tensor(v, dtype=torch.int64) for k, v in num_edges.items()},
-      edge_types=out_types, device=self.device)
+    # global node count of each type the partition book can tell (the local shard cannot)
+    totals = {}
+    for nt, pb in (self.data.node_pb.items() if isinstance(self.data.node_pb, dict) else ()):
+      if isinstance(pb, torch.Tensor):
+        totals[nt] = pb.numel()
+      elif hasattr(pb, 'partition_bounds'):
+        totals[nt] = int(pb.partition_bounds[-1])
+      elif hasattr(pb, '_ranges'):
+        totals[nt] = int(pb._ranges[-1])
+    return await self._drive(self.sampler._hetero_loop(seeds_dict, totals))
 
   # ------------------------------------------------------------------ from edges
   async def _sample_from_edges(self, inputs: EdgeSamplerInput):
     """Negatives are drawn against the *local* graph view: strict on the p2p plane (the
     view spans every shard), local-partition-only on the rpc plane like the reference
     (dist_neighbor_sampler.py:411-413)."""
-    src = inputs.row.to(self.device, dtype=torch.int64)
-    dst = inputs.col.to(self.device, dtype=torch.int64)
-    edge_label = inputs.label.to(self.device) if inputs.label is not None else None
-    input_type, neg = inputs.input_type, inputs.neg_sampling
-    num_pos = src.numel()
-    if neg is not None:
-      self.sampler.with_neg = True
-      self.sampler.lazy_init_sampler()
-      self.sampler.lazy_init_neg_sampler()
-      ns = self.sampler._neg_sampler if self.data_cls == 'homo' else self.sampler._neg_sampler[input_type]
-      num_neg = math.ceil(num_pos * neg.amount)
-      pair = ns.sample(num_neg, padding=True).to(self.device)
-      if neg.is_binary():
-        src, dst = torch.cat([src, pair[0]]), torch.cat([dst, pair[1]])
-        if edge_label is None:
-          edge_label = torch.ones(num_pos, device=self.device)
-        edge_label = torch.cat([edge_label, edge_label.new_zeros((pair.shape[1],) + tuple(edge_label.shape[1:]))])
-      else:
-        dst = torch.cat([dst, pair[1]])
+    seeds, metadata = self.sampler._link_seeds(inputs)
     if self.data_cls == 'homo':
-      seed, inverse = torch.unique(torch.cat([src, dst]), return_inverse=True)
-      out = await self._homo_from_seeds(seed)
-      NeighborSampler._attach_link_metadata(out, neg, inverse, num_pos, edge_label, src.numel())
-      return out
-    src_t, dst_t = input_type[0], input_type[-1]
-    if src_t == dst_t:
-      seed, inverse = torch.unique(torch.cat([src, dst]), return_inverse=True)
-      seeds_dict = {src_t: seed}
-      inv_src, inv_dst = inverse[:src.numel()], inverse[src.numel():]
+      out = await self._homo_from_seeds(seeds)
     else:
-      s_seed, inv_src = torch.unique(src, return_inverse=True)
-      d_seed, inv_dst = torch.unique(dst, return_inverse=True)
-      seeds_dict = {src_t: s_seed, dst_t: d_seed}
-    out = await self._hetero_from_seeds(seeds_dict)
-    out.input_type = input_type
-    if neg is None or neg.is_binary():
-      out.metadata = {'edge_label_index': torch.stack([inv_src, inv_dst]), 'edge_label': edge_label}
-    else:
-      out.metadata = {'src_index': inv_src[:num_pos], 'dst_pos_index': inv_dst[:num_pos],
-                      'dst_neg_index': inv_dst[num_pos:].view(num_pos, -1)}
+      out = await self._hetero_from_seeds(seeds)
+      out.input_type = inputs.input_type
+    out.metadata = metadata
     return out
 
   # ------------------------------------------------------------------ subgraph
@@ -355,17 +238,7 @@ class DistNeighborSampler(ConcurrentEventLoop):
       out = self.sampler.subgraph(NodeSamplerInput(seeds))
       out.batch = seeds
       return out
-    nodes = [seeds]
-    if self.num_neighbors is not None:
-      frontier = torch.unique(seeds)
-      stream = self.sampler._next_stream(len(self.num_neighbors))
-      for h, k in enumerate(self.num_neighbors):
-        nbr = (await self._sample_one_hop(frontier, k, None, stream + h)).nbr
-        if nbr.numel() == 0:
-          break
-        frontier = torch.unique(nbr)
-        nodes.append(frontier)
-    node = torch.unique(torch.cat(nodes))          # ascending ids, like the single-machine subgraph()
+    node = torch.unique(await self._drive(self.sampler._subgraph_loop(seeds)))   # ascending ids, like subgraph()
     owners = self.dist_graph.get_node_partitions(node, None)
     futs, rows_g, cols_g, eids_g = [], [], [], []
     for p in range(self.num_partitions):

@@ -269,10 +269,23 @@ class NeighborSampler(BaseSampler):
       return SamplerOutput(node=node, row=nbr_local, col=tgt_local, edge=eids if self.with_edge else None,
                            batch=node[:nn[0]], num_sampled_nodes=nn, num_sampled_edges=ne,
                            device=self.device)
-    return self._generic_sample_from_nodes(seeds)
+    return self._drive(self._homo_loop(seeds))
 
-  def _generic_sample_from_nodes(self, seeds: torch.Tensor) -> SamplerOutput:
-    """Hop-by-hop path (CPU, or -1 fanouts): one-hop sampler + IdTable."""
+  # ------------------------------------------------------------------ hop loops
+  # A hop loop is a generator: it yields the one-hop requests of a hop as a list of (ids, k, etype, stream), is sent
+  # back their NeighborOutputs in the same order and finally returns its result.  `_drive` serves the requests here;
+  # DistNeighborSampler serves them over the graph's partitions.
+  def _drive(self, loop):
+    outs = None
+    while True:
+      try:
+        reqs = loop.send(outs)
+      except StopIteration as done:
+        return done.value
+      outs = [self.sample_one_hop(*r) for r in reqs]
+
+  def _homo_loop(self, seeds: torch.Tensor):
+    """Hop-by-hop sample of a homogeneous graph (CPU, -1 fanouts, partitioned graphs): one-hop sampler + IdTable."""
     table = IdTable(self.device, self._max_sampled_nodes(seeds.numel()))
     table.init(seeds)
     n0 = table.size()
@@ -282,7 +295,7 @@ class NeighborSampler(BaseSampler):
     nn, ne = [n0], []
     stream = self._next_stream(len(self.num_neighbors))
     for h, k in enumerate(self.num_neighbors):
-      out = self.sample_one_hop(frontier, k, stream=stream + h)
+      out, = yield [(frontier, k, None, stream + h)]
       if out.nbr.numel() == 0:
         break
       before = table.size()
@@ -357,9 +370,6 @@ class NeighborSampler(BaseSampler):
   def _hetero_arena_ok(self) -> bool:
     if not self.is_cuda or self.num_hops > 4 or self.num_hops < 1:
       return False
-    import os
-    if os.environ.get('GLT_B200_HETERO_ARENA', '1') == '0':
-      return False
     return all(0 <= int(k) <= 512 for v in self.num_neighbors.values() for k in v)
 
   def _get_hetero_arena(self, seed_counts: Dict[NodeType, int]):
@@ -425,13 +435,23 @@ class NeighborSampler(BaseSampler):
   def _hetero_sample_from_nodes(self, seeds_dict: Dict[NodeType, torch.Tensor]) -> HeteroSamplerOutput:
     if self._hetero_arena_ok():
       return self._hetero_arena_sample({nt: v.to(self.device, dtype=torch.int64) for nt, v in seeds_dict.items()})
+    return self._drive(self._hetero_loop(seeds_dict))
+
+  def _hetero_loop(self, seeds_dict: Dict[NodeType, torch.Tensor],
+                   type_totals: Optional[Dict[NodeType, int]] = None):
+    """Hop-by-hop sample of a heterogeneous graph: per-type IdTables, one request per relation with a frontier.
+    `type_totals` (node count of each type, for graphs this process holds only a shard of) bounds the tables in
+    place of the local graph sizes; a type it leaves out gets the fan-out bound alone."""
     n_seed_total = sum(v.numel() for v in seeds_dict.values())
     cap = self._hetero_table_cap(n_seed_total)
     tables: Dict[NodeType, IdTable] = {}
 
     def table_of(nt):
       if nt not in tables:
-        bound = self._hetero_type_bound(nt, n_seed_total)
+        if type_totals is None:
+          bound = self._hetero_type_bound(nt, n_seed_total)
+        else:
+          bound = self._hetero_type_bound(nt, n_seed_total, type_totals[nt]) if nt in type_totals else None
         tables[nt] = IdTable(self.device, min(cap, bound) if bound else cap)
       return tables[nt]
 
@@ -446,19 +466,21 @@ class NeighborSampler(BaseSampler):
     count_dict(src_dict, num_nodes, 1)
     batch = {nt: v.clone() for nt, v in src_dict.items()}
     rows, cols, eids = {}, {}, {}
-    stream = self._next_stream(self.num_hops * max(1, len(self.edge_types)))
+    n_et = max(1, len(self.edge_types))
+    stream = self._next_stream(self.num_hops * n_et)
     for h in range(self.num_hops):
       before = {nt: t.size() for nt, t in tables.items()}
-      hop_edges: Dict[EdgeType, torch.Tensor] = {}
+      reqs = []
       for ei, etype in enumerate(self.edge_types):
-        src_t, nbr_t = self._etype_ends(etype)
-        src = src_dict.get(src_t)
-        if src is None or src.numel() == 0:
-          continue
-        out = self.sample_one_hop(src, self.num_neighbors[etype][h], etype,
-                                  stream=stream + h * len(self.edge_types) + ei)
+        src = src_dict.get(self._etype_ends(etype)[0])
+        if src is not None and src.numel() > 0:
+          reqs.append((src, self.num_neighbors[etype][h], etype, stream + h * n_et + ei))
+      outs = yield reqs
+      hop_edges: Dict[EdgeType, torch.Tensor] = {}
+      for (_, _, etype, _), out in zip(reqs, outs):
         if out.nbr.numel() == 0:
           continue
+        src_t, nbr_t = self._etype_ends(etype)
         nbr_local = table_of(nbr_t).insert(out.nbr)
         s_local = torch.repeat_interleave(src_local[src_t], out.nbr_num)
         key = reverse_edge_type(etype) if self.edge_dir == 'out' else etype
@@ -493,6 +515,18 @@ class NeighborSampler(BaseSampler):
     """Link sampling with optional binary / triplet negatives (PyG semantics;
     reference neighbor_sampler.py:319-446)."""
     inputs = EdgeSamplerInput.cast(inputs)
+    seeds, metadata = self._link_seeds(inputs)
+    if self._g_cls == 'homo':
+      out = self._sample_from_nodes(seeds)
+    else:
+      out = self._hetero_sample_from_nodes(seeds)
+      out.input_type = inputs.input_type
+    out.metadata = metadata
+    return out
+
+  def _link_seeds(self, inputs: EdgeSamplerInput):
+    """Negatives, seed dedup and metadata of a link batch -> (seeds: a tensor, or a dict by node type on
+    heterogeneous graphs, the output's metadata)."""
     src = inputs.row.to(self.device, dtype=torch.int64)
     dst = inputs.col.to(self.device, dtype=torch.int64)
     edge_label = inputs.label.to(self.device) if inputs.label is not None else None
@@ -519,38 +553,18 @@ class NeighborSampler(BaseSampler):
         dst = torch.cat([dst, neg_pair[1].to(self.device)])
         assert edge_label is None, 'triplet mode does not take edge labels'
 
-    if self._g_cls == 'homo':
-      seed = torch.cat([src, dst])
-      seed, inverse = torch.unique(seed, return_inverse=True)
-      out = self._sample_from_nodes(seed)
-      self._attach_link_metadata(out, neg, inverse, num_pos, edge_label, src.numel())
-      return out
-
-    src_t, dst_t = input_type[0], input_type[-1]
-    if src_t == dst_t:
+    if self._g_cls == 'homo' or input_type[0] == input_type[-1]:
       seed, inverse = torch.unique(torch.cat([src, dst]), return_inverse=True)
-      seeds_dict = {src_t: seed}
+      seeds = seed if self._g_cls == 'homo' else {input_type[0]: seed}
       inv_src, inv_dst = inverse[:src.numel()], inverse[src.numel():]
     else:
       s_seed, inv_src = torch.unique(src, return_inverse=True)
       d_seed, inv_dst = torch.unique(dst, return_inverse=True)
-      seeds_dict = {src_t: s_seed, dst_t: d_seed}
-    out = self._hetero_sample_from_nodes(seeds_dict)
-    out.input_type = input_type
+      seeds = {input_type[0]: s_seed, input_type[-1]: d_seed}
     if neg is None or neg.is_binary():
-      out.metadata = {'edge_label_index': torch.stack([inv_src, inv_dst]), 'edge_label': edge_label}
-    else:
-      out.metadata = {'src_index': inv_src[:num_pos], 'dst_pos_index': inv_dst[:num_pos],
-                      'dst_neg_index': inv_dst[num_pos:].view(num_pos, -1)}
-    return out
-
-  @staticmethod
-  def _attach_link_metadata(out, neg, inverse, num_pos, edge_label, n_src):
-    if neg is None or neg.is_binary():
-      out.metadata = {'edge_label_index': inverse.view(2, -1), 'edge_label': edge_label}
-    else:
-      out.metadata = {'src_index': inverse[:num_pos], 'dst_pos_index': inverse[num_pos:2 * num_pos],
-                      'dst_neg_index': inverse[2 * num_pos:].view(num_pos, -1)}
+      return seeds, {'edge_label_index': torch.stack([inv_src, inv_dst]), 'edge_label': edge_label}
+    return seeds, {'src_index': inv_src[:num_pos], 'dst_pos_index': inv_dst[:num_pos],
+                   'dst_neg_index': inv_dst[num_pos:].view(num_pos, -1)}
 
   # ------------------------------------------------------------------ PyG v1
   def sample_pyg_v1(self, ids: torch.Tensor):
@@ -578,20 +592,25 @@ class NeighborSampler(BaseSampler):
     seeds = inputs.node.to(self.device, dtype=torch.int64)
     assert self._g_cls == 'homo', 'subgraph sampling supports homogeneous graphs'
     self.lazy_init_sampler()
+    all_nodes = self._drive(self._subgraph_loop(seeds))
+    node, rows, cols, eids, mapping = self.node_subgraph(all_nodes, seeds.numel())
+    return SamplerOutput(node=node, row=rows, col=cols, edge=eids if self.with_edge else None,
+                         device=self.device, metadata=mapping)
+
+  def _subgraph_loop(self, seeds: torch.Tensor):
+    """k-hop node expansion of a subgraph sample, as a hop loop: returns the seeds followed by the unique
+    neighbours of every hop."""
     nodes = [seeds]
     if self.num_neighbors is not None:
       frontier = torch.unique(seeds)
       stream = self._next_stream(len(self.num_neighbors))
       for h, k in enumerate(self.num_neighbors):
-        nbr = self.sample_one_hop(frontier, k, stream=stream + h).nbr
-        if nbr.numel() == 0:
+        out, = yield [(frontier, k, None, stream + h)]
+        if out.nbr.numel() == 0:
           break
-        nodes.append(torch.unique(nbr))
-        frontier = nodes[-1]
-    all_nodes = torch.cat(nodes)
-    node, rows, cols, eids, mapping = self.node_subgraph(all_nodes, seeds.numel())
-    return SamplerOutput(node=node, row=rows, col=cols, edge=eids if self.with_edge else None,
-                         device=self.device, metadata=mapping)
+        frontier = torch.unique(out.nbr)
+        nodes.append(frontier)
+    return torch.cat(nodes)
 
   def node_subgraph(self, all_nodes: torch.Tensor, num_seeds: int = 0):
     """Induced subgraph on exactly `all_nodes` (no neighbourhood expansion).

@@ -248,6 +248,53 @@ def test_dist_hetero_neighbor_loader(edge_dir):
   run_workers(_w_hetero_loader, args=(edge_dir,), timeout=300)
 
 
+def _w_rpc_sample_matches_single_process(rank, world, port):
+  import graphlearn_for_pytorch_b200 as glt
+  import graphlearn_for_pytorch_b200.distributed as d
+  from dist_utils import build_hetero_partition
+  from graphlearn_for_pytorch_b200.sampler import (EdgeSamplerInput, NegativeSampling, NeighborSampler,
+                                                    NodeSamplerInput)
+  from graphlearn_for_pytorch_b200.typing import as_str
+  d.init_worker_group(world, rank)
+  d.init_rpc('127.0.0.1', port)
+  ds, edges = build_hetero_partition(rank, world, 'out')
+  # full neighbourhoods: the sample depends neither on the Philox streams nor on the order of a shard's rows
+  s = d.DistNeighborSampler(ds, [-1, -1], with_edge=True, edge_dir='out', seed=5)
+  s.start_loop()
+  seeds = torch.arange(rank, 20, 3)
+  msg = s.sample_from_nodes(NodeSamplerInput(seeds, 'user'))
+  whole = glt.data.Dataset(edge_dir='out')
+  whole.init_graph(edges, graph_mode='CPU', num_nodes={'user': 20, 'item': 20})
+  ref = NeighborSampler(whole.graph, [-1, -1], with_edge=True, seed=5).sample_from_nodes(NodeSamplerInput(seeds, 'user'))
+  assert {k[:-len('.ids')] for k in msg if k.endswith('.ids')} == {as_str(nt) for nt in ref.node}
+  for nt in ref.node:
+    assert set(msg[f'{as_str(nt)}.ids'].tolist()) == set(ref.node[nt].tolist()), nt
+    # 'user' only appears at hop 0: no trailing zero hops
+    assert msg[f'{as_str(nt)}.num_sampled_nodes'].tolist() == ref.num_sampled_nodes[nt].tolist(), nt
+  assert {k[:-len('.rows')] for k in msg if k.endswith('.rows')} == {as_str(et) for et in ref.row}
+  for et in ref.row:
+    k = as_str(et)
+    got = zip(msg[f'{as_str(et[0])}.ids'][msg[f'{k}.rows']].tolist(),
+              msg[f'{as_str(et[2])}.ids'][msg[f'{k}.cols']].tolist(), msg[f'{k}.eids'].tolist())
+    want = zip(ref.node[et[0]][ref.row[et]].tolist(), ref.node[et[2]][ref.col[et]].tolist(), ref.edge[et].tolist())
+    assert set(got) == set(want), et
+    assert msg[f'{k}.num_sampled_edges'].tolist() == ref.num_sampled_edges[et].tolist(), et
+  # triplet link sampling takes no edge labels, as on one process
+  with pytest.raises(AssertionError, match='triplet mode does not take edge labels'):
+    s.sample_from_edges(EdgeSamplerInput(torch.tensor([0, 1]), torch.tensor([0, 1]), label=torch.ones(2),
+                                         input_type=('user', 'u2i', 'item'),
+                                         neg_sampling=NegativeSampling('triplet', 1)))
+  s.shutdown_loop()
+  d.barrier()
+  d.shutdown_rpc()
+
+
+def test_rpc_hetero_sample_matches_single_process():
+  """The rpc data plane returns the sample of a NeighborSampler over the whole graph: the same node and edge sets
+  and the same per-hop counts."""
+  run_workers(_w_rpc_sample_matches_single_process, timeout=300)
+
+
 def _w_dist_table(rank, world, port, out):
   import numpy as np
   import graphlearn_for_pytorch_b200.distributed as d

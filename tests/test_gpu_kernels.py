@@ -293,8 +293,8 @@ def test_hetero_and_link_sampling_gpu_matches_cpu(native):
 def test_hetero_arena_igbh_shape_matches_cpu_sampler(native):
   """Native grouped hetero sampler/inducer (HeteroArena) on an IGBH-shaped schema (4 node types, 7 relations,
   3 hops, edge_dir='in'): the sampled edge SET of every relation and the node set of every type must equal the
-  CPU sampler's (same Philox streams), local ids must be hop-contiguous, and the generic per-relation device path
-  (GLT_B200_HETERO_ARENA=0) must agree as well."""
+  CPU sampler's (same Philox streams), local ids must be hop-contiguous, and the generic per-relation hop loop on
+  the device must agree as well."""
   import os
   sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), 'examples'))
   from common import synthetic_igbh
@@ -306,11 +306,9 @@ def test_hetero_arena_igbh_shape_matches_cpu_sampler(native):
     ds.init_graph(edges, graph_mode='CPU' if mode == 'CPU' else 'CUDA', device=0, num_nodes=sizes)
     s = NeighborSampler(ds.graph, [4, 3, 2], seed=9, device=None if mode == 'CPU' else DEV, edge_dir='in')
     if mode == 'CUDA-generic':
-      os.environ['GLT_B200_HETERO_ARENA'] = '0'
-    try:
+      outs[mode] = [s._drive(s._hetero_loop({'paper': seeds.to(DEV)})) for _ in range(2)]
+    else:
       outs[mode] = [s.sample_from_nodes(NodeSamplerInput(seeds, 'paper')) for _ in range(2)]
-    finally:
-      os.environ.pop('GLT_B200_HETERO_ARENA', None)
   for it in range(2):
     a = outs['CPU'][it]
     for other in ('CUDA', 'CUDA-generic'):
