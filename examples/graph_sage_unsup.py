@@ -4,6 +4,9 @@
   python examples/graph_sage_unsup.py                  # LinkNeighborLoader + eager GraphSAGE + torch Adam
   python examples/graph_sage_unsup.py --mode engine    # GraphSageLinkEngine (GraphSageLinkTrainer without a GPU),
                                                        # then the held-out link AUC of the inference() embeddings
+  python examples/graph_sage_unsup.py --mode engine --rank-k 20
+                                                       # also recall@20 of the held-out edges over every node
+                                                       # (training edges excluded), Hits@20 and MRR
 """
 import argparse
 
@@ -18,6 +21,8 @@ p = argparse.ArgumentParser()
 p.add_argument('--mode', default='loader', choices=['loader', 'engine'])
 p.add_argument('--epochs', type=int, default=2)
 p.add_argument('--steps-per-epoch', type=int, default=40, help='engine mode: training steps per epoch')
+p.add_argument('--rank-k', type=int, default=0,
+               help='engine mode: also rank every node for each held-out edge endpoint and print recall@K, Hits@K, MRR')
 args = p.parse_args()
 
 cuda = torch.cuda.is_available()
@@ -57,23 +62,41 @@ def run_engine():
   topo = glt.data.Topology(torch.cat([train, train.flip(0)], 1), layout='CSR', num_nodes=N)
   in_dim = (x.shape[1] + 7) // 8 * 8                       # the engine wants feature rows of a multiple of 8
   feats = F.pad(x, (0, in_dim - x.shape[1]))
+  graph = glt.data.Graph(topo, 'CUDA' if cuda else 'CPU', 0 if cuda else None)
   if cuda:
-    graph = glt.data.Graph(topo, 'CUDA', 0)
     ut = glt.data.UnifiedTensor(0, torch.bfloat16)
     ut.append_shared_tensor(feats.to(device, torch.bfloat16))
     model = GraphSageLinkEngine(graph, ut._table(), in_dim, N, fanouts=[10, 10], batch_size=bs, hidden=64,
                                 out_channels=64, lr=5e-3, device=device)
     model.warmup_and_capture(n_eager=1)
   else:
-    model = GraphSageLinkTrainer(glt.data.Graph(topo, 'CPU'), feats, in_dim, fanouts=[10, 10], hidden=64,
+    model = GraphSageLinkTrainer(graph, feats, in_dim, fanouts=[10, 10], hidden=64,
                                  out_channels=64, lr=5e-3)
   for epoch in range(args.epochs):
     perm = train[:, torch.randperm(train.shape[1], generator=g)[:args.steps_per_epoch * bs]]
     losses = [float(model.train_step(perm[:, i:i + bs])) for i in range(0, perm.shape[1], bs)]
     print(f'epoch {epoch}: loss {sum(losses) / len(losses):.4f}')
   neg = torch.randint(0, N, (2, n_held), generator=g)     # as many uniform random pairs as held-out edges
-  emb = model.inference().cpu()
+  emb_dev = model.inference()
+  emb = emb_dev.cpu()
   print(f'held-out link AUC {link_auc(emb, held, neg):.4f} ({n_held} edges vs {n_held} random pairs)')
+  if args.rank_k > 0:
+    rank_report(emb_dev, graph, held, neg, N)
+
+
+def rank_report(emb, graph, held, neg, N):
+  """recall@K of the held-out edges over every node (training edges excluded), and Hits@K / MRR of the held-out edges
+  against the random pairs."""
+  from graphlearn_for_pytorch_b200.models import link_hits_at_k, link_mrr, link_recall_at_k, link_scores, link_topk
+  K = args.rank_k
+  truth = glt.data.Topology(torch.cat([held, held.flip(0)], 1), layout='CSR', num_nodes=N)
+  queries = torch.unique(held).to(emb.device)
+  ids, _ = link_topk(emb, queries, K, exclude=graph)
+  recall, hit = link_recall_at_k(ids, (truth.indptr, truth.indices), queries)
+  pos, negs = link_scores(emb, held), link_scores(emb, neg)
+  print(f'held-out recall@{K} {recall:.4f} (hit rate {hit:.4f}, {queries.numel()} query nodes, training edges '
+        f'excluded); Hits@{K} {link_hits_at_k(pos, negs, K):.4f}, '
+        f'MRR {link_mrr(pos, negs.unsqueeze(0).expand(pos.numel(), -1)):.4f} against the random pairs')
 
 
 run_loader() if args.mode == 'loader' else run_engine()

@@ -1094,6 +1094,86 @@ static Tensor label_prop(GraphHandle* graph, const Tensor& base, int64_t c, int6
   return buf[(num_layers - 1) & 1];
 }
 
+// Exact top-k of <emb[q], emb[c]> over the candidate ids c of [lo, hi) for every query q (csrc/cuda/link_topk.cu), with
+// q itself and the columns of row q of `exclude` never returned.  emb: bf16 [N, d]; queries: int64 [n] in [0, N).
+// Returns (ids int64 [n, k], scores fp32 [n, k]), (score desc, id asc), padded with (-1, -inf).  splits = 0 picks the
+// candidate split count from n and the SM count; any count gives bitwise identical results.
+static std::tuple<Tensor, Tensor> link_topk(const Tensor& emb, const Tensor& queries, int64_t k, int64_t lo, int64_t hi,
+                                            GraphHandle* exclude, int64_t splits) {
+  TORCH_CHECK(emb.is_cuda(), "link_topk: emb must be a CUDA tensor");
+  c10::cuda::CUDAGuard guard(emb.device());
+  TORCH_CHECK(emb.dim() == 2, "link_topk: emb must be 2-D [N, d]");
+  const int64_t N = emb.size(0), d = emb.size(1);
+  TORCH_CHECK(d % 8 == 0 && d >= 8 && d <= 512,
+              fmt("link_topk: width %lld, the kernel takes a multiple of 8 in [8, 512]", static_cast<long long>(d)));
+  check_rows(emb, torch::kBFloat16, d, "link_topk: emb must be contiguous, 16-byte aligned bf16 [N, d]");
+  TORCH_CHECK(k >= 1 && k <= 128, fmt("link_topk: k = %lld, the kernel takes 1 to 128", static_cast<long long>(k)));
+  TORCH_CHECK(lo >= 0 && lo <= hi && hi <= N,
+              fmt("link_topk: candidate range [%lld, %lld) is not inside [0, %lld)", static_cast<long long>(lo),
+                  static_cast<long long>(hi), static_cast<long long>(N)));
+  TORCH_CHECK(hi - lo < (int64_t(1) << 31), "link_topk: at most 2^31 - 1 candidates");
+  TORCH_CHECK(N < (int64_t(1) << 32) - 1, "link_topk: at most 2^32 - 2 nodes");
+  TORCH_CHECK(queries.dim() == 1, "link_topk: queries must be 1-D");
+  check_ids(queries, "link_topk: queries must be contiguous int64 on emb's device");
+  TORCH_CHECK(splits >= 0, "link_topk: splits must be >= 0 (0: chosen from n)");
+  if (exclude != nullptr)
+    TORCH_CHECK(exclude->tbl.num_parts == 0 || exclude->device == emb.get_device(),
+                "link_topk: the exclusion graph must live on emb's device");
+  const int64_t n = queries.numel();
+  const auto i64 = queries.options();
+  Tensor ids = torch::full({n, k}, -1, i64);
+  Tensor scores = torch::full({n, k}, -std::numeric_limits<float>::infinity(), emb.options().dtype(torch::kFloat32));
+  if (n == 0) return {ids, scores};
+  const int64_t qmin = queries.min().item<int64_t>(), qmax = queries.max().item<int64_t>();
+  TORCH_CHECK(qmin >= 0 && qmax < N, fmt("link_topk: query ids must lie in [0, %lld), got [%lld, %lld]",
+                                         static_cast<long long>(N), static_cast<long long>(qmin),
+                                         static_cast<long long>(qmax)));
+  if (hi == lo) return {ids, scores};
+
+  int smem_optin = 0;
+  cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, emb.get_device());
+  const int stages = link_topk_stages(static_cast<int>(d), static_cast<int>(k), static_cast<size_t>(smem_optin));
+  TORCH_CHECK(stages > 0, "link_topk: the device has too little shared memory for this width and k");
+  const int64_t q_tiles = (n + 63) / 64, c_tiles = (hi - lo + 63) / 64;
+  TORCH_CHECK(q_tiles < (int64_t(1) << 31), "link_topk: too many queries");
+  if (splits == 0) {   // one wave: every resident CTA slot busy, as few splits as that takes
+    int sms = 0;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, emb.get_device());
+    const int64_t slots = static_cast<int64_t>(sms) * link_topk_ctas_per_sm(static_cast<int>(d), static_cast<int>(k), stages);
+    splits = std::max<int64_t>(1, std::min<int64_t>(64, slots / q_tiles));
+  }
+  splits = std::min(splits, c_tiles);
+  TORCH_CHECK(splits <= 65535, "link_topk: at most 65535 splits");
+  const int64_t per = (c_tiles + splits - 1) / splits;
+  splits = (c_tiles + per - 1) / per;   // no empty split
+
+  Tensor qrows = emb.index_select(0, queries);
+  Tensor part = torch::empty({splits, n, k}, i64);
+  LinkTopkLaunch L{};
+  int rc = make_tmap_bf16_2d(L.maps[0], qrows.data_ptr(), n, d, d, 64, 64);
+  TORCH_CHECK(rc == 0, fmt("link_topk: cuTensorMapEncodeTiled failed for the query rows (rc=%d)", rc));
+  rc = make_tmap_bf16_2d(L.maps[1], static_cast<const at::BFloat16*>(emb.data_ptr()) + lo * d, hi - lo, d, d, 64, 64);
+  TORCH_CHECK(rc == 0, fmt("link_topk: cuTensorMapEncodeTiled failed for the candidate rows (rc=%d)", rc));
+  LinkTopkArgs& a = L.args;
+  if (exclude != nullptr) a.g = exclude->tbl;
+  else a.g.num_parts = 0;
+  a.queries = queries.data_ptr<int64_t>();
+  a.n = n;
+  a.lo = lo;
+  a.hi = hi;
+  a.d = static_cast<int>(d);
+  a.k = static_cast<int>(k);
+  a.part_keys = part.data_ptr<int64_t>();
+  a.ids = ids.data_ptr<int64_t>();
+  a.scores = scores.data_ptr<float>();
+  L.splits = static_cast<int>(splits);
+  L.tiles_per_split = static_cast<int>(per);
+  L.stages = stages;
+  launch_link_topk(L, cur_stream());
+  check_cuda_err("link_topk");
+  return {ids, scores};
+}
+
 static void add_block_f32(const Tensor& dA, int64_t col, int64_t d, const Tensor& counters, int64_t n_hops, Tensor dH) {
   c10::cuda::CUDAGuard guard(dA.device());
   TORCH_CHECK(d % 8 == 0, "add_block_f32: d must be a multiple of 8");
@@ -2672,6 +2752,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("bias"), py::arg("relu"), py::arg("out"), py::arg("mean_only") = false);
   m.def("label_prop", &label_prop, py::arg("graph"), py::arg("base"), py::arg("c"), py::arg("num_layers"),
         py::arg("alpha"), py::arg("norm"), py::arg("lo"), py::arg("hi"), py::arg("fixed") = py::none());
+  m.def("link_topk", &link_topk, py::arg("emb"), py::arg("queries"), py::arg("k"), py::arg("lo"), py::arg("hi"),
+        py::arg("exclude") = nullptr, py::arg("splits") = 0);
   m.def("sage_aggregate_block", &sage_aggregate_block);
   m.def("sage_scatter_block", &sage_scatter_block);
   m.def("add_block_f32", &add_block_f32);

@@ -766,6 +766,34 @@ struct HgtFullAttnArgs {
 };
 void launch_hgt_full_attention(const HgtFullAttnArgs& a, cudaStream_t s);
 
+// ---- link_topk.cu (exact top-K link retrieval over a candidate id range) ---------------------------------------
+// For every query row i of [0, n): the k ids c of [lo, hi) with the largest fp32 <emb[queries[i]], emb[c]> (bf16
+// wgmma, fp32 accumulation), ordered by (score desc, id asc), excluding queries[i] itself and the columns of row
+// queries[i] of g (column-sorted; g.num_parts = 0 or a row past the graph excludes nothing).  Slots past the number of
+// eligible candidates get id -1 and score -inf.
+struct LinkTopkArgs {
+  GraphTable g;
+  const int64_t* queries;       // [n], each in [0, N)
+  int64_t n;
+  int64_t lo, hi;               // candidate ids [lo, hi), hi - lo < 2^31
+  int d, k;                     // d a multiple of 8 in [8, 512], k in [1, 128]
+  int64_t* part_keys;           // scratch [splits, n, k]
+  int64_t* ids;                 // [n, k]
+  float* scores;                // [n, k]
+};
+struct alignas(64) LinkTopkLaunch {
+  unsigned char maps[2][128];   // CUtensorMap: gathered query rows bf16 [n, d]; candidate rows bf16 [hi - lo, d]
+  LinkTopkArgs args;
+  int splits, tiles_per_split;  // candidate tiles of 64 ids per split; every split non-empty
+  int stages;                   // from link_topk_stages
+};
+// Candidate ring stages that fit `smem_limit` bytes of shared memory at (d, k) (0: none fit).
+int link_topk_stages(int d, int k, size_t smem_limit);
+size_t link_topk_smem_bytes(int d, int k, int stages);
+// resident CTAs per SM at (d, k, stages)
+int link_topk_ctas_per_sm(int d, int k, int stages);
+void launch_link_topk(const LinkTopkLaunch& L, cudaStream_t s);
+
 // programmatic-dependent-launch switch (launch_utils.h); returns the previous value
 int set_pdl(int on);
 void launch_tc_gemm(const TcGemmLaunch& L, int num_sms, cudaStream_t s);
