@@ -2003,6 +2003,188 @@ static void m2v_begin(Tensor state) {
 }
 
 // ---------------------------------------------------------------------------
+// Knowledge-graph embeddings (cuda/kge.cu, models/kge.py).  model: 0 TransE, 1 DistMult, 2 ComplEx, 3 RotatE.
+// ---------------------------------------------------------------------------
+// ent fp32 [N, D * entity parts], rel fp32 [R, D * relation parts], D a multiple of 8 in [8, 512]; returns D.
+static int64_t check_kge_tables(int64_t model, const Tensor& ent, const Tensor& rel, const char* who) {
+  TORCH_CHECK(model >= 0 && model <= 3, fmt("%s: model must be 0 (TransE), 1 (DistMult), 2 (ComplEx) or 3 (RotatE)", who));
+  const int pe = kge_entity_parts(static_cast<int>(model)), pr = kge_relation_parts(static_cast<int>(model));
+  TORCH_CHECK(ent.dim() == 2 && ent.size(1) % pe == 0, fmt("%s: ent must be fp32 [N, %d D]", who, pe));
+  const int64_t D = ent.size(1) / pe;
+  TORCH_CHECK(D % 8 == 0 && D >= 8 && D <= 512, fmt("%s: D must be a multiple of 8 in [8, 512]", who));
+  check_rows(ent, torch::kFloat32, pe * D, fmt("%s: ent must be a contiguous fp32 [N, %d D] tensor on the device", who, pe).c_str());
+  check_rows(rel, torch::kFloat32, pr * D, fmt("%s: rel must be a contiguous fp32 [R, %d D] tensor on the device", who, pr).c_str());
+  TORCH_CHECK(ent.size(0) >= 1 && ent.size(0) < (int64_t(1) << 31) && rel.size(0) >= 1 &&
+              rel.size(0) < (int64_t(1) << 31), fmt("%s: need 1 <= N, R < 2^31", who));
+  return D;
+}
+
+// grad: a contiguous fp32 tensor of t's shape; touched: contiguous uint8 [rows of t]
+static void check_kge_grad(const Tensor& t, const Tensor& grad, const Tensor& touched, const char* who) {
+  check_rows(grad, torch::kFloat32, t.size(1), fmt("%s: gradients must be contiguous fp32 tensors of the tables' shapes", who).c_str());
+  TORCH_CHECK(grad.size(0) == t.size(0), fmt("%s: gradients must be contiguous fp32 tensors of the tables' shapes", who));
+  TORCH_CHECK(on_dev(touched) && touched.scalar_type() == torch::kUInt8 && touched.is_contiguous() &&
+              touched.numel() == t.size(0), fmt("%s: touched flags must be contiguous uint8, one per table row", who));
+}
+
+// neg[i * K + j] of the first min(count[0], B) positives of a batch of B: uniform in [0, N).
+static void kge_negatives(const Tensor& count, int64_t batch_size, int64_t num_neg, int64_t N, int64_t seed,
+                          const Tensor& step, Tensor neg) {
+  c10::cuda::CUDAGuard guard(neg.device());
+  TORCH_CHECK(batch_size >= 1 && num_neg >= 1 && batch_size * num_neg < (int64_t(1) << 31),
+              "kge_negatives: need batch_size, num_neg >= 1 and batch_size * num_neg < 2^31");
+  TORCH_CHECK(N >= 1 && N < (int64_t(1) << 31), "kge_negatives: need 1 <= N < 2^31");
+  check_counters(count, 0, "kge_negatives: count must be int32 [>= 1] on the device");
+  check_counters(step, 0, "kge_negatives: step must be int32 [>= 1] on the device");
+  TORCH_CHECK(neg.dim() == 2 && neg.size(0) == batch_size && neg.size(1) == num_neg,
+              "kge_negatives: neg must be int64 [batch_size, num_neg]");
+  check_ids(neg, "kge_negatives: neg must be contiguous int64 on the device");
+  launch_kge_negatives(count.data_ptr<int32_t>(), static_cast<int>(batch_size), static_cast<int>(num_neg), N,
+                       static_cast<uint64_t>(seed), step.data_ptr<int32_t>(), neg.data_ptr<int64_t>(), cur_stream());
+  check_cuda_err("kge_negatives");
+}
+
+// Loss of the first min(count[0], B) triples of trip (int64 [3, B]) and their negatives (written to loss[0]);
+// gradients red.added into grad_ent / grad_rel, touched flags set for every row looked up.
+static void kge_loss_grad(int64_t model, const Tensor& trip, const Tensor& count, const Tensor& neg, const Tensor& ent,
+                          const Tensor& rel, double margin, int64_t p, Tensor grad_ent, Tensor grad_rel,
+                          Tensor touched_ent, Tensor touched_rel, Tensor loss) {
+  c10::cuda::CUDAGuard guard(ent.device());
+  const int64_t D = check_kge_tables(model, ent, rel, "kge_loss_grad");
+  TORCH_CHECK(trip.dim() == 2 && trip.size(0) == 3 && trip.size(1) >= 1, "kge_loss_grad: trip must be int64 [3, B]");
+  check_ids(trip, "kge_loss_grad: trip must be contiguous int64 on the tables' device");
+  const int64_t B = trip.size(1);
+  TORCH_CHECK(neg.dim() == 2 && neg.size(0) == B && neg.size(1) >= 1 && B * neg.size(1) < (int64_t(1) << 31),
+              "kge_loss_grad: neg must be int64 [B, K]");
+  check_ids(neg, "kge_loss_grad: neg must be contiguous int64 on the tables' device");
+  check_counters(count, 0, "kge_loss_grad: count must be int32 [>= 1] on the device");
+  TORCH_CHECK(p == 1 || p == 2, "kge_loss_grad: p must be 1 or 2");
+  check_kge_grad(ent, grad_ent, touched_ent, "kge_loss_grad");
+  check_kge_grad(rel, grad_rel, touched_rel, "kge_loss_grad");
+  TORCH_CHECK(on_dev(loss) && loss.scalar_type() == torch::kFloat32 && loss.numel() >= 1,
+              "kge_loss_grad: loss must be fp32 [>= 1] on the device");
+  launch_kge_loss_grad(static_cast<int>(model), trip.data_ptr<int64_t>(), static_cast<int>(B),
+                       count.data_ptr<int32_t>(), neg.data_ptr<int64_t>(), static_cast<int>(neg.size(1)),
+                       ent.data_ptr<float>(), rel.data_ptr<float>(), ent.size(0), rel.size(0), static_cast<int>(D),
+                       static_cast<float>(margin), static_cast<int>(p), grad_ent.data_ptr<float>(),
+                       grad_rel.data_ptr<float>(), touched_ent.data_ptr<uint8_t>(), touched_rel.data_ptr<uint8_t>(),
+                       loss.data_ptr<float>(), cur_stream());
+  check_cuda_err("kge_loss_grad");
+}
+
+// h, r, t: int64 [n] on the tables' device, every id in range (checked here, with one host sync)
+static void check_kge_triples(const Tensor& h, const Tensor& r, const Tensor& t, int64_t N, int64_t R, const char* who) {
+  for (const Tensor* x : {&h, &r, &t}) {
+    TORCH_CHECK(x->dim() == 1 && x->numel() == h.numel(), fmt("%s: h, r and t must be 1-D of one length", who));
+    check_ids(*x, fmt("%s: h, r and t must be contiguous int64 on the tables' device", who).c_str());
+  }
+  if (h.numel() == 0) return;
+  const Tensor lo = torch::stack({h.min(), r.min(), t.min()}).cpu(), hi = torch::stack({h.max(), r.max(), t.max()}).cpu();
+  const int64_t* l = lo.data_ptr<int64_t>();
+  const int64_t* u = hi.data_ptr<int64_t>();
+  TORCH_CHECK(l[0] >= 0 && u[0] < N && l[2] >= 0 && u[2] < N, fmt("%s: entity ids must lie in [0, %lld)", who, static_cast<long long>(N)));
+  TORCH_CHECK(l[1] >= 0 && u[1] < R, fmt("%s: relation ids must lie in [0, %lld)", who, static_cast<long long>(R)));
+}
+
+// fp32 [n] scores of the triples (h[i], r[i], t[i]).
+static Tensor kge_score(int64_t model, const Tensor& ent, const Tensor& rel, const Tensor& h, const Tensor& r,
+                        const Tensor& t, double margin, int64_t p) {
+  TORCH_CHECK(ent.is_cuda(), "kge_score: ent must be a CUDA tensor");
+  c10::cuda::CUDAGuard guard(ent.device());
+  const int64_t D = check_kge_tables(model, ent, rel, "kge_score");
+  TORCH_CHECK(p == 1 || p == 2, "kge_score: p must be 1 or 2");
+  check_kge_triples(h, r, t, ent.size(0), rel.size(0), "kge_score");
+  Tensor out = torch::empty({h.numel()}, ent.options());
+  if (h.numel() == 0) return out;
+  launch_kge_score(static_cast<int>(model), h.data_ptr<int64_t>(), r.data_ptr<int64_t>(), t.data_ptr<int64_t>(),
+                   h.numel(), ent.data_ptr<float>(), rel.data_ptr<float>(), static_cast<int>(D),
+                   static_cast<float>(margin), static_cast<int>(p), out.data_ptr<float>(), cur_stream());
+  check_cuda_err("kge_score");
+  return out;
+}
+
+// float64 [n] ranks of the true tail (tail = true) or head among all N entities: 1 + #better + #tied / 2, with the
+// true entity and the ids of the query's range of `keys` (sorted int64 (f R + r) N + c, f the fixed entity) left out.
+// splits = 0 picks the candidate split count from n and the SM count; every count gives the same ranks.
+static Tensor kge_rank(int64_t model, const Tensor& ent, const Tensor& rel, const Tensor& h, const Tensor& r,
+                       const Tensor& t, bool tail, const c10::optional<Tensor>& keys, double margin, int64_t p,
+                       int64_t splits) {
+  TORCH_CHECK(ent.is_cuda(), "kge_rank: ent must be a CUDA tensor");
+  c10::cuda::CUDAGuard guard(ent.device());
+  const int64_t D = check_kge_tables(model, ent, rel, "kge_rank");
+  TORCH_CHECK(p == 1 || p == 2, "kge_rank: p must be 1 or 2");
+  TORCH_CHECK(splits >= 0, "kge_rank: splits must be >= 0 (0: chosen from n)");
+  const int64_t N = ent.size(0), R = rel.size(0), n = h.numel();
+  check_kge_triples(h, r, t, N, R, "kge_rank");
+  if (has(keys)) {
+    TORCH_CHECK(keys->dim() == 1, "kge_rank: keys must be 1-D");
+    check_ids(*keys, "kge_rank: keys must be contiguous int64 on the tables' device");
+  }
+  if (n == 0) return torch::empty({0}, ent.options().dtype(torch::kFloat64));
+  const int64_t q_tiles = (n + 63) / 64, c_tiles = (N + 63) / 64;
+  TORCH_CHECK(q_tiles < (int64_t(1) << 31), "kge_rank: too many queries");
+  if (splits == 0) {   // about two CTAs per SM, as few splits as that takes
+    int sms = 0;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, ent.get_device());
+    splits = std::max<int64_t>(1, (2 * static_cast<int64_t>(sms) + q_tiles - 1) / q_tiles);
+  }
+  splits = std::min(splits, c_tiles);
+  const int64_t per = (c_tiles + splits - 1) / splits;
+  splits = (c_tiles + per - 1) / per;   // no empty split
+  TORCH_CHECK(splits <= 65535, "kge_rank: at most 65535 splits");
+  Tensor q = torch::empty({n, ent.size(1)}, ent.options());
+  Tensor den = torch::empty({model == kKgeTransE ? N : 1}, ent.options());
+  Tensor counts = torch::empty({n}, h.options());
+  KgeRankArgs a{};
+  a.model = static_cast<int>(model);
+  a.D = static_cast<int>(D);
+  a.p = static_cast<int>(p);
+  a.margin = static_cast<float>(margin);
+  a.tail = tail;
+  a.h = h.data_ptr<int64_t>();
+  a.r = r.data_ptr<int64_t>();
+  a.t = t.data_ptr<int64_t>();
+  a.n = n;
+  a.N = N;
+  a.R = R;
+  a.ent = ent.data_ptr<float>();
+  a.rel = rel.data_ptr<float>();
+  a.keys = has(keys) && keys->numel() > 0 ? keys->data_ptr<int64_t>() : nullptr;
+  a.n_keys = has(keys) ? keys->numel() : 0;
+  a.den = den.data_ptr<float>();
+  a.q = q.data_ptr<float>();
+  a.counts = reinterpret_cast<unsigned long long*>(counts.data_ptr<int64_t>());
+  a.splits = static_cast<int>(splits);
+  a.tiles_per_split = static_cast<int>(per);
+  launch_kge_rank(a, cur_stream());
+  check_cuda_err("kge_rank");
+  const Tensor better = counts.bitwise_right_shift(32), tied = counts.bitwise_and(0xFFFFFFFFLL);
+  return better.to(torch::kFloat64) + 1.0 + tied.to(torch::kFloat64) * 0.5;
+}
+
+// torch.optim.SparseAdam step t = step[0] on the touched rows of one KGE table (entity or relation) and its moments;
+// clears their gradient rows and flags.
+static void kge_sparse_adam(Tensor w, Tensor grad, Tensor m, Tensor v, Tensor touched, const Tensor& step, double lr,
+                            double b1, double b2, double eps) {
+  c10::cuda::CUDAGuard guard(w.device());
+  TORCH_CHECK(w.dim() == 2 && w.size(1) % 8 == 0 && w.size(1) >= 8 && w.size(1) <= 1024,
+              "kge_sparse_adam: w must be fp32 [rows, W] with W a multiple of 8 in [8, 1024]");
+  check_rows(w, torch::kFloat32, w.size(1), "kge_sparse_adam: w must be a contiguous fp32 [rows, W] tensor on the device");
+  check_kge_grad(w, grad, touched, "kge_sparse_adam");
+  for (const Tensor* t : {&m, &v})
+    TORCH_CHECK(on_dev(*t) && t->scalar_type() == torch::kFloat32 && t->is_contiguous() && aligned16(*t) &&
+                t->sizes() == w.sizes(), "kge_sparse_adam: m and v must be contiguous fp32 tensors of w's shape");
+  check_counters(step, 0, "kge_sparse_adam: step must be int32 [>= 1] on the device");
+  TORCH_CHECK(lr > 0 && b1 >= 0 && b1 < 1 && b2 >= 0 && b2 < 1 && eps > 0,
+              "kge_sparse_adam: need lr > 0, 0 <= betas < 1 and eps > 0");
+  launch_sparse_adam(w.data_ptr<float>(), grad.data_ptr<float>(), m.data_ptr<float>(), v.data_ptr<float>(),
+                     touched.data_ptr<uint8_t>(), w.size(0), static_cast<int>(w.size(1)), step.data_ptr<int32_t>(),
+                     static_cast<float>(lr), static_cast<float>(b1), static_cast<float>(b2), static_cast<float>(eps),
+                     cur_stream());
+  check_cuda_err("kge_sparse_adam");
+}
+
+// ---------------------------------------------------------------------------
 // SealArena: the static per-link arena and parameter layout of SealEngine's step (cuda/seal.cu).
 // ---------------------------------------------------------------------------
 struct SealArena {
@@ -2803,6 +2985,17 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("sparse_adam", &sparse_adam, py::arg("metapath"), py::arg("emb"), py::arg("grad"), py::arg("m"), py::arg("v"),
         py::arg("touched"), py::arg("step"), py::arg("lr"), py::arg("b1"), py::arg("b2"), py::arg("eps"));
   m.def("m2v_begin", &m2v_begin, py::arg("state"));
+  m.def("kge_negatives", &kge_negatives, py::arg("count"), py::arg("batch_size"), py::arg("num_neg"), py::arg("N"),
+        py::arg("seed"), py::arg("step"), py::arg("neg"));
+  m.def("kge_loss_grad", &kge_loss_grad, py::arg("model"), py::arg("trip"), py::arg("count"), py::arg("neg"),
+        py::arg("ent"), py::arg("rel"), py::arg("margin"), py::arg("p"), py::arg("grad_ent"), py::arg("grad_rel"),
+        py::arg("touched_ent"), py::arg("touched_rel"), py::arg("loss"));
+  m.def("kge_score", &kge_score, py::arg("model"), py::arg("ent"), py::arg("rel"), py::arg("h"), py::arg("r"),
+        py::arg("t"), py::arg("margin"), py::arg("p"));
+  m.def("kge_rank", &kge_rank, py::arg("model"), py::arg("ent"), py::arg("rel"), py::arg("h"), py::arg("r"),
+        py::arg("t"), py::arg("tail"), py::arg("keys"), py::arg("margin"), py::arg("p"), py::arg("splits") = 0);
+  m.def("kge_sparse_adam", &kge_sparse_adam, py::arg("w"), py::arg("grad"), py::arg("m"), py::arg("v"),
+        py::arg("touched"), py::arg("step"), py::arg("lr"), py::arg("b1"), py::arg("b2"), py::arg("eps"));
   m.def("dropout_bf16", &dropout_bf16, py::arg("Z"), py::arg("counters"), py::arg("n_hops"), py::arg("p"),
         py::arg("seed"), py::arg("layer"), py::arg("step_dev") = py::none());
   m.def("zero_grads", &zero_grads);

@@ -794,6 +794,44 @@ size_t link_topk_smem_bytes(int d, int k, int stages);
 int link_topk_ctas_per_sm(int d, int k, int stages);
 void launch_link_topk(const LinkTopkLaunch& L, cudaStream_t s);
 
+// ---- kge.cu (knowledge-graph embeddings: TransE, DistMult, ComplEx, RotatE) -------------------------------------------
+// Entity rows are fp32 [D] or [re | im] (2D: ComplEx, RotatE); relation rows [D] (RotatE: the phase) or [re | im]
+// (ComplEx).  D is a multiple of 8 in [8, 512].  p (1 or 2) is TransE's norm; margin is RotatE's score offset and the
+// margin of the TransE / DistMult ranking loss.
+enum KgeModel { kKgeTransE = 0, kKgeDistMult = 1, kKgeComplEx = 2, kKgeRotatE = 3 };
+int kge_entity_parts(int model);
+int kge_relation_parts(int model);
+// neg[i * K + j] for i < min(*n_dev, B): uniform in [0, N), Philox(seed, step, i, j).  Slots past n are not written.
+void launch_kge_negatives(const int32_t* n_dev, int B, int K, int64_t N, uint64_t seed, const int32_t* step_dev,
+                          int64_t* neg, cudaStream_t s);
+// trip int64 [3, B] (head, relation, tail rows); the first min(*n_dev, B) columns are the positives.  Positive i
+// corrupts its head (i < n / 2) or tail with neg[i * K + j].  Writes the loss to *loss, red.adds the gradients into
+// gent / grel and sets tent / trel for every row looked up.
+void launch_kge_loss_grad(int model, const int64_t* trip, int B, const int32_t* n_dev, const int64_t* neg, int K,
+                          const float* ent, const float* rel, int64_t N, int64_t R, int D, float margin, int p,
+                          float* gent, float* grel, uint8_t* tent, uint8_t* trel, float* loss, cudaStream_t s);
+// out[i] = score(h[i], r[i], t[i]), ids in range.
+void launch_kge_score(int model, const int64_t* h, const int64_t* r, const int64_t* t, int64_t n, const float* ent,
+                      const float* rel, int D, float margin, int p, float* out, cudaStream_t s);
+// counts[i] = (#candidates scoring above the true entity << 32) + #candidates tied with it, over every entity except
+// the true one and the ids of the query's filter range.  tail: query (h, r, ?) with truth t, else (?, r, t) with
+// truth h.  keys (sorted int64, may be null): (f R + r) N + c with f the query's fixed entity.
+struct KgeRankArgs {
+  int model, D, p;
+  float margin;
+  bool tail;
+  const int64_t *h, *r, *t;     // [n], ids in range
+  int64_t n, N, R;
+  const float *ent, *rel;
+  const int64_t* keys;
+  int64_t n_keys;
+  float* den;                   // scratch [N] (TransE)
+  float* q;                     // scratch [n, entity width]
+  unsigned long long* counts;   // [n]
+  int splits, tiles_per_split;  // candidate tiles of 64 ids per split
+};
+void launch_kge_rank(const KgeRankArgs& a, cudaStream_t s);
+
 // programmatic-dependent-launch switch (launch_utils.h); returns the previous value
 int set_pdl(int on);
 void launch_tc_gemm(const TcGemmLaunch& L, int num_sms, cudaStream_t s);

@@ -12,3 +12,4 @@ from .metapath2vec import MetaPath2VecEngine
 from .seal_engine import SealEngine
 from .label_prop import LabelPropagation, CorrectAndSmooth
 from .link_rank import link_topk, link_scores, link_recall_at_k, link_hits_at_k, link_mrr
+from .kge import KgeEngine, kge_filter

@@ -148,3 +148,30 @@ def rmat_csr_shard(num_nodes: int, num_edges: int, row_begin: int, row_end: int,
     torch.cumsum(torch.bincount(rows, minlength=n_rows), 0, out=indptr[1:])
   return {'indptr': indptr, 'indices': indices.contiguous(), 'eids': None, 'weights': None,
           'row_begin': int(row_begin), 'row_end': int(row_end)}
+
+
+def synthetic_kg(num_nodes: int, num_relations: int, num_triples: int,
+                 seed: int = 0) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+  """A seeded knowledge graph with planted structure: (train, valid, test) int64 [3, m] (head, relation, tail).
+
+  Entity e belongs to cluster e // 8 of C = num_nodes // 8 clusters in a chain; relation r links
+  cluster c to cluster c + r + 1 (when it exists), so a triple's tail cluster is a translation of its head cluster.
+  TransE, ComplEx and RotatE can represent this exactly; DistMult only up to its symmetry in head and tail.  Triples
+  draw r, then a head cluster with a successor, then a uniform head and tail inside the two clusters; duplicates are
+  dropped, and the distinct triples are split 80 / 10 / 10 in a seeded order.  Needs C >= num_relations + 1."""
+  N, R, M, S = int(num_nodes), int(num_relations), int(num_triples), 8
+  C = N // S
+  if R < 1 or M < 1 or C < R + 1:
+    raise ValueError(f'synthetic_kg needs num_relations, num_triples >= 1 and num_nodes // 8 >= '
+                     f'num_relations + 1 (got N={N}, R={R}, triples={M})')
+  g = torch.Generator().manual_seed(int(seed))
+  r = torch.randint(0, R, (M,), generator=g)
+  span = C - r - 1                                   # head clusters with a successor at distance r + 1
+  c = (torch.rand(M, generator=g) * span).long().clamp_max(span - 1)
+  h = c * S + torch.randint(0, S, (M,), generator=g)
+  t = (c + r + 1) * S + torch.randint(0, S, (M,), generator=g)
+  trip = torch.unique(torch.stack([h, r, t]), dim=1)
+  trip = trip[:, torch.randperm(trip.size(1), generator=g)]
+  m = trip.size(1)
+  a, b = int(0.8 * m), int(0.9 * m)
+  return trip[:, :a].contiguous(), trip[:, a:b].contiguous(), trip[:, b:].contiguous()
